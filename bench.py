@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py — rays/s (training) and fps (inference) of the Instant-NGP hot path on B200 (driver contract: task statement).
+"""bench.py — rays/s (training) and fps (inference) of the Instant-NGP hot path on one or more H100s.
 
-    python bench.py --gpus N --steps K --warmup W [--config NAME]     # this repository (CUDA, sm_100a)
+    python bench.py --gpus N --steps K --warmup W [--config NAME]     # this repository (CUDA, sm_90a)
+    python bench.py ... --dump-outputs DIR     # also write what the last timed step computed, DIR/<name>.npy
     python bench.py --impl reference --gpus N --steps K ... [--config NAME]   # reference restatement on host cores
 
 A training "step" = one pass of the hot path over one batch of synthetic rays:
@@ -77,7 +78,7 @@ def measured_peaks():
             d = json.load(f)
         return (float(d["hbm_gbs"]), float(d.get("bf16_tflops_sustained", d.get("bf16_tflops", 1418.0))),
                 "measured (MEASURED_PEAKS.json: HBM copy GB/s, sustained dense bf16 TFLOP/s)")
-    return 6650.0, 1418.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, 989.0, "fallback (H100 SXM data sheet: HBM3 GB/s, dense bf16 TFLOP/s)"
 
 
 def ncu_traffic(config, kernel, samples):
@@ -100,9 +101,34 @@ def ncu_traffic(config, kernel, samples):
     return d["kernels"][kernel]["dram_bytes"], src
 
 
+DUMP_BYTES = 64 << 20         # --dump-outputs: at most this many bytes in all
+DUMP_SAMPLE = 1 << 21         # larger arrays: this many elements at fixed, seeded positions
+
+
+def dump_outputs(out_dir, arrays):
+    """Write each array as out_dir/<name>.npy (float64 if it was float64, else float32).  An array of more than
+    DUMP_SAMPLE elements is replaced by the elements at DUMP_SAMPLE fixed positions (seeded, sorted, the same in every
+    run), so that two builds given the same arguments can be compared output for output."""
+    os.makedirs(out_dir, exist_ok=True)
+    total = 0
+    for name, a in arrays.items():
+        if hasattr(a, "detach"):
+            a = a.detach().cpu().numpy()
+        a = np.asarray(a)
+        a = a.astype(np.float64 if a.dtype == np.float64 else np.float32)
+        if a.size > DUMP_SAMPLE:
+            idx = np.sort(np.random.default_rng(SEED).choice(a.size, DUMP_SAMPLE, replace=False))
+            a = a.reshape(-1)[idx]
+            name += "_sample"
+        total += a.nbytes
+        if total > DUMP_BYTES:
+            raise ValueError(f"--dump-outputs: more than {DUMP_BYTES} bytes")
+        np.save(os.path.join(out_dir, name + ".npy"), a)
+
+
 # --------------------------------------------------------------------------------------------------
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
     Q = ("clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -361,11 +387,19 @@ def run_train(args, cfg_name, cfg):
     launches0 = _lib.launch_count()
     graph0 = fast.graph_kernel_launches
 
+    last = {}
+
     def timed_steps():
         for k in range(args.steps):
-            step_fn(args.warmup + k, args.warmup + k)
+            last["loss"] = step_fn(args.warmup + k, args.warmup + k)
         fast.flush()   # every one of the K updates is applied inside the timed region
     ms_total = timed(timed_steps)
+    if args.dump_outputs and rank == 0:
+        # what a caller of the step receives: the loss, the sample count and the updated parameters (hash table +
+        # MLP, fp32 master copy)
+        dump_outputs(args.dump_outputs, {"loss": last["loss"].float().reshape(1),
+                                         "samples": sample_counts[-1].reshape(1),
+                                         "params": trainer.flat_param})
     trainer.p2p_check()   # (several ranks) no peer barrier gave up waiting
     clock_info = clocks.stop() if rank == 0 else None
     launches = _lib.launch_count() - launches0            # eager launches of libngp_b200 kernels
@@ -437,7 +471,7 @@ def run_train(args, cfg_name, cfg):
                        "peer-memory optimizer step: NVLink P2P reduce-scatter + Adam on the owned 1/N + fp16 all-gather "
                        "in ONE kernel per rank (csrc/p2p.cu), no NCCL in the step" if trainer.p2p is not None else
                        "1 NCCL all-reduce/step"),
-                   "l2": "no flush: per-step working set (~%d MB of per-sample tensors) exceeds the 126 MB L2; "
+                   "l2": "no flush: per-step working set (~%d MB of per-sample tensors) exceeds the 50 MB L2; "
                          "new rays every step" % int(spr * BATCH * (2010 if half else 2872) / 1e6),
                    "density_grid_update": f"inside timed loop every {UPDATE_INTERVAL} steps (warm-up mode); "
                                           f"{upd_ms:.3f} ms each",
@@ -481,7 +515,7 @@ def kernel_roofline(torch, cfg_name, cfg, fast, trainer, dev, ms_step):
     def t(fn, reps=5):
         out = []
         for _ in range(reps):
-            flush.fill_(1)                      # evict L2 (126 MB) between repeats
+            flush.fill_(1)                      # evict L2 (50 MB) between repeats
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             torch.cuda.synchronize()
             e0.record()
@@ -534,10 +568,9 @@ def kernel_roofline(torch, cfg_name, cfg, fast, trainer, dev, ms_step):
            "algorithmic_bytes_per_sample": BYTES_PER_SAMPLE.get(top, (None, None))[col],
            "kernel_ms": times, "kernels": kernels,
            "sum_kernel_ms": sum(times.values()), "ms_per_step": ms_step,
-           "note": "fp16 table (21.8 MiB) + fp32 grad (43.6 MiB) fit the 126 MB L2: the hash gathers / atomics never "
-                   "reach HBM, their limiter is the SM's L1TEX/LSU wavefront rate (one 128-B line per cycle per SM for "
-                   "divergent loads, ~1.3 cycles per lane for scattered RED) — DESIGN.md §4; algorithmic GB/s over the "
-                   "HBM peak is what the contract asks for and can exceed the DRAM traffic by 10x"}
+           "note": "fp16 table (21.8 MiB) + fp32 grad (43.6 MiB) together exceed the 50 MB L2 of an H100; how much of the "
+                   "hash gathers / atomics reach DRAM, and what limits those kernels, has not been measured on the H100 "
+                   "(DESIGN.md §4): algorithmic GB/s over the HBM peak is not a DRAM utilisation for them"}
     return out
 
 
@@ -616,8 +649,15 @@ def run_frame(args, cfg_name, cfg):
         res = frame(pose)
         k += 1
     launches0 = _lib.launch_count()
-    ms = timed(lambda: [frame(pose) for _ in range(args.steps)]) / args.steps
+    last = {}
+
+    def timed_frames():
+        for _ in range(args.steps):
+            last["res"] = frame(pose)
+    ms = timed(timed_frames) / args.steps
     launches = _lib.launch_count() - launches0
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, {k: last["res"][k] for k in ("rgb", "depth", "opacity")})
     clock_info = clocks.stop()
     total_samples = int(res["total_samples"])
     fr = next(iter(model.__dict__.get("_frame_renderers", {}).values()), None)
@@ -648,7 +688,7 @@ def run_frame(args, cfg_name, cfg):
         "vs_baseline": None, "dtype": "f16", "data": "synthetic",
         "config": {"workload": cfg["workload"], "name": cfg_name, "rays": w * h, "samples_evaluated": total_samples,
                    "samples_per_ray": total_samples / (w * h), "psnr_vs_teacher_frame": psnr_teacher,
-                   "l2": "no flush: one frame touches ~%d MB of per-sample tensors (> 126 MB L2)"
+                   "l2": "no flush: one frame touches ~%d MB of per-sample tensors (> 50 MB L2)"
                          % int(total_samples * 692 / 1e6), **info},
         "e2e": {"value": 1e3 / ms_e2e, "unit": "frames/s", "h2d_bytes_per_step": 48, "d2h_bytes_per_step": w * h * 12,
                 "ms_per_step": ms_e2e,
@@ -895,7 +935,9 @@ def run_reference(args, cfg_name, cfg):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=40)
+    ap.add_argument("--steps", type=int, default=40,
+                    help="timed steps (frames) of the CUDA arms; --impl reference caps them by --ref-budget and reports "
+                         "steps_requested beside the steps it ran")
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--config", default="lego_half", choices=sorted(CONFIGS),
@@ -917,6 +959,9 @@ def main():
     ap.add_argument("--ncu-window", type=int, default=0,
                     help="profiling aid: wrap this many extra steps in cudaProfilerStart/Stop "
                          "(use with `ncu --profile-from-start off`); numbers printed under ncu are not bench values")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last one computed as DIR/<name>.npy (float32/64, "
+                         "large arrays as a fixed seeded sample; at most 64 MB)")
     args = ap.parse_args()
     if args.warmup < 3 and args.impl == "ours":
         args.warmup = 3

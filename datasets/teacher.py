@@ -2,8 +2,8 @@
 
 No NeRF dataset exists offline (SURVEY.md §8c), so "PSNR vs ref" is measured against a teacher: the only trained
 artefact the reference ships — its mobile-demo Lego model (deployment/InstantNGP/taichi_ngp/compiled/*.bin: L=4 F=4
-dense grid, 16-wide MLPs, occupancy bitfield), staged git-ignored under oracle/_ref/lego_deployment by
-``__graft_entry__.build()``.  The teacher is loaded with ``modules.utils.load_deployment_model`` and rendered with the
+dense grid, 16-wide MLPs, occupancy bitfield), rebuilt git-ignored under oracle/_ref/lego_deployment from
+tests/golden/ by ``__graft_entry__.build()``.  The teacher is loaded with ``modules.utils.load_deployment_model`` and rendered with the
 CUDA path (``render(test_time=True)``, T_threshold 1e-2 as the demo uses, white background); the images then play
 the role of datasets/nsvf.py's ``self.rays`` (train split) / per-view ``rgb`` (test split), with the Synthetic-NeRF
 Lego intrinsics (datasets/nsvf.py:37-44) and cameras on the upper hemisphere at the shipped pose's radius (1.396).
@@ -71,8 +71,8 @@ class TeacherLego(SyntheticLego):
             dev = self.poses.device
             teacher = teacher if teacher is not None else load_teacher(dev)
             if teacher is None:
-                raise FileNotFoundError("teacher model not staged: run __graft_entry__.build() where /root/reference "
-                                        "exists, or set NGP_TEACHER_DIR to a folder with the six .bin files")
+                raise FileNotFoundError("teacher model not staged: run __graft_entry__.build(), "
+                                        "or set NGP_TEACHER_DIR to a folder with the six .bin files")
             self.images = render_views(teacher, self.directions, self.poses)
         self.rays = self.images
         return self.rays

@@ -1,5 +1,5 @@
 /*
- * ngp_b200.h — C-ABI of the B200-native Instant-NGP hot path.
+ * ngp_b200.h — C-ABI of the Instant-NGP hot path for the H100 (sm_90a).
  *
  * This header is the drop-in boundary.  Every entry point replaces one Taichi
  * kernel (or one torch op sequence) of taichi-dev/taichi-nerfs; the reference
@@ -215,21 +215,10 @@ int ngp_dir_encode(const float* dirs, float* out, int64_t n, void* stream);
  *   -> sigmas [n] fp32, rgbs [n,3] fp16, h [n,16] fp16 (geometry feature)
  * With `save` != NULL (ngp_mlp_save_bytes(n) = 40 n bytes, 16-byte aligned) the forward also stores what
  * torch.autograd would keep for the backward and is cheap to keep: h [n,16] fp16 and the fp16 sigmoid output
- * [n,4]; the backward given the same `save` then restarts from h (8 MMA rounds per tile instead of 10) and
+ * [n,4]; the backward given the same `save` then restarts from h (layers 2 and 5 are not recomputed) and
  * forms sigmoid' from the saved output exactly as torch's sigmoid_backward does.  save == NULL: the backward
  * recomputes everything from (emb, dirs). */
 int64_t ngp_mlp_save_bytes(int64_t n);
-/* Selects the forward implementation for fp16 embeddings: 0 = auto (v2 where it applies), 1 = v1 (activations
- * in shared memory, mlp.cu), 2 = v2 (TMA-fed, activations in tensor memory, mlp_fwd_v2.cu; an error instead of a
- * silent fall-back when it cannot run).  Same results bit for bit; exists for A/B timing and the parity tests.
- * The environment variable NGP_MLP_FWD overrides the argument. */
-int ngp_mlp_set_impl(int fwd_impl);
-/* The same switch for the backward with fp16 embeddings and saved activations: 0 = auto (v2), 1 = v1 (one tile per CTA,
- * CTA-wide barrier per round, MMAs issued by one thread), 2 = v2 (three tile slots per persistent CTA, per-slot
- * mbarriers, MMAs issued by converged warps with descriptors from constant memory, weight-gradient MMAs on their own
- * warp).  Same MMAs and epilogues, results equal up to the order of the fp32 weight-gradient sums.  The environment
- * variable NGP_MLP_BWD overrides the argument. */
-int ngp_mlp_set_bwd_impl(int bwd_impl);
 int ngp_mlp_fwd(const void* emb, int emb_dtype, const float* dirs, const ngp_mlp_weights* w,
                 float* sigmas, void* rgbs_f16, void* save, int64_t n, void* stream);
 /* backward: dsigmas [n] fp32, drgbs [n,3] fp16 -> demb [n,32] (emb dtype) and

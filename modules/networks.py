@@ -102,7 +102,7 @@ class NGP(nn.Module):
 
     # -- network ----------------------------------------------------------------------------------
     def _fusable(self, x):
-        """True when the stock architecture is in use, so the fused sm_100a MLP kernel applies."""
+        """True when the stock architecture is in use, so the fused sm_90a MLP kernel applies."""
         return (x.is_cuda and _fused_mlp_available()
                 and self.pos_encoder.out_dim == 32
                 and self.xyz_encoder.net_depth == 1 and self.xyz_encoder.net_width == 64

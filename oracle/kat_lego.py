@@ -6,9 +6,13 @@ occupancy bitfield, pose, pixel directions).  Rendering it end to end with the o
 ray/AABB -> march -> dense hash indexing -> SH -> MLP weight layout -> compositing
 (restating deployment/InstantNGP/taichi_ngp/kernels.py:262-571 and new_kernels.py:4-18) must produce
 the yellow Lego bulldozer; any indexing / layout mistake produces noise.  This pins the oracle against
-the reference's own artefact (test infrastructure; needs /root/reference, i.e. the build container).
+the reference's own artefact (test infrastructure).  The model is stored shrunk under tests/golden/
+(lego_deployment.npz + lego_table_level3.npz, made by tests/golden/make_golden.py: the hash-table entries a render
+through the occupancy grid can read, in fp16); stage() rebuilds the six .bin files from it under oracle/_ref/.
 
-    python -m oracle.kat_lego            # writes tests/golden/lego_kat.png + lego_kat_stats.json
+    NGP_REFERENCE=<taichi-nerfs checkout> python -m oracle.kat_lego
+        # writes tests/golden/lego_kat.png + lego_kat_stats.json from the reference's ORIGINAL .bin files; it refuses
+        # to run without them, so the golden image is never re-derived from the shrunk copy
 """
 from __future__ import annotations
 
@@ -20,7 +24,42 @@ import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
-REF_DIR = "/root/reference/deployment/InstantNGP/taichi_ngp/compiled"
+GOLDEN = os.path.join(ROOT, "tests", "golden")
+REF_DIR = os.path.join(ROOT, "oracle", "_ref", "lego_deployment")   # git-ignored, rebuilt by stage()
+FILES = ("hash_embedding", "sigma_weights", "rgb_weights", "density_bitfield", "pose", "directions")
+TABLE_ENTRIES, TABLE_FEATURES = 2794024, 4     # make_hash_layout(2 ** 21, 4, 32, 128, 4)
+
+
+def _write_bin(path, code, a):
+    """[int32 dtype code][int32 numel][payload]; written to a temporary name first so a reader never sees half."""
+    tmp = f"{path}.{os.getpid()}.tmp"
+    with open(tmp, "wb") as f:
+        f.write(np.array([code, a.size], np.int32).tobytes())
+        f.write(np.ascontiguousarray(a).tobytes())
+    os.replace(tmp, path)
+
+
+def stage(dest=REF_DIR):
+    """Rebuild the six deployment .bin files of the shipped Lego model in `dest` from the golden data (once);
+    hash-table entries outside the stored set are zero.  Returns `dest`."""
+    if all(os.path.exists(os.path.join(dest, n + ".bin")) for n in FILES):
+        return dest
+    os.makedirs(dest, exist_ok=True)
+    g = np.load(os.path.join(GOLDEN, "lego_deployment.npz"))
+    fine = np.load(os.path.join(GOLDEN, "lego_table_level3.npz"))["table_fine"]
+    mask = np.unpackbits(g["table_mask"])[:TABLE_ENTRIES].astype(bool)
+    table = np.zeros((TABLE_ENTRIES, TABLE_FEATURES), np.float32)
+    table[mask] = np.concatenate([g["table_coarse"], fine]).astype(np.float32)   # entries in index order
+    dx, dy = g["dir_x"], g["dir_y"]
+    dirs = np.stack(np.broadcast_arrays(dx[None, :], dy[:, None], np.float32(1)), -1).astype(np.float32)
+    bits = np.load(os.path.join(GOLDEN, "lego_bitfield.npz"))["bitfield"]
+    _write_bin(os.path.join(dest, "hash_embedding.bin"), 0, table.reshape(-1))
+    _write_bin(os.path.join(dest, "sigma_weights.bin"), 0, g["sigma_weights"].astype(np.float32))
+    _write_bin(os.path.join(dest, "rgb_weights.bin"), 0, g["rgb_weights"].astype(np.float32))
+    _write_bin(os.path.join(dest, "density_bitfield.bin"), 4, bits.view(np.uint32))
+    _write_bin(os.path.join(dest, "pose.bin"), 0, g["pose"].astype(np.float32))
+    _write_bin(os.path.join(dest, "directions.bin"), 0, dirs.reshape(-1))
+    return dest
 
 
 def read_bin(path):
@@ -52,16 +91,18 @@ def deployment_mlp(emb, dirs, sigma_w, rgb_w):
     return sigma.astype(np.float32), (1 / (1 + np.exp(-o))).astype(np.float32)
 
 
-def render(step=2, T_threshold=1e-2, max_samples=1024):
+def render(step=2, T_threshold=1e-2, max_samples=1024, src=None):
+    """Render the shipped view from the six .bin files in `src` (default: the copy stage() rebuilds)."""
     sys.path.insert(0, ROOT)
+    src = src or stage()
     from oracle import oracle as O
     from taichi_nerfs_b200.layout import make_hash_layout
-    emb_table = read_bin(os.path.join(REF_DIR, "hash_embedding.bin"))
-    sigma_w = read_bin(os.path.join(REF_DIR, "sigma_weights.bin"))
-    rgb_w = read_bin(os.path.join(REF_DIR, "rgb_weights.bin"))
-    bits = read_bin(os.path.join(REF_DIR, "density_bitfield.bin")).view(np.uint8)
-    pose = read_bin(os.path.join(REF_DIR, "pose.bin")).reshape(3, 4)
-    directions = read_bin(os.path.join(REF_DIR, "directions.bin")).reshape(600, 300, 3)  # (h, w) row-major
+    emb_table = read_bin(os.path.join(src, "hash_embedding.bin"))
+    sigma_w = read_bin(os.path.join(src, "sigma_weights.bin"))
+    rgb_w = read_bin(os.path.join(src, "rgb_weights.bin"))
+    bits = read_bin(os.path.join(src, "density_bitfield.bin")).view(np.uint8)
+    pose = read_bin(os.path.join(src, "pose.bin")).reshape(3, 4)
+    directions = read_bin(os.path.join(src, "directions.bin")).reshape(600, 300, 3)  # (h, w) row-major
     lay = make_hash_layout(2 ** 21, 4, 32, 128, 4)
     assert lay.total_param_size == emb_table.size
 
@@ -88,7 +129,10 @@ def stats(rgb, opacity, spr):
 
 
 def main():
-    rgb, opacity, spr, _ = render()
+    src = os.path.join(os.environ.get("NGP_REFERENCE", ""), "deployment", "InstantNGP", "taichi_ngp", "compiled")
+    if not os.environ.get("NGP_REFERENCE") or not all(os.path.exists(os.path.join(src, n + ".bin")) for n in FILES):
+        sys.exit("set NGP_REFERENCE to a taichi-nerfs checkout: the golden image is made from the original model files")
+    rgb, opacity, spr, _ = render(src=src)
     st = stats(rgb, opacity, spr)
     out = os.path.join(ROOT, "tests", "golden")
     from PIL import Image

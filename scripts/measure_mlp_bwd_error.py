@@ -1,4 +1,4 @@
-"""Measured error of the tcgen05 MLP backward against the oracle (per gradient block), to set the test tolerances."""
+"""Measured error of the fused MLP backward against the oracle (per gradient block), to set the test tolerances."""
 import os
 import sys
 

@@ -1,4 +1,4 @@
-"""Kernel-time breakdown of the training step (torch.profiler, CUDA activities) — run on the GPU box."""
+"""Kernel-time breakdown of the training step (torch.profiler, CUDA activities) — run on the GPU."""
 import os
 import sys
 

@@ -1,7 +1,7 @@
 """Real (concurrent, warm) GPU timeline of the graph-captured training step: kernel start / end stamps from CUPTI via
 torch.profiler, for a few steady-state replays.  Prints, per step: the span (first kernel start -> last kernel end), the
 summed kernel time on the critical stream, the gaps between consecutive kernels, and the overlap of the optimizer branch
-with the marching branch.  Run on the GPU box:  python scripts/step_timeline.py [out.txt]"""
+with the marching branch.  Run on the GPU:  python scripts/step_timeline.py [out.txt]"""
 import json
 import os
 import sys

@@ -1,4 +1,4 @@
-"""Isolated timing of the tcgen05 MLP kernels (CUDA events, L2 flushed between repeats): forward with / without the
+"""Isolated timing of the fused MLP kernels (CUDA events, L2 flushed between repeats): forward with / without the
 save buffer, backward restarting from the saved activations vs recomputing everything."""
 import os
 import statistics
@@ -34,31 +34,13 @@ def t(fn, reps=7):
     return statistics.median(out)
 
 
-from taichi_nerfs_b200 import _lib
-
-for impl, tag in ((1, "v1 smem"), (2, "v2 tmem")):
-    _lib.load().ngp_mlp_set_impl(impl)
-    for name, fn in [("fwd", lambda: ops.mlp_fwd(emb, dirs, ws)), ("fwd+save", lambda: ops.mlp_fwd(emb, dirs, ws, with_save=True))]:
-        try:
-            fn()
-            us = t(fn) * 1e3
-            print(f"{name + ' ' + tag:22s} {us:8.1f} us   (n = {n}; {18816 * n / us / 1e6:6.1f} TFLOP/s, "
-                  f"{(86 + (40 if 'save' in name else 0)) * n / us / 1e3:6.0f} GB/s algorithmic)", flush=True)
-        except Exception as e:  # noqa: BLE001
-            print(f"{name} {tag}: FAILED {e}", flush=True)
-_lib.load().ngp_mlp_set_impl(0)
-outs = {}
-for bwd_impl, tag in ((1, "v1 (1 tile / CTA)"), (2, "v2 (3 slots / CTA)")):
-    _lib.load().ngp_mlp_set_bwd_impl(bwd_impl)
-    for name, fn in [
-                     ("bwd recompute", lambda: ops.mlp_bwd(emb, dirs, ws, dsig, drgb)),
-                     ("bwd saved", lambda: ops.mlp_bwd(emb, dirs, ws, dsig, drgb, save=save))]:
-        if bwd_impl == 2 and name == "bwd recompute":
-            continue    # v2 exists for the saved-activation path only
-        outs[(name, bwd_impl)] = fn()
-        us = t(fn) * 1e3
-        print(f"{name + ' ' + tag:34s} {us:8.1f} us   (n = {n}; {37632 * n / us / 1e6:6.1f} TFLOP/s)", flush=True)
-_lib.load().ngp_mlp_set_bwd_impl(0)
-a, b = outs[("bwd saved", 1)], outs[("bwd saved", 2)]
-print("v2 vs v1: d_emb bit-equal:", bool(torch.equal(a[0], b[0])), " max |dW| diff / max |dW|:",
-      float((a[1] - b[1]).abs().max() / a[1].abs().max()))
+for name, fn in [("fwd", lambda: ops.mlp_fwd(emb, dirs, ws)), ("fwd+save", lambda: ops.mlp_fwd(emb, dirs, ws, with_save=True))]:
+    fn()
+    us = t(fn) * 1e3
+    print(f"{name:22s} {us:8.1f} us   (n = {n}; {18816 * n / us / 1e6:6.1f} TFLOP/s, "
+          f"{(86 + (40 if 'save' in name else 0)) * n / us / 1e3:6.0f} GB/s algorithmic)", flush=True)
+for name, fn in [("bwd recompute", lambda: ops.mlp_bwd(emb, dirs, ws, dsig, drgb)),
+                 ("bwd saved", lambda: ops.mlp_bwd(emb, dirs, ws, dsig, drgb, save=save))]:
+    fn()
+    us = t(fn) * 1e3
+    print(f"{name:34s} {us:8.1f} us   (n = {n}; {37632 * n / us / 1e6:6.1f} TFLOP/s)", flush=True)

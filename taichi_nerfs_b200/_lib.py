@@ -58,8 +58,6 @@ def _declare(lib):
         "ngp_mse_loss_grad": (ci, [vp, vp, vp, f32, f32, vp, vp, vp, i64, vp]),
         "ngp_dir_encode": (ci, [vp, vp, i64, vp]),
         "ngp_mlp_save_bytes": (i64, [i64]),
-        "ngp_mlp_set_impl": (ci, [ci]),
-        "ngp_mlp_set_bwd_impl": (ci, [ci]),
         "ngp_mlp_fwd": (ci, [vp, ci, vp, mw, vp, vp, vp, i64, vp]),
         "ngp_mlp_bwd": (ci, [vp, ci, vp, mw, vp, vp, vp, vp, vp, i64, vp]),
         "ngp_composite_train_fwd": (ci, [vp, vp, ci, vp, vp, vp, f32, vp, vp, vp, vp, vp, i64, i64, vp]),

@@ -4,7 +4,7 @@
 // (fp16 table, fp16 accumulate) of the reference.  Per-level scale/resolution come from the
 // host-built ngp_hash_layout (see include/ngp_b200.h) instead of a per-thread expf.
 //
-// B200 mapping.  The reference launches one thread per (sample, level) with the level as the
+// GPU mapping.  The reference launches one thread per (sample, level) with the level as the
 // fastest index and block_dim=16, so a warp touches 2 samples x 16 unrelated table regions and
 // every thread pays 8 integer modulos.  Here a CTA owns 512 consecutive samples (xyz staged once in
 // shared memory), WARP w handles LEVEL w and each lane walks a chunk of 16 consecutive samples.
@@ -12,8 +12,8 @@
 // 8 corners only when the cell changes (37x fewer loads at level 0, ~1x at the finest levels),
 // (b) the backward accumulates w*dy in registers and issues its 8 vector atomics only at cell
 // changes, and (c) all lanes of a warp stay inside one level's table slab (L1/L2 locality).
-// The fp16 table (21.8 MiB) and the fp32 gradient (43.6 MiB) both fit B200's 126 MB L2, so these
-// kernels are L2-gather / L2-atomic bound, not HBM bound.  Results are staged in shared memory
+// The fp16 table (21.8 MiB) and the fp32 gradient (43.6 MiB) together exceed the H100's 50 MB L2; how much of
+// the gathers and atomics L2 serves has not been measured on the H100.  Results are staged in shared memory
 // ([level][sample], chunk stride 17 words = conflict-free) and written with coalesced stores in
 // the reference's [n, L*F] row-major layout.
 #include "common.cuh"

@@ -4,7 +4,7 @@
 // device helpers modules/utils.py:54-117 of the reference, in strict fp32 source order (every
 // op an explicit *_rn intrinsic) so that sample positions are bit-identical to the CPU oracle.
 //
-// B200 notes: these kernels are latency-bound integer/fp32 work over a 256 KiB..1.5 MiB
+// GPU notes: these kernels are latency-bound integer/fp32 work over a 256 KiB..1.5 MiB
 // bitfield that lives in L1/L2 — there is nothing for tensor cores here.  Training march is
 // count -> single-CTA scan -> write, giving a deterministic, ray-ordered sample layout without
 // the global atomics (ray_march.py:76-81) or the n_rays*1024-row scratch (ray_march.py:149-168).

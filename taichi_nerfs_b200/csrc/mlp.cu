@@ -1,6 +1,5 @@
-// mlp.cu — the fused NGP MLP (sigma net 32->64->16, SH, rgb net 32->64->64->3) on the
-// 5th-generation tensor cores: tcgen05.mma with operands in shared memory and fp32 accumulators
-// in tensor memory (TMEM), one 128-sample tile per CTA iteration.
+// mlp.cu — the fused NGP MLP (sigma net 32->64->16, SH, rgb net 32->64->64->3) on the Hopper warpgroup tensor
+// cores: wgmma.mma_async with fp32 accumulators in registers, one 64-sample tile per warpgroup (CTA) iteration.
 //
 // Replaces, in the reference, five torch.nn.Linear (cuBLAS) calls under torch.autocast(fp16) plus
 // ~10 elementwise/cat/cast kernels: modules/networks.py:136-166 (NGP.density/forward), :369-380
@@ -8,380 +7,277 @@
 // rgb-net input stage).  Numerics follow autocast: fp16 operands, fp32 accumulate, every layer
 // output rounded to fp16, TruncExp / direction normalisation / SH in fp32.
 //
-// Data layout.  All MMA operands live in shared memory in the canonical UMMA *no-swizzle*
-// ("interleaved") layout: 8x8 fp16 core matrices of 128 contiguous bytes (row stride 16 B);
-// core matrices adjacent along K are LBO = 128 B apart, 8-row groups are SBO = (K/8)*128 B apart.
-// A thread owns one sample row, so an epilogue writes 16-byte chunks that are bank-conflict free
-// per quarter warp, and the same buffer can later be consumed K-major (forward) or MN-major
-// (weight gradients) by swapping LBO/SBO.  Weights (9,408 fp16 = 18.4 KB, W5 zero-padded to 16
-// rows) stay resident in shared memory for the lifetime of the persistent CTA.
-//
-// Roofline: tensor pipe for the MMAs (18,816 FLOP/sample forward) but K is only 32/64, so the
-// kernel is bounded by the TMEM->register->shared epilogue round trips and by 86 B/sample of HBM
-// traffic (emb 64 B + dir 12 B in, sigma 4 B + rgb 6 B out); see DESIGN.md.
-#include <stdlib.h>
-
-#include "tcgen05.cuh"
-
-namespace ngp {
-int mlp_fwd_v2_launch(const void* emb_f16, const float* dirs, const ngp_mlp_weights* w, float* sigmas, void* rgbs,
-                      void* save, int64_t n, const int32_t* n_dev, cudaStream_t st);
-}
+// Data layout.  Weights (9,408 fp16 = 18.4 KB, W5 zero-padded to 16 rows) stay resident in shared memory for the
+// lifetime of the persistent CTA, in the no-swizzle core-matrix layout (8x8 fp16 core matrices of 128 contiguous
+// bytes): the forward reads them K-major (D = X W^T), the backward reads the same copy MN-major (dX = dY W).
+// Forward: only the embedding tile goes through shared memory (layer 1 is an SS MMA); every later layer takes its A
+// operand from registers — the previous layer's accumulators, converted to fp16 pairs in place (wgmma.cuh).
+// Backward: the dX chain runs the same way from registers; the weight gradients dW = dY^T X (M = 64, K = the tile's
+// 64 samples) read both operands MN-major from shared-memory copies of the activations and accumulate in registers
+// across all tiles of the persistent CTA, flushed once at the end with fp32 atomics.
+#include "wgmma.cuh"
 
 namespace {
-using namespace ngp_tc;
+using namespace ngp_wg;
 
-constexpr int kRows = 128;          // sample rows per tile == TMEM lanes
-constexpr int kThreads = 256;       // TWO threads per row: warps 0-3 own accumulator columns [0,32), warps 4-7 own [32,64)
-constexpr int kThreadsBwd = 288;    // backward: + warp 8, which only issues MMAs (the 8-MMA weight-gradient batches of a
-                                    // round are issued while warps 0-7 run that round's epilogue)
-                                    // (a warp may touch TMEM lanes 32*(warp%4)..+31), halving every epilogue's latency
-constexpr uint32_t kTmemCols = 64;  // fp32 accumulator columns (max N = 64)
-
-// shared memory map (bytes).  Weights first (tcgen05.cuh, shared by all MLP kernels), then activation buffers.
-constexpr int kB64 = kTile * 64 * 2;         // one [128 x 64] fp16 operand buffer
+constexpr int kThreads = 128;   // one warpgroup
+constexpr int kB64 = kTile * 64 * 2;   // one [64 x 64] fp16 operand buffer
 constexpr int kB32 = kTile * 32 * 2;
 constexpr int kB16 = kTile * 16 * 2;
-// forward kernel: two ping-pong buffers
-constexpr int kBufA = kAct;
-constexpr int kBufB = kBufA + kB64;
-constexpr int kBar = kBufB + kB64;           // mbarrier (8 B) + tmem base (4 B)
-constexpr int kSmemBytes = kBar + 16;
-// backward kernel: every activation of the recomputed forward stays resident
-constexpr int kE = kAct;                     // X = emb            [128 x 32]
-constexpr int kH1 = kE + kB32;               // relu(X W1^T)       [128 x 64]   (later: dH1)
-constexpr int kX3 = kH1 + kB64;              // [SH | h]           [128 x 32]
-constexpr int kH3 = kX3 + kB32;              // relu(X3 W3^T)      [128 x 64]   (later: dH1)
-constexpr int kH4 = kH3 + kB64;              // relu(H3 W4^T)      [128 x 64]   (later: dH3)
-constexpr int kDH4 = kH4 + kB64;             // dL/dH4             [128 x 64]
-constexpr int kDO = kDH4 + kB64;             // dL/do (3 of 16)    [128 x 16]
-constexpr int kDH = kDO + kB16;              // dL/dh              [128 x 16]
-constexpr int kBarBwd = kDH + kB16;
-constexpr int kSmemBytesBwd = kBarBwd + 32;  // 110,624 B -> 2 CTAs / SM
-// TMEM columns of the backward kernel: per-tile accumulator + persistent weight-gradient accumulators
-constexpr uint32_t kTmemColsBwd = 256;
-constexpr uint32_t kColDW4 = 64, kColDW1 = 128, kColDW3 = 160, kColDW2T = 192, kColDW5T = 208;
 
-// ---- optional per-round clock trace (scripts/mlp_round_trace.py builds a separate library with -DNGP_MLP_TRACE)
-#ifdef NGP_MLP_TRACE
-__device__ long long g_mlp_trace[2 * 4 * 32];
-#define NGP_TR(k)                                                                                   \
-    do {                                                                                            \
-        if (blockIdx.x == 0 && (tid == 0 || tid == 160) && tile_no < 4)                             \
-            g_mlp_trace[(tid ? 128 : 0) + tile_no * 32 + (k)] = clock64();                          \
-    } while (0)
-#else
-#define NGP_TR(k) ((void)0)
-#endif
+// forward: the embedding tile
+constexpr int kX = kAct;
+constexpr int kSmemFwd = kX + kB32;           // 24,576 B
+// backward: the activations the weight-gradient MMAs read
+constexpr int kE = kAct;                       // X = emb            [64 x 32]
+constexpr int kH1 = kE + kB32;                 // relu(X W1^T)       [64 x 64]
+constexpr int kX3 = kH1 + kB64;                // [SH | h]           [64 x 32]
+constexpr int kH3 = kX3 + kB32;                // relu(X3 W3^T)      [64 x 64]
+constexpr int kH4 = kH3 + kB64;                // relu(H3 W4^T)      [64 x 64]
+constexpr int kDO = kH4 + kB64;                // dL/do (3 of 16)    [64 x 16]
+constexpr int kDH4 = kDO + kB16;               // dL/dH4             [64 x 64]
+constexpr int kDH3 = kDH4 + kB64;              // dL/dH3             [64 x 64]
+constexpr int kDH = kDH3 + kB64;               // dL/dh              [64 x 16]
+constexpr int kDH1 = kDH + kB16;               // dL/dH1             [64 x 64]
+constexpr int kSmemBwd = kDH1 + kB64;          // 81,920 B
 
-// per-thread inputs of one tile row, fetched one tile ahead so the ~1 us DRAM latency overlaps the
-// previous tile's MMA / epilogue rounds
-struct RowIn {
-    uint4 e[2];          // this thread's 2 of the row's 4 embedding chunks (16 fp16 values)
-    float dx, dy, dz;    // used by hh == 1 (SH)
-    float dsig, dr[3];   // backward only, used by hh == 0
-    uint4 hs[2];         // backward with saved activations: h (16 fp16) of this row, used by hh == 0
-    uint2 rgb;           // ... and the forward's fp16 rgb output (3 used)
-};
 // activations saved by the forward for the backward (ngp_mlp_save_bytes): [n_max x 16] fp16 h = sigma-net output,
 // then [n_max x 4] fp16 rgb (the sigmoid output, as torch's sigmoid backward keeps it)
 __device__ __forceinline__ const __half* save_rgb_ptr(const __half* save, int64_t n_max) { return save + n_max * 16; }
 __device__ __forceinline__ __half* save_rgb_ptr(__half* save, int64_t n_max) { return save + n_max * 16; }
 
-template <typename TEmb, bool kBwd, bool kSaved = false>
-__device__ __forceinline__ RowIn load_row(const TEmb* __restrict__ emb, const float* __restrict__ dirs,
-                                           const float* __restrict__ dsigmas, const __half* __restrict__ drgbs,
-                                           int64_t i, bool valid, int hh, const __half* __restrict__ save = nullptr,
-                                           int64_t n_max = 0) {
-    RowIn r;
-    r.e[0] = r.e[1] = make_uint4(0, 0, 0, 0);
-    r.hs[0] = r.hs[1] = make_uint4(0, 0, 0, 0);
-    r.rgb = make_uint2(0, 0);
-    r.dx = 0.f; r.dy = 0.f; r.dz = 1.f; r.dsig = 0.f; r.dr[0] = r.dr[1] = r.dr[2] = 0.f;
-    if (valid) {
+__device__ __forceinline__ float r16(float x) { return __half2float(__float2half_rn(x)); }
+
+// the two 16-byte chunks of embedding row `row` that thread half `q2` (0/1) stages
+template <typename TEmb>
+__device__ __forceinline__ void load_emb(const TEmb* __restrict__ emb, int64_t row, bool valid, int q2, uint4 e[2]) {
+    e[0] = e[1] = make_uint4(0, 0, 0, 0);
+    if (!valid) return;
 #pragma unroll
-        for (int q = 0; q < 2; ++q) {
-            const int kc = hh * 2 + q;
-            if constexpr (sizeof(TEmb) == 2) {
-                r.e[q] = __ldg(reinterpret_cast<const uint4*>(emb + i * 32) + kc);
-            } else {
-                const float4 a = __ldg(reinterpret_cast<const float4*>(emb + i * 32 + kc * 8));
-                const float4 b = __ldg(reinterpret_cast<const float4*>(emb + i * 32 + kc * 8 + 4));
-                r.e[q] = make_uint4(pack_h2(a.x, a.y), pack_h2(a.z, a.w), pack_h2(b.x, b.y), pack_h2(b.z, b.w));
-            }
-        }
-        if (hh == 1) {
-            r.dx = __ldg(dirs + i * 3 + 0);
-            r.dy = __ldg(dirs + i * 3 + 1);
-            r.dz = __ldg(dirs + i * 3 + 2);
-        } else if constexpr (kBwd) {
-            r.dsig = __ldg(dsigmas + i);
-#pragma unroll
-            for (int c = 0; c < 3; ++c) r.dr[c] = __half2float(drgbs[i * 3 + c]);
-            if constexpr (kSaved) {
-                r.hs[0] = __ldg(reinterpret_cast<const uint4*>(save + i * 16));
-                r.hs[1] = __ldg(reinterpret_cast<const uint4*>(save + i * 16) + 1);
-                r.rgb = __ldg(reinterpret_cast<const uint2*>(save_rgb_ptr(save, n_max) + i * 4));
-            }
+    for (int q = 0; q < 2; ++q) {
+        const int kc = q2 * 2 + q;
+        if constexpr (sizeof(TEmb) == 2) {
+            e[q] = __ldg(reinterpret_cast<const uint4*>(emb + row * 32) + kc);
+        } else {
+            const float4 a = __ldg(reinterpret_cast<const float4*>(emb + row * 32 + kc * 8));
+            const float4 b = __ldg(reinterpret_cast<const float4*>(emb + row * 32 + kc * 8 + 4));
+            e[q] = make_uint4(pack_h2(a.x, a.y), pack_h2(a.z, a.w), pack_h2(b.x, b.y), pack_h2(b.z, b.w));
         }
     }
-    return r;
+}
+
+// ---- register fragments (wgmma.cuh): a thread holds rows r0 = 16*warp + lane/4 and r1 = r0 + 8, column pairs
+// 2t, 2t+1 (+8, +16, ...) with t = lane % 4.  Fragment kk of a [64 x K] operand covers columns 16kk..16kk+15.
+__device__ __forceinline__ void relu_frags(const float* d, int nk, uint32_t (*f)[4]) {
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk)
+        if (kk < nk)
+#pragma unroll
+            for (int q = 0; q < 4; ++q) f[kk][q] = pack_h2_relu(d[8 * kk + 2 * q], d[8 * kk + 2 * q + 1]);
+}
+// fragment kk -> the shared-memory operand layout of a [64 x K] buffer
+__device__ __forceinline__ void store_frag(uint8_t* buf, int K, int kk, const uint32_t f[4], int r0, int t) {
+    *reinterpret_cast<uint32_t*>(buf + chunk_off(r0, 2 * kk, K) + 4 * t) = f[0];
+    *reinterpret_cast<uint32_t*>(buf + chunk_off(r0 + 8, 2 * kk, K) + 4 * t) = f[1];
+    *reinterpret_cast<uint32_t*>(buf + chunk_off(r0, 2 * kk + 1, K) + 4 * t) = f[2];
+    *reinterpret_cast<uint32_t*>(buf + chunk_off(r0 + 8, 2 * kk + 1, K) + 4 * t) = f[3];
+}
+__device__ __forceinline__ uint32_t load_pair(const uint8_t* buf, int K, int row, int col) {
+    return *reinterpret_cast<const uint32_t*>(buf + chunk_off(row, col >> 3, K) + (col & 7) * 2);
+}
+// backward hidden epilogue: fp16(D) masked by relu'(act) (act = the post-ReLU forward activation, a [64 x 64]
+// buffer), as select semantics like threshold_backward -> fragments + the dst buffer
+__device__ __forceinline__ void relu_bwd_frags(const float* d, const uint8_t* act, uint8_t* dst, int r0, int t,
+                                               uint32_t (*f)[4]) {
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+            const uint32_t a = load_pair(act, 64, r0 + 8 * (q & 1), 16 * kk + 8 * (q >> 1) + 2 * t);
+            f[kk][q] = pack_h2(d[8 * kk + 2 * q], d[8 * kk + 2 * q + 1]) &
+                       __hgt2_mask(*reinterpret_cast<const __half2*>(&a), __float2half2_rn(0.0f));
+        }
+        store_frag(dst, 64, kk, f[kk], r0, t);
+    }
+}
+// fp16 pair (e[2t], e[2t+1]) of a 16-vector without dynamic register indexing
+__device__ __forceinline__ uint32_t pick_pair(const float* e, int t) {
+    float a = e[0], b = e[1];
+#pragma unroll
+    for (int c = 1; c < 4; ++c)
+        if (t == c) {
+            a = e[2 * c];
+            b = e[2 * c + 1];
+        }
+    return pack_h2(a, b);
+}
+// X3 fragment 0: SH16((d/|d| + 1)/2) of rows r0 (d0) and r1 (d1)  (networks.py:162-164)
+__device__ __forceinline__ void sh_frag(const float* d0, const float* d1, int t, uint32_t f[4]) {
+    float e[16];
+    float inv = 1.0f / sqrtf(d0[0] * d0[0] + d0[1] * d0[1] + d0[2] * d0[2]);
+    sh16((d0[0] * inv + 1.0f) / 2.0f, (d0[1] * inv + 1.0f) / 2.0f, (d0[2] * inv + 1.0f) / 2.0f, e);
+    f[0] = pick_pair(e, t);
+    f[2] = pick_pair(e + 8, t);
+    inv = 1.0f / sqrtf(d1[0] * d1[0] + d1[1] * d1[1] + d1[2] * d1[2]);
+    sh16((d1[0] * inv + 1.0f) / 2.0f, (d1[1] * inv + 1.0f) / 2.0f, (d1[2] * inv + 1.0f) / 2.0f, e);
+    f[1] = pick_pair(e, t);
+    f[3] = pick_pair(e + 8, t);
+}
+__device__ __forceinline__ void load_dir(const float* __restrict__ dirs, int64_t i, bool valid, float d[3]) {
+    d[0] = 0.f; d[1] = 0.f; d[2] = 1.f;
+    if (valid) {
+        d[0] = __ldg(dirs + i * 3 + 0);
+        d[1] = __ldg(dirs + i * 3 + 1);
+        d[2] = __ldg(dirs + i * 3 + 2);
+    }
+}
+
+// fp32 atomics of a [64 x N] accumulator into grad_w (dst(m, col) -> address, or null to skip); element 4j + 2k + c
+// of a thread is (row r0 + 8k, column 8j + 2t + c)
+template <int N, typename F>
+__device__ __forceinline__ void flush_acc(const float* d, int r0, int t, bool& bad, F dst) {
+#pragma unroll
+    for (int e = 0; e < N / 2; ++e) {
+        const int j = e >> 2, k = (e >> 1) & 1, c = e & 1;
+        bad = bad || !(fabsf(d[e]) < INFINITY);
+        if (float* p = dst(r0 + 8 * k, 8 * j + 2 * t + c)) atomicAdd(p, d[e]);
+    }
+}
+
+// per-CTA occupancy of a kernel on the current device, for the persistent grid
+template <typename K>
+int ctas_per_sm(K kernel, int smem) {
+    int b = 0;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, kernel, kThreads, smem) != cudaSuccess || b < 1) {
+        cudaGetLastError();
+        b = 1;
+    }
+    return b;
 }
 
 template <typename TEmb>
-__global__ void __launch_bounds__(kThreads, 4) mlp_fwd_kernel(const TEmb* __restrict__ emb, const float* __restrict__ dirs,
+__global__ void __launch_bounds__(kThreads, 3) mlp_fwd_kernel(const TEmb* __restrict__ emb, const float* __restrict__ dirs,
                                                            ngp_mlp_weights w, float* __restrict__ sigmas,
                                                            __half* __restrict__ rgbs, __half* __restrict__ save,
                                                            int64_t n_max, const int32_t* __restrict__ n_dev) {
     extern __shared__ __align__(128) uint8_t smem[];
     const int64_t n = n_dev ? min(n_max, max((int64_t)*n_dev, (int64_t)0)) : n_max;
-    const int tid = threadIdx.x, warp = tid >> 5, row = tid & (kRows - 1), hh = tid >> 7;
-    const uint32_t bar = smem_u32(smem + kBar);
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + kBar + 8);
-
-    // ---- one-time setup: weights -> smem, mbarrier, TMEM allocation
-    stage_weight(smem + kW1, w.w1, 64, 64, 32, kThreads);
-    stage_weight(smem + kW2, w.w2, 16, 16, 64, kThreads);
-    stage_weight(smem + kW3, w.w3, 64, 64, 32, kThreads);
-    stage_weight(smem + kW4, w.w4, 64, 64, 64, kThreads);
-    stage_weight(smem + kW5, w.w5, 3, 16, 64, kThreads);
-    if (tid == 0) {
-        mbar_init(bar, 1);
-        fence_barrier_init();
-    }
-    if (warp == 0) tmem_alloc(smem_u32(tmem_slot), kTmemCols);
-    fence_proxy_async();
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-    const uint32_t tmem_row = tmem_base + ((uint32_t)((warp & 3) * 32) << 16);  // this warp's 32 lanes
-    uint32_t phase = 0;
-
-    const uint32_t aA = smem_u32(smem + kBufA), aB = smem_u32(smem + kBufB);
-    const uint32_t aW1 = smem_u32(smem + kW1), aW2 = smem_u32(smem + kW2), aW3 = smem_u32(smem + kW3),
-                   aW4 = smem_u32(smem + kW4), aW5 = smem_u32(smem + kW5);
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, t = lane & 3;
+    const int r0 = 16 * warp + (lane >> 2), srow = tid >> 1, q2 = tid & 1;
+    stage_weights(smem, w);
+    const uint32_t aX = smem_u32(smem + kX), aW1 = smem_u32(smem + kW1), aW2 = smem_u32(smem + kW2),
+                   aW3 = smem_u32(smem + kW3), aW4 = smem_u32(smem + kW4), aW5 = smem_u32(smem + kW5);
 
     const int64_t n_tiles = (n + kTile - 1) / kTile;
-    RowIn cur = load_row<TEmb, false>(emb, dirs, nullptr, nullptr, (int64_t)blockIdx.x * kTile + row,
-                                      (int64_t)blockIdx.x * kTile + row < n, hh);
-    [[maybe_unused]] int tile_no = -1;
+    uint4 cur[2];
+    load_emb(emb, (int64_t)blockIdx.x * kTile + srow, (int64_t)blockIdx.x * kTile + srow < n, q2, cur);
     for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-        ++tile_no;
-        NGP_TR(31);
-        const int64_t i = tile * kTile + row;
-        const bool valid = i < n;
+        // ---- stage X = emb[tile rows] as fp16 (K = 32 layout); inputs were fetched one tile ago
+        *reinterpret_cast<uint4*>(smem + kX + chunk_off(srow, 2 * q2, 32)) = cur[0];
+        *reinterpret_cast<uint4*>(smem + kX + chunk_off(srow, 2 * q2 + 1, 32)) = cur[1];
+        {
+            const int64_t in = (tile + gridDim.x) * kTile + srow;
+            load_emb(emb, in, in < n, q2, cur);
+        }
+        const int64_t i0 = tile * kTile + r0, i1 = i0 + 8;
+        const bool v0 = i0 < n, v1 = i1 < n;
+        float d0[3], d1[3];
+        load_dir(dirs, i0, v0, d0);
+        load_dir(dirs, i1, v1, d1);
+        fence_proxy_async();
+        __syncthreads();   // also orders the weight staging before the first tile
 
-        // ---- stage X = emb[i, 0:32] as fp16 into bufA (K = 32 layout); inputs were fetched one tile ago
+        // ---- layer 1: H1 = relu(X W1^T)                       [64x32]x[32x64]
+        float acc[32];
+        uint32_t f[4][4];
+        wgmma_fence();
+        wgmma_ss_n64<0, 0>(acc, desc_kmajor(aX, 32, 0), desc_kmajor(aW1, 32, 0), 0u);
+        wgmma_ss_n64<0, 0>(acc, desc_kmajor(aX, 32, 1), desc_kmajor(aW1, 32, 1), 1u);
+        wgmma_commit();
+        wgmma_wait_all();
+        relu_frags(acc, 4, f);
+
+        // ---- layer 2: h = H1 W2^T                             [64x64]x[64x16]
+        float h[8];
+        wgmma_fence();
 #pragma unroll
-        for (int q = 0; q < 2; ++q) *reinterpret_cast<uint4*>(smem + kBufA + chunk_off(row, hh * 2 + q, 32)) = cur.e[q];
-        const float dx = cur.dx, dy = cur.dy, dz = cur.dz;
-        {   // prefetch the next tile of this CTA
-            const int64_t in = (tile + gridDim.x) * kTile + row;
-            cur = load_row<TEmb, false>(emb, dirs, nullptr, nullptr, in, in < n, hh);
+        for (int kk = 0; kk < 4; ++kk) wgmma_rs_n16<0>(h, f[kk], desc_kmajor(aW2, 64, kk), kk > 0 ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait_all();
+        // sigma = TruncExp(h[:,0]) (networks.py:22-24, :146); X3 = [SH | h]
+        if (t == 0) {
+            if (v0) sigmas[i0] = expf(r16(h[0]));
+            if (v1) sigmas[i1] = expf(r16(h[2]));
         }
-        fence_proxy_async();
-        tc_fence_before();
-        __syncthreads();
-
-        // ---- layer 1: H1 = relu(X W1^T)                       [128x32]x[32x64]
-        NGP_TR(0);
-        if (tid == 0) {
-            tc_fence_after();
-            issue_layer(tmem_base, aA, aW1, 32, 64, bar);
-        }
-        NGP_TR(1);
-        mbar_wait(bar, phase);
-        phase ^= 1;
-        tc_fence_after();
-        NGP_TR(2);
-        epilogue_hidden(tmem_row, smem + kBufB, row, hh);
-        NGP_TR(3);
-        fence_proxy_async();
-        tc_fence_before();
-        NGP_TR(4);
-        __syncthreads();
-        NGP_TR(5);
-
-        // ---- layer 2: h = H1 W2^T                             [128x64]x[64x16]
-        NGP_TR(6);
-        if (tid == 0) {
-            tc_fence_after();
-            issue_layer(tmem_base, aB, aW2, 64, 16, bar);
-        }
-        NGP_TR(7);
-        mbar_wait(bar, phase);
-        phase ^= 1;
-        tc_fence_after();
-        NGP_TR(8);
-        if (hh == 0) {
-            // sigma = TruncExp(h[:,0]) (networks.py:22-24, :146) and the geometry half of X3 = [SH | h]
-            float h[16];
-            tmem_ld16(tmem_row, h);
-            const float h0 = __half2float(__float2half_rn(h[0]));
-            if (valid) sigmas[i] = expf(h0);
-            uint8_t* dst = smem + kBufA;
-            const uint4 lo = make_uint4(pack_h2(h[0], h[1]), pack_h2(h[2], h[3]), pack_h2(h[4], h[5]), pack_h2(h[6], h[7]));
-            const uint4 hi = make_uint4(pack_h2(h[8], h[9]), pack_h2(h[10], h[11]), pack_h2(h[12], h[13]), pack_h2(h[14], h[15]));
-            *reinterpret_cast<uint4*>(dst + chunk_off(row, 2, 32)) = lo;
-            *reinterpret_cast<uint4*>(dst + chunk_off(row, 3, 32)) = hi;
-            if (save != nullptr && valid) {   // the backward restarts from h instead of recomputing layers 1-2 serially
-                reinterpret_cast<uint4*>(save + i * 16)[0] = lo;
-                reinterpret_cast<uint4*>(save + i * 16)[1] = hi;
+        uint32_t x3[2][4];
+        sh_frag(d0, d1, t, x3[0]);
+        x3[1][0] = pack_h2(h[0], h[1]);
+        x3[1][1] = pack_h2(h[2], h[3]);
+        x3[1][2] = pack_h2(h[4], h[5]);
+        x3[1][3] = pack_h2(h[6], h[7]);
+        if (save != nullptr) {   // the backward restarts from h instead of recomputing layers 1-2
+            if (v0) {
+                reinterpret_cast<uint32_t*>(save + i0 * 16)[t] = x3[1][0];
+                reinterpret_cast<uint32_t*>(save + i0 * 16)[4 + t] = x3[1][2];
             }
-        } else {
-            // the direction half, in parallel: SH16((d/|d| + 1)/2)  (networks.py:162-164)
-            const float inv = 1.0f / sqrtf(dx * dx + dy * dy + dz * dz);
-            float e[16];
-            sh16((dx * inv + 1.0f) / 2.0f, (dy * inv + 1.0f) / 2.0f, (dz * inv + 1.0f) / 2.0f, e);
-            uint8_t* dst = smem + kBufA;
-            *reinterpret_cast<uint4*>(dst + chunk_off(row, 0, 32)) =
-                make_uint4(pack_h2(e[0], e[1]), pack_h2(e[2], e[3]), pack_h2(e[4], e[5]), pack_h2(e[6], e[7]));
-            *reinterpret_cast<uint4*>(dst + chunk_off(row, 1, 32)) =
-                make_uint4(pack_h2(e[8], e[9]), pack_h2(e[10], e[11]), pack_h2(e[12], e[13]), pack_h2(e[14], e[15]));
+            if (v1) {
+                reinterpret_cast<uint32_t*>(save + i1 * 16)[t] = x3[1][1];
+                reinterpret_cast<uint32_t*>(save + i1 * 16)[4 + t] = x3[1][3];
+            }
         }
-        NGP_TR(9);
-        fence_proxy_async();
-        tc_fence_before();
-        NGP_TR(10);
-        __syncthreads();
-        NGP_TR(11);
 
-        // ---- layer 3: H3 = relu(X3 W3^T)                      [128x32]x[32x64]
-        NGP_TR(12);
-        if (tid == 0) {
-            tc_fence_after();
-            issue_layer(tmem_base, aA, aW3, 32, 64, bar);
-        }
-        NGP_TR(13);
-        mbar_wait(bar, phase);
-        phase ^= 1;
-        tc_fence_after();
-        NGP_TR(14);
-        epilogue_hidden(tmem_row, smem + kBufB, row, hh);
-        NGP_TR(15);
-        fence_proxy_async();
-        tc_fence_before();
-        NGP_TR(16);
-        __syncthreads();
-        NGP_TR(17);
+        // ---- layer 3: H3 = relu(X3 W3^T)                      [64x32]x[32x64]
+        wgmma_fence();
+        wgmma_rs_n64<0>(acc, x3[0], desc_kmajor(aW3, 32, 0), 0u);
+        wgmma_rs_n64<0>(acc, x3[1], desc_kmajor(aW3, 32, 1), 1u);
+        wgmma_commit();
+        wgmma_wait_all();
+        relu_frags(acc, 4, f);
 
-        // ---- layer 4: H4 = relu(H3 W4^T)                      [128x64]x[64x64]
-        NGP_TR(18);
-        if (tid == 0) {
-            tc_fence_after();
-            issue_layer(tmem_base, aB, aW4, 64, 64, bar);
-        }
-        NGP_TR(19);
-        mbar_wait(bar, phase);
-        phase ^= 1;
-        tc_fence_after();
-        NGP_TR(20);
-        epilogue_hidden(tmem_row, smem + kBufA, row, hh);
-        NGP_TR(21);
-        fence_proxy_async();
-        tc_fence_before();
-        NGP_TR(22);
-        __syncthreads();
-        NGP_TR(23);
-
-        // ---- layer 5: rgb = sigmoid(H4 W5^T)                  [128x64]x[64x16(3 used)]
-        NGP_TR(24);
-        if (tid == 0) {
-            tc_fence_after();
-            issue_layer(tmem_base, aA, aW5, 64, 16, bar);
-        }
-        NGP_TR(25);
-        mbar_wait(bar, phase);
-        phase ^= 1;
-        tc_fence_after();
-        NGP_TR(26);
-        if (hh == 0) {
-            float o[16];
-            tmem_ld16(tmem_row, o);
-            if (valid) {
-                __half out[3];
+        // ---- layer 4: H4 = relu(H3 W4^T)                      [64x64]x[64x64]
+        wgmma_fence();
 #pragma unroll
-                for (int c = 0; c < 3; ++c) {
-                    const float oc = __half2float(__float2half_rn(o[c]));
-                    out[c] = __float2half_rn(1.0f / (1.0f + expf(-oc)));
-                    rgbs[i * 3 + c] = out[c];
-                }
+        for (int kk = 0; kk < 4; ++kk) wgmma_rs_n64<0>(acc, f[kk], desc_kmajor(aW4, 64, kk), kk > 0 ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait_all();
+        relu_frags(acc, 4, f);
+
+        // ---- layer 5: rgb = sigmoid(H4 W5^T)                  [64x64]x[64x8 (3 used)]
+        float o[4];
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) wgmma_rs_n8<0>(o, f[kk], desc_kmajor(aW5, 64, kk), kk > 0 ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait_all();
+        if (t < 2) {   // t = 0: channels 0, 1; t = 1: channel 2 (column 3 is padding)
+#pragma unroll
+            for (int k = 0; k < 2; ++k) {
+                const int64_t i = k ? i1 : i0;
+                if (!(k ? v1 : v0)) continue;
+                const __half a = __float2half_rn(1.0f / (1.0f + expf(-r16(o[2 * k]))));
+                const __half b = __float2half_rn(1.0f / (1.0f + expf(-r16(o[2 * k + 1]))));
+                rgbs[i * 3 + 2 * t] = a;
+                if (t == 0) rgbs[i * 3 + 1] = b;
                 if (save != nullptr) {
-                    const __half2 a = __halves2half2(out[0], out[1]), b = __halves2half2(out[2], __float2half_rn(0.0f));
-                    *reinterpret_cast<uint2*>(save_rgb_ptr(save, n_max) + i * 4) =
-                        make_uint2(*reinterpret_cast<const uint32_t*>(&a), *reinterpret_cast<const uint32_t*>(&b));
+                    const __half2 p = __halves2half2(a, t == 0 ? b : __float2half_rn(0.0f));
+                    reinterpret_cast<__half2*>(save_rgb_ptr(save, n_max) + i * 4)[t] = p;
                 }
             }
         }
-        NGP_TR(27);
-        tc_fence_before();
-        __syncthreads();  // bufA / TMEM are reused by the next tile
     }
-
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) tmem_dealloc(tmem_base, kTmemCols);
 }
 
 // =====================================================================================================
 // Backward.  Replaces the autograd graph of the five nn.Linear layers (cuBLAS dX + dW GEMMs), ReLU /
-// Sigmoid / TruncExp backward (modules/networks.py:26-30) under autocast.  Per 128-sample tile:
-//   1. recompute the forward activations into shared memory (nothing was saved by the forward);
-//   2. chain  dO -> dH4 -> dH3 -> dX3 -> dH -> dH1 -> dE  with  dX = dY * W  as tcgen05 MMAs whose B
-//      operand is the SAME shared-memory weight copy read MN-major (i.e. transposed by descriptor);
-//   3. weight gradients  dW = dY^T * X  as M=64 MMAs with K = the 128 samples of the tile, both operands
-//      read MN-major from the activation buffers, accumulated in TMEM across ALL tiles of the persistent
-//      CTA and flushed once at the end with fp32 atomics (9,408 per CTA).
+// Sigmoid / TruncExp backward (modules/networks.py:26-30) under autocast.  Per 64-sample tile:
+//   1. recompute the forward activations (with saved activations, layers 2 and 5 are skipped: h and rgb are read);
+//   2. chain  dO -> dH4 -> dH3 -> dX3 -> dh -> dH1 -> dE  with  dX = dY W  as RS MMAs whose B operand is the SAME
+//      shared-memory weight copy read MN-major;
+//   3. weight gradients  dW = dY^T X  as SS MMAs (both operands MN-major from shared memory) issued together with the
+//      round's dX MMA, accumulated in registers across all tiles of the persistent CTA.
 // Gradient operands of invalid (tail) rows are zero, so they do not contribute to dW.
-
-// generic GEMM issue: operand = (start address, LBO, SBO, bytes to advance per 16-wide K step)
-struct Operand {
-    uint32_t addr, lbo, sbo, kstep;
-};
-// operand stored as [row][K cols] (row-block stride K*16 B) and consumed K-major (rows = M or N)
-__host__ __device__ __forceinline__ Operand op_kmajor(uint32_t addr, int K) { return {addr, 128u, (uint32_t)K * 16u, 256u}; }
-// the same storage consumed MN-major: MN = the stored columns, K = the stored rows
-__host__ __device__ __forceinline__ Operand op_mnmajor(uint32_t addr, int K) { return {addr, (uint32_t)K * 16u, 128u, (uint32_t)K * 32u}; }
-
-__host__ __device__ constexpr uint32_t idesc_full(int m, int n, int a_mn, int b_mn) {
-    return (1u << 4) | ((uint32_t)a_mn << 15) | ((uint32_t)b_mn << 16) | ((uint32_t)(n >> 3) << 17) |
-           ((uint32_t)(m >> 4) << 24);
-}
-
-__device__ __forceinline__ void issue_gemm(uint32_t tmem_d, const Operand& a, const Operand& b, int ksteps,
-                                           uint32_t idesc, bool accumulate) {
-    for (int k = 0; k < ksteps; ++k) {
-        const uint64_t da = smem_desc(a.addr + k * a.kstep, a.lbo, a.sbo);
-        const uint64_t db = smem_desc(b.addr + k * b.kstep, b.lbo, b.sbo);
-        umma_f16(tmem_d, da, db, idesc, (accumulate || k > 0) ? 1u : 0u);
-    }
-}
-
-// backward hidden epilogue: TMEM [128 x 64] fp32 -> fp16, masked by relu'(act) where `act` holds the
-// post-ReLU forward activation of this thread's row -> dst (K = 64 layout).  dst may alias act.
-__device__ __forceinline__ void epilogue_relu_bwd(uint32_t tmem_row, const uint8_t* act, uint8_t* dst, int row, int hh) {
-    float v[32];
-    tmem_ld32(tmem_row + hh * 32, v);
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-        const int kc = hh * 4 + q;
-        const uint4 a = *reinterpret_cast<const uint4*>(act + chunk_off(row, kc, 64));
-        const uint32_t aw[4] = {a.x, a.y, a.z, a.w};
-        uint32_t o[4];
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-            // relu'(act) as a per-half bit mask (0xffff where act > 0): select semantics like threshold_backward,
-            // one HSET2.BM + LOP3 per pair instead of two unpack / compare / select chains
-            const __half2 ah = *reinterpret_cast<const __half2*>(&aw[j]);
-            o[j] = pack_h2(v[q * 8 + 2 * j], v[q * 8 + 2 * j + 1]) & __hgt2_mask(ah, __float2half2_rn(0.0f));
-        }
-        *reinterpret_cast<uint4*>(dst + chunk_off(row, kc, 64)) = make_uint4(o[0], o[1], o[2], o[3]);
-    }
-}
-
 template <typename TEmb, bool kSaved>
-__global__ void __launch_bounds__(kThreadsBwd, 2) mlp_bwd_kernel(const TEmb* __restrict__ emb, const float* __restrict__ dirs,
+__global__ void __launch_bounds__(kThreads, 2) mlp_bwd_kernel(const TEmb* __restrict__ emb, const float* __restrict__ dirs,
                                                            ngp_mlp_weights w, const __half* __restrict__ save,
                                                            const float* __restrict__ dsigmas,
                                                            const __half* __restrict__ drgbs, TEmb* __restrict__ demb,
@@ -390,921 +286,286 @@ __global__ void __launch_bounds__(kThreadsBwd, 2) mlp_bwd_kernel(const TEmb* __r
                                                            int32_t* __restrict__ found_inf) {
     extern __shared__ __align__(128) uint8_t smem[];
     const int64_t n = n_dev ? min(n_max, max((int64_t)*n_dev, (int64_t)0)) : n_max;
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, row = tid & (kRows - 1), hh = tid >> 7;
-    const bool worker = tid < kThreads;   // warps 0-7: two threads per tile row; warp 8 (hh == 2): MMA issue only
-    const uint32_t bar = smem_u32(smem + kBarBwd);
-    const uint32_t bar2 = smem_u32(smem + kBarBwd + 16);
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + kBarBwd + 8);
-    uint32_t phase2 = 0;
-
-    stage_weight(smem + kW1, w.w1, 64, 64, 32, kThreads);
-    stage_weight(smem + kW2, w.w2, 16, 16, 64, kThreads);
-    stage_weight(smem + kW3, w.w3, 64, 64, 32, kThreads);
-    stage_weight(smem + kW4, w.w4, 64, 64, 64, kThreads);
-    stage_weight(smem + kW5, w.w5, 3, 16, 64, kThreads);
-    if (tid == 0) {
-        mbar_init(bar, 1);
-        mbar_init(bar2, 1);
-        fence_barrier_init();
-    }
-    if (warp == 0) tmem_alloc(smem_u32(tmem_slot), kTmemColsBwd);
-    fence_proxy_async();
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-    const uint32_t tmem_row = tmem_base + ((uint32_t)((warp & 3) * 32) << 16);
-    uint32_t phase = 0;
-
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, t = lane & 3;
+    const int r0 = 16 * warp + (lane >> 2), srow = tid >> 1, q2 = tid & 1;
+    stage_weights(smem, w);
     const uint32_t aW1 = smem_u32(smem + kW1), aW2 = smem_u32(smem + kW2), aW3 = smem_u32(smem + kW3),
                    aW4 = smem_u32(smem + kW4), aW5 = smem_u32(smem + kW5);
     const uint32_t aE = smem_u32(smem + kE), aH1 = smem_u32(smem + kH1), aX3 = smem_u32(smem + kX3),
-                   aH3 = smem_u32(smem + kH3), aH4 = smem_u32(smem + kH4), aDH4 = smem_u32(smem + kDH4),
-                   aDO = smem_u32(smem + kDO), aDH = smem_u32(smem + kDH);
+                   aH3 = smem_u32(smem + kH3), aH4 = smem_u32(smem + kH4), aDO = smem_u32(smem + kDO),
+                   aDH4 = smem_u32(smem + kDH4), aDH3 = smem_u32(smem + kDH3), aDH = smem_u32(smem + kDH),
+                   aDH1 = smem_u32(smem + kDH1);
 
-// One MMA round.  DX feeds the next epilogue and is committed to `bar`; DW (weight-gradient MMAs, may be
-// empty) is issued right behind it and runs while the epilogue executes.  tcgen05.commit tracks ALL prior
-// MMAs of the issuing thread, so the commit of round r+1 also covers DW of round r: every buffer a DW
-// reads is only overwritten after a later round's wait — except the last round's, which commits to `bar2`.
-#define NGP_ROUND2(DX, DW, LAST)               \
-    fence_proxy_async();                       \
-    tc_fence_before();                         \
-    __syncthreads();                           \
-    if (tid == kThreads) {                     \
-        tc_fence_after();                      \
-        DX;                                    \
-        umma_commit(bar);                      \
-        DW;                                    \
-        if (LAST) umma_commit(bar2);           \
-    }                                          \
-    mbar_wait(bar, phase);                     \
-    phase ^= 1;                                \
-    tc_fence_after();
-#define NGP_ROUND(ISSUE) NGP_ROUND2(ISSUE, (void)0, false)
+    // weight-gradient accumulators: dW4 [64 out x 64 in], dW3 / dW1 [64 out x 32 in], dW2^T [64 in x 16 out],
+    // dW5^T [64 in x 8 (3 used)]
+    float gW4[32], gW3[16], gW1[16], gW2T[8], gW5T[4];
+#pragma unroll
+    for (int j = 0; j < 32; ++j) gW4[j] = 0.f;
+#pragma unroll
+    for (int j = 0; j < 16; ++j) gW3[j] = gW1[j] = 0.f;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) gW2T[j] = 0.f;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) gW5T[j] = 0.f;
 
-    bool first = true;  // first tile of this CTA: weight-gradient accumulators start from zero
     const int64_t n_tiles = (n + kTile - 1) / kTile;
-    RowIn cur = load_row<TEmb, true, kSaved>(emb, dirs, dsigmas, drgbs, (int64_t)blockIdx.x * kTile + row,
-                                             worker && (int64_t)blockIdx.x * kTile + row < n, hh, save, n_max);
+    uint4 cur[2];
+    load_emb(emb, (int64_t)blockIdx.x * kTile + srow, (int64_t)blockIdx.x * kTile + srow < n, q2, cur);
     for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-        const int64_t i = tile * kTile + row;
-        const bool valid = worker && i < n;
-
-        // ================= forward recompute =================
-        if (worker) {
+        *reinterpret_cast<uint4*>(smem + kE + chunk_off(srow, 2 * q2, 32)) = cur[0];
+        *reinterpret_cast<uint4*>(smem + kE + chunk_off(srow, 2 * q2 + 1, 32)) = cur[1];
+        {
+            const int64_t in = (tile + gridDim.x) * kTile + srow;
+            load_emb(emb, in, in < n, q2, cur);
+        }
+        // this thread's two rows: directions, upstream gradients, saved activations
+        int64_t ii[2];
+        bool vv[2];
+        float dd[2][3], dsig[2], dr[2][3];
+        uint32_t hs[2][2] = {{0u, 0u}, {0u, 0u}};
+        uint2 rgb_saved[2] = {make_uint2(0, 0), make_uint2(0, 0)};
 #pragma unroll
-            for (int q = 0; q < 2; ++q) *reinterpret_cast<uint4*>(smem + kE + chunk_off(row, hh * 2 + q, 32)) = cur.e[q];
-        }
-        const float dx = cur.dx, dy = cur.dy, dz = cur.dz, dsig = cur.dsig;  // dirs: hh == 1, dsig/dr: hh == 0
-        const float dr[3] = {cur.dr[0], cur.dr[1], cur.dr[2]};
-        [[maybe_unused]] const uint4 hs0 = cur.hs[0], hs1 = cur.hs[1];
-        [[maybe_unused]] const uint2 rgb_saved = cur.rgb;
-        {   // prefetch the next tile of this CTA (consumed one iteration later)
-            const int64_t in = (tile + gridDim.x) * kTile + row;
-            cur = load_row<TEmb, true, kSaved>(emb, dirs, dsigmas, drgbs, in, worker && in < n, hh, save, n_max);
-        }
-        float h0 = 0.0f;
-        if constexpr (kSaved) {
-            // X3 = [SH | h] straight from the saved h: layers 2 and 5 are not recomputed (8 MMA rounds instead of 10)
-            if (hh == 0) {
-                const __half2 h01 = *reinterpret_cast<const __half2*>(&hs0.x);
-                h0 = __low2float(h01);
-                *reinterpret_cast<uint4*>(smem + kX3 + chunk_off(row, 2, 32)) = hs0;
-                *reinterpret_cast<uint4*>(smem + kX3 + chunk_off(row, 3, 32)) = hs1;
-            }
-        }
-        NGP_ROUND(issue_layer_mma(tmem_base, aE, aW1, 32, 64))          // H1 = relu(E W1^T)
-        if (worker) epilogue_hidden(tmem_row, smem + kH1, row, hh);
-        if constexpr (!kSaved) {
-            NGP_ROUND(issue_layer_mma(tmem_base, aH1, aW2, 64, 16))     // h = H1 W2^T
-            if (hh == 0) {
-                float h[16];
-                tmem_ld16(tmem_row, h);
-                h0 = __half2float(__float2half_rn(h[0]));
-                uint8_t* dst = smem + kX3;
-                *reinterpret_cast<uint4*>(dst + chunk_off(row, 2, 32)) =
-                    make_uint4(pack_h2(h[0], h[1]), pack_h2(h[2], h[3]), pack_h2(h[4], h[5]), pack_h2(h[6], h[7]));
-                *reinterpret_cast<uint4*>(dst + chunk_off(row, 3, 32)) =
-                    make_uint4(pack_h2(h[8], h[9]), pack_h2(h[10], h[11]), pack_h2(h[12], h[13]), pack_h2(h[14], h[15]));
-            }
-        }
-        if (hh == 1) {
-            const float inv = 1.0f / sqrtf(dx * dx + dy * dy + dz * dz);
-            float e[16];
-            sh16((dx * inv + 1.0f) / 2.0f, (dy * inv + 1.0f) / 2.0f, (dz * inv + 1.0f) / 2.0f, e);
-            uint8_t* dst = smem + kX3;
-            *reinterpret_cast<uint4*>(dst + chunk_off(row, 0, 32)) =
-                make_uint4(pack_h2(e[0], e[1]), pack_h2(e[2], e[3]), pack_h2(e[4], e[5]), pack_h2(e[6], e[7]));
-            *reinterpret_cast<uint4*>(dst + chunk_off(row, 1, 32)) =
-                make_uint4(pack_h2(e[8], e[9]), pack_h2(e[10], e[11]), pack_h2(e[12], e[13]), pack_h2(e[14], e[15]));
-        }
-        NGP_ROUND(issue_layer_mma(tmem_base, aX3, aW3, 32, 64))         // H3 = relu(X3 W3^T)
-        if (worker) epilogue_hidden(tmem_row, smem + kH3, row, hh);
-        NGP_ROUND(issue_layer_mma(tmem_base, aH3, aW4, 64, 64))         // H4 = relu(H3 W4^T)
-        if (worker) epilogue_hidden(tmem_row, smem + kH4, row, hh);
-        if constexpr (!kSaved) {
-            NGP_ROUND(issue_layer_mma(tmem_base, aH4, aW5, 64, 16))     // o = H4 W5^T
-        }
-        if (hh == 0) {
-            // dL/do = dL/drgb * rgb (1 - rgb), rounded to fp16 like the autocast graph
-            float rgbv[3];
-            if constexpr (kSaved) {   // torch's sigmoid backward also uses the saved fp16 output
-                const __half2 a = *reinterpret_cast<const __half2*>(&rgb_saved.x);
-                const __half2 b = *reinterpret_cast<const __half2*>(&rgb_saved.y);
-                rgbv[0] = __low2float(a);
-                rgbv[1] = __high2float(a);
-                rgbv[2] = __low2float(b);
-            } else {
-                float o[16];
-                tmem_ld16(tmem_row, o);
+        for (int k = 0; k < 2; ++k) {
+            ii[k] = tile * kTile + r0 + 8 * k;
+            vv[k] = ii[k] < n;
+            load_dir(dirs, ii[k], vv[k], dd[k]);
+            dsig[k] = vv[k] ? __ldg(dsigmas + ii[k]) : 0.f;
 #pragma unroll
-                for (int c = 0; c < 3; ++c) {
-                    const float oc = __half2float(__float2half_rn(o[c]));
-                    rgbv[c] = __half2float(__float2half_rn(1.0f / (1.0f + expf(-oc))));
+            for (int c = 0; c < 3; ++c) dr[k][c] = vv[k] ? __half2float(drgbs[ii[k] * 3 + c]) : 0.f;
+            if constexpr (kSaved) {
+                if (vv[k]) {
+                    hs[k][0] = __ldg(reinterpret_cast<const uint32_t*>(save + ii[k] * 16) + t);
+                    hs[k][1] = __ldg(reinterpret_cast<const uint32_t*>(save + ii[k] * 16) + 4 + t);
+                    rgb_saved[k] = __ldg(reinterpret_cast<const uint2*>(save_rgb_ptr(save, n_max) + ii[k] * 4));
                 }
             }
-            float d_o[3];
-#pragma unroll
-            for (int c = 0; c < 3; ++c) d_o[c] = dr[c] * rgbv[c] * (1.0f - rgbv[c]);
-            *reinterpret_cast<uint4*>(smem + kDO + chunk_off(row, 0, 16)) =
-                make_uint4(pack_h2(d_o[0], d_o[1]), pack_h2(d_o[2], 0.0f), 0u, 0u);
-        } else if (hh == 1) {
-            *reinterpret_cast<uint4*>(smem + kDO + chunk_off(row, 1, 16)) = make_uint4(0u, 0u, 0u, 0u);
         }
+        fence_proxy_async();
+        __syncthreads();
+
+        // ================= forward recompute =================
+        float acc[32], a32[16];
+        uint32_t f[4][4];
+        wgmma_fence();                                                   // H1 = relu(E W1^T)
+        wgmma_ss_n64<0, 0>(acc, desc_kmajor(aE, 32, 0), desc_kmajor(aW1, 32, 0), 0u);
+        wgmma_ss_n64<0, 0>(acc, desc_kmajor(aE, 32, 1), desc_kmajor(aW1, 32, 1), 1u);
+        wgmma_commit();
+        wgmma_wait_all();
+        relu_frags(acc, 4, f);
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) store_frag(smem + kH1, 64, kk, f[kk], r0, t);
+        uint32_t x3[2][4];
+        float h0[2];
+        if constexpr (kSaved) {   // X3 = [SH | h] straight from the saved h
+            x3[1][0] = hs[0][0];
+            x3[1][1] = hs[1][0];
+            x3[1][2] = hs[0][1];
+            x3[1][3] = hs[1][1];
+            h0[0] = __low2float(*reinterpret_cast<const __half2*>(&hs[0][0]));
+            h0[1] = __low2float(*reinterpret_cast<const __half2*>(&hs[1][0]));
+        } else {
+            float h[8];
+            wgmma_fence();                                               // h = H1 W2^T
+#pragma unroll
+            for (int kk = 0; kk < 4; ++kk) wgmma_rs_n16<0>(h, f[kk], desc_kmajor(aW2, 64, kk), kk > 0 ? 1u : 0u);
+            wgmma_commit();
+            wgmma_wait_all();
+            h0[0] = r16(h[0]);
+            h0[1] = r16(h[2]);
+            x3[1][0] = pack_h2(h[0], h[1]);
+            x3[1][1] = pack_h2(h[2], h[3]);
+            x3[1][2] = pack_h2(h[4], h[5]);
+            x3[1][3] = pack_h2(h[6], h[7]);
+        }
+        sh_frag(dd[0], dd[1], t, x3[0]);
+        store_frag(smem + kX3, 32, 0, x3[0], r0, t);
+        store_frag(smem + kX3, 32, 1, x3[1], r0, t);
+        wgmma_fence();                                                   // H3 = relu(X3 W3^T)
+        wgmma_rs_n64<0>(acc, x3[0], desc_kmajor(aW3, 32, 0), 0u);
+        wgmma_rs_n64<0>(acc, x3[1], desc_kmajor(aW3, 32, 1), 1u);
+        wgmma_commit();
+        wgmma_wait_all();
+        relu_frags(acc, 4, f);
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) store_frag(smem + kH3, 64, kk, f[kk], r0, t);
+        wgmma_fence();                                                   // H4 = relu(H3 W4^T)
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) wgmma_rs_n64<0>(acc, f[kk], desc_kmajor(aW4, 64, kk), kk > 0 ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait_all();
+        relu_frags(acc, 4, f);
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) store_frag(smem + kH4, 64, kk, f[kk], r0, t);
+        // rgb of this thread's columns 2t, 2t+1 (t < 2; channel 3 is padding)
+        float rgbv[2][2] = {{0.f, 0.f}, {0.f, 0.f}};
+        if constexpr (kSaved) {   // torch's sigmoid backward also uses the saved fp16 output
+#pragma unroll
+            for (int k = 0; k < 2; ++k) {
+                const uint32_t p = t == 0 ? rgb_saved[k].x : rgb_saved[k].y;
+                rgbv[k][0] = __low2float(*reinterpret_cast<const __half2*>(&p));
+                rgbv[k][1] = __high2float(*reinterpret_cast<const __half2*>(&p));
+            }
+        } else {
+            float o[4];
+            wgmma_fence();                                               // o = H4 W5^T
+#pragma unroll
+            for (int kk = 0; kk < 4; ++kk) wgmma_rs_n8<0>(o, f[kk], desc_kmajor(aW5, 64, kk), kk > 0 ? 1u : 0u);
+            wgmma_commit();
+            wgmma_wait_all();
+#pragma unroll
+            for (int k = 0; k < 2; ++k)
+#pragma unroll
+                for (int c = 0; c < 2; ++c) rgbv[k][c] = r16(1.0f / (1.0f + expf(-r16(o[2 * k + c]))));
+        }
+        // dL/do = dL/drgb * rgb (1 - rgb), rounded to fp16 like the autocast graph; columns 3..15 are zero
+        uint32_t dof[4] = {0u, 0u, 0u, 0u};
+        if (t < 2) {
+#pragma unroll
+            for (int k = 0; k < 2; ++k) {
+                const float g0 = t == 0 ? dr[k][0] : dr[k][2];
+                const float g1 = t == 0 ? dr[k][1] : 0.f;
+                dof[k] = pack_h2(g0 * rgbv[k][0] * (1.0f - rgbv[k][0]), g1 * rgbv[k][1] * (1.0f - rgbv[k][1]));
+            }
+        }
+        store_frag(smem + kDO, 16, 0, dof, r0, t);
+        fence_proxy_async();
+        __syncthreads();
 
         // ================= backward =================
         // R1: dH4pre = dO W5 ;  dW5^T += H4^T dO
-        NGP_ROUND2(
-            issue_gemm(tmem_base, op_kmajor(aDO, 16), op_mnmajor(aW5, 64), 1, idesc_full(128, 64, 0, 1), false),
-            issue_gemm(tmem_base + kColDW5T, op_mnmajor(aH4, 64), op_mnmajor(aDO, 16), 8, idesc_full(64, 16, 1, 1), !first),
-            false)
-        if (worker) epilogue_relu_bwd(tmem_row, smem + kH4, smem + kDH4, row, hh);
-        // R2: dH3pre = dH4 W4 ;  dW4 += dH4^T H3
-        NGP_ROUND2(
-            issue_gemm(tmem_base, op_kmajor(aDH4, 64), op_mnmajor(aW4, 64), 4, idesc_full(128, 64, 0, 1), false),
-            issue_gemm(tmem_base + kColDW4, op_mnmajor(aDH4, 64), op_mnmajor(aH3, 64), 8, idesc_full(64, 64, 1, 1), !first),
-            false)
-        if (worker) epilogue_relu_bwd(tmem_row, smem + kH3, smem + kH4, row, hh);      // dH3 -> H4's buffer (H4 is dead)
-        // R3: dX3 = dH3 W3 ;  dW3 += dH3^T X3
-        NGP_ROUND2(
-            issue_gemm(tmem_base, op_kmajor(aH4, 64), op_mnmajor(aW3, 32), 4, idesc_full(128, 32, 0, 1), false),
-            issue_gemm(tmem_base + kColDW3, op_mnmajor(aH4, 64), op_mnmajor(aX3, 32), 8, idesc_full(64, 32, 1, 1), !first),
-            false)
-        if (hh == 0) {
-            // dh = dX3[:, 16:32] (+ TruncExp backward on h[:,0], networks.py:26-30), fp16
-            float g[16];
-            tmem_ld16(tmem_row + 16, g);
-            const float ds = __half2float(__float2half_rn(dsig * expf(fminf(fmaxf(h0, -15.0f), 15.0f))));
-            g[0] = __half2float(__float2half_rn(g[0])) + ds;
-            *reinterpret_cast<uint4*>(smem + kDH + chunk_off(row, 0, 16)) =
-                make_uint4(pack_h2(g[0], g[1]), pack_h2(g[2], g[3]), pack_h2(g[4], g[5]), pack_h2(g[6], g[7]));
-            *reinterpret_cast<uint4*>(smem + kDH + chunk_off(row, 1, 16)) =
-                make_uint4(pack_h2(g[8], g[9]), pack_h2(g[10], g[11]), pack_h2(g[12], g[13]), pack_h2(g[14], g[15]));
-        }
-        // R4: dH1pre = dh W2 ;  dW2^T += H1^T dh
-        NGP_ROUND2(
-            issue_gemm(tmem_base, op_kmajor(aDH, 16), op_mnmajor(aW2, 64), 1, idesc_full(128, 64, 0, 1), false),
-            issue_gemm(tmem_base + kColDW2T, op_mnmajor(aH1, 64), op_mnmajor(aDH, 16), 8, idesc_full(64, 16, 1, 1), !first),
-            false)
-        if (worker) epilogue_relu_bwd(tmem_row, smem + kH1, smem + kH3, row, hh);      // dH1 -> H3's buffer (H3 is dead)
-        // R5: dE = dH1 W1 ;  dW1 += dH1^T E
-        NGP_ROUND2(
-            issue_gemm(tmem_base, op_kmajor(aH3, 64), op_mnmajor(aW1, 32), 4, idesc_full(128, 32, 0, 1), false),
-            issue_gemm(tmem_base + kColDW1, op_mnmajor(aH3, 64), op_mnmajor(aE, 32), 8, idesc_full(64, 32, 1, 1), !first),
-            true)
-        if (worker) {
-            const int g = hh;  // columns [16*hh, 16*hh+16) of dE
-            float v[16];
-            tmem_ld16(tmem_row + g * 16, v);
-            if (valid) {
-                if constexpr (sizeof(TEmb) == 2) {
-                    uint4* o = reinterpret_cast<uint4*>(demb + i * 32 + g * 16);
-                    o[0] = make_uint4(pack_h2(v[0], v[1]), pack_h2(v[2], v[3]), pack_h2(v[4], v[5]), pack_h2(v[6], v[7]));
-                    o[1] = make_uint4(pack_h2(v[8], v[9]), pack_h2(v[10], v[11]), pack_h2(v[12], v[13]), pack_h2(v[14], v[15]));
-                } else {
-                    float4* o = reinterpret_cast<float4*>(demb + i * 32 + g * 16);
+        wgmma_fence();
+        wgmma_rs_n64<1>(acc, dof, desc_mnmajor(aW5, 64, 0), 0u);
 #pragma unroll
-                    for (int q = 0; q < 4; ++q) {  // fp16-rounded like the autocast graph, stored as fp32
-                        o[q] = make_float4(__half2float(__float2half_rn(v[4 * q])), __half2float(__float2half_rn(v[4 * q + 1])),
-                                           __half2float(__float2half_rn(v[4 * q + 2])), __half2float(__float2half_rn(v[4 * q + 3])));
-                    }
-                }
-            }
-        }
-        first = false;
-        mbar_wait(bar2, phase2);  // dW1 (reads E and dH1) must finish before the next tile restages them
-        phase2 ^= 1;
-        tc_fence_before();
+        for (int kk = 0; kk < 4; ++kk) wgmma_ss_n8<1, 1>(gW5T, desc_mnmajor(aH4, 64, kk), desc_mnmajor(aDO, 16, kk), 1u);
+        wgmma_commit();
+        wgmma_wait_all();
+        relu_bwd_frags(acc, smem + kH4, smem + kDH4, r0, t, f);
+        fence_proxy_async();
         __syncthreads();
-    }
-#undef NGP_ROUND
-#undef NGP_ROUND2
-
-    // ---- flush the weight-gradient accumulators: M = 64 rows live on TMEM lanes (m%16) + 32*(m/16)
-    if (!first && warp < 4) {
-        const int m = warp * 16 + lane;  // row held by this thread when lane < 16
-        const bool has_row = lane < 16;
-        float v[16];
-        bool bad = false;   // non-finite weight gradient (GradScaler's inf check, raised at the source)
-        auto chk = [&]() {
+        // R2: dH3pre = dH4 W4 ;  dW4 += dH4^T H3
+        wgmma_fence();
 #pragma unroll
-            for (int j = 0; j < 16; ++j) bad = bad || !(fabsf(v[j]) < INFINITY);
-        };
-        // dW4 [64 out x 64 in]
+        for (int kk = 0; kk < 4; ++kk) wgmma_rs_n64<1>(acc, f[kk], desc_mnmajor(aW4, 64, kk), kk > 0 ? 1u : 0u);
 #pragma unroll
-        for (int g = 0; g < 4; ++g) {
-            tmem_ld16(tmem_row + kColDW4 + g * 16, v);
-            if (has_row) chk();
-            if (has_row)
+        for (int kk = 0; kk < 4; ++kk) wgmma_ss_n64<1, 1>(gW4, desc_mnmajor(aDH4, 64, kk), desc_mnmajor(aH3, 64, kk), 1u);
+        wgmma_commit();
+        wgmma_wait_all();
+        relu_bwd_frags(acc, smem + kH3, smem + kDH3, r0, t, f);
+        fence_proxy_async();
+        __syncthreads();
+        // R3: dX3 = dH3 W3 ;  dW3 += dH3^T X3
+        wgmma_fence();
 #pragma unroll
-                for (int j = 0; j < 16; ++j) atomicAdd(grad_w + (NGP_MLP_W1 + NGP_MLP_W2 + NGP_MLP_W3) + m * 64 + g * 16 + j, v[j]);
-        }
-        // dW1 [64 out x 32 in], dW3 [64 out x 32 in]
+        for (int kk = 0; kk < 4; ++kk) wgmma_rs_n32<1>(a32, f[kk], desc_mnmajor(aW3, 32, kk), kk > 0 ? 1u : 0u);
 #pragma unroll
-        for (int g = 0; g < 2; ++g) {
-            tmem_ld16(tmem_row + kColDW1 + g * 16, v);
-            if (has_row) chk();
-            if (has_row)
+        for (int kk = 0; kk < 4; ++kk) wgmma_ss_n32<1, 1>(gW3, desc_mnmajor(aDH3, 64, kk), desc_mnmajor(aX3, 32, kk), 1u);
+        wgmma_commit();
+        wgmma_wait_all();
+        // dh = dX3[:, 16:32] (+ TruncExp backward on h[:,0], networks.py:26-30), fp16
+        if (t == 0) {
 #pragma unroll
-                for (int j = 0; j < 16; ++j) atomicAdd(grad_w + m * 32 + g * 16 + j, v[j]);
-            tmem_ld16(tmem_row + kColDW3 + g * 16, v);
-            if (has_row) chk();
-            if (has_row)
-#pragma unroll
-                for (int j = 0; j < 16; ++j) atomicAdd(grad_w + (NGP_MLP_W1 + NGP_MLP_W2) + m * 32 + g * 16 + j, v[j]);
-        }
-        // dW2^T [64 in x 16 out] -> W2 is [16 out x 64 in]
-        tmem_ld16(tmem_row + kColDW2T, v);
-        if (has_row) chk();
-        if (has_row)
-#pragma unroll
-            for (int j = 0; j < 16; ++j) atomicAdd(grad_w + NGP_MLP_W1 + j * 64 + m, v[j]);
-        // dW5^T [64 in x 16 (3 used)] -> W5 is [3 out x 64 in]
-        tmem_ld16(tmem_row + kColDW5T, v);
-        if (has_row) chk();   // columns 3..15 hold products with the zero padding of dO: finite unless dO is not
-        if (has_row)
-#pragma unroll
-            for (int j = 0; j < 3; ++j) atomicAdd(grad_w + (NGP_MLP_W1 + NGP_MLP_W2 + NGP_MLP_W3 + NGP_MLP_W4) + j * 64 + m, v[j]);
-        if (bad && found_inf != nullptr) *found_inf = 1;
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) tmem_dealloc(tmem_base, kTmemColsBwd);
-}
-
-// =====================================================================================================
-// Backward v2 — fp16 embeddings + saved activations, i.e. the training hot path.  The same MMAs and epilogues as
-// mlp_bwd_kernel on a different schedule.  What limits that kernel is not the tensor pipe (22 %), shared memory or
-// issue slots but the ISSUE of its 62 tiny MMAs per tile by one thread: ~90 cycles per tcgen05.mma when a single
-// active lane builds the descriptors in ordinary registers (every 32-bit half goes through R2UR), 5.6 k cycles per
-// tile, with the whole CTA waiting at a barrier for that thread in each of the 8 rounds
-// (profiles/r2_mlp_bwd_v2_trace_single_thread_issue.txt).  Here:
-//   * ONE persistent CTA per SM runs THREE tile slots (64 KB each), each owned by its own warpgroup (one thread per
-//     sample row).  The sigma-net recompute (E -> H1) is moved behind the rgb-net rounds so that six buffers per slot
-//     suffice, and no buffer is overwritten before a full round has passed since its last asynchronous reader was
-//     issued — nothing on the dependent chain ever waits for a weight-gradient MMA;
-//   * a slot's dX / recompute MMAs (22 per tile) are issued by the slot's own warp 0 right behind a 128-thread named
-//     barrier: a CONVERGED warp, one elected lane, descriptors fetched from constant memory straight into uniform
-//     registers (LDCU -> UTCHMMA, ~3 instructions per MMA): no hand-off to another warp on the chain
-//     epilogue -> MMA -> commit -> epilogue;
-//   * the weight-gradient MMAs (40 per tile, M = 64, K = the tile's 128 samples) are issued by a separate warp for all
-//     slots; only this warp touches the weight-gradient accumulators.  Slots hand it their operands through
-//     mbarriers rdw[s][2] and learn through dwb[s][2] (tcgen05.commit) that an operand may be overwritten; two
-//     requests per slot may be outstanding, hence the two alternating barriers (a parity-tracked mbarrier must not be
-//     two phases ahead of its waiter).
-//
-//   round  dX / recompute MMA   weight-gradient MMA (background)   epilogue writes                     waits for (besides D)
-//   L3     D = X3 W3^T                                             H3 = relu(D)          -> H3buf      dW1 of the previous tile
-//   L4     D = H3 W4^T                                             H4 = relu(D)          -> H4buf
-//   R1     D = dO W5            dW5^T += H4^T dO                   dH4 = D relu'(H4)     -> dH4buf
-//   R2     D = dH4 W4           dW4 += dH4^T H3                    dH3 = D relu'(H3)     -> H4buf      dW5^T (H4buf)
-//   R3     D = dH3 W3           dW3 += dH3^T X3                    dh -> DHbuf ; E       -> H3buf      dW4 (H3buf, dH4buf)
-//   L1     D = E W1^T                                              H1 = relu(D)          -> dH4buf
-//   R4     D = dh W2            dW2^T += H1^T dh                   dH1 = D relu'(H1)     -> H4buf      dW3 (H4buf, X3buf)
-//   R5     D = dH1 W1           dW1 += dH1^T E                     dE -> global                        dW2^T (dH4buf, DHbuf)
-//
-// Measured (1.71 M samples, profiles/r2_time_mlp_bwd_v2.txt): 312 us (v1) -> 249 us, bit-identical dL/dE, weight
-// gradients equal up to the order of the fp32 sums; per-round clock trace: profiles/r2_mlp_bwd_v2_trace_3slots.txt.
-constexpr int kSlotsB = 3;
-constexpr int kThreadsB2 = kSlotsB * 128 + 32;   // 416: three slot warpgroups + the weight-gradient issue warp
-constexpr int kIssuerB2 = kSlotsB * 4;           // warp 12
-constexpr int kSX3 = 0;                          // [SH | h]                          [128 x 32]
-constexpr int kSH3 = kSX3 + kB32;                // H3 -> E ([128 x 32])              [128 x 64]
-constexpr int kSH4 = kSH3 + kB64;                // H4 -> dH3 -> dH1                  [128 x 64]
-constexpr int kSD4 = kSH4 + kB64;                // dH4 -> H1                         [128 x 64]
-constexpr int kSDO = kSD4 + kB64;                // dL/do (3 of 16)                   [128 x 16]
-constexpr int kSDH = kSDO + kB16;                // dL/dh                             [128 x 16]
-constexpr int kSlotBytes = kSDH + kB16;          // 65,536
-constexpr int kBarB2 = kAct + kSlotsB * kSlotBytes;            // acc[3], rdw[3][2], dwb[3][2], fin, tmem base
-constexpr int kSmemB2 = kBarB2 + 8 * (5 * kSlotsB + 1) + 16;   // 217,232 B -> 1 CTA / SM
-constexpr uint32_t kTmemColsB2 = 512;
-constexpr uint32_t kDWB = kSlotsB * 64;          // weight-gradient accumulators behind the tile accumulators
-constexpr uint32_t kB2DW4 = kDWB, kB2DW1 = kDWB + 64, kB2DW3 = kDWB + 96, kB2DW2T = kDWB + 128, kB2DW5T = kDWB + 144;
-
-#ifdef NGP_MLP_TRACE
-// per-round clock trace of CTA 0, tiles j = 1, 2 of every slot (scripts/mlp_bwd_trace.py)
-__device__ long long g_bwd_iss[4 * 2 * 8 * 2];   // (slot index < kSlotsB)   // [slot][j-1][round][weight-gradient issue: operands ready, issued]
-__device__ long long g_bwd_wrk[4 * 2 * 8 * 3];   // [slot][j-1][round][acc wait done, epilogue done, dX MMA issued]
-#define NGP_BTR_I(s_, j_, l_, k_)                                                                  \
-    do {                                                                                           \
-        if (blockIdx.x == 0 && (threadIdx.x & 31) == 0 && (j_) >= 1 && (j_) <= 2)                  \
-            g_bwd_iss[(((s_) * 2 + ((j_) - 1)) * 8 + (l_)) * 2 + (k_)] = clock64();                \
-    } while (0)
-#define NGP_BTR_W(s_, j_, l_, k_)                                                                  \
-    do {                                                                                           \
-        if (blockIdx.x == 0 && row == 0 && (j_) >= 1 && (j_) <= 2)                                 \
-            g_bwd_wrk[(((s_) * 2 + ((j_) - 1)) * 8 + (l_)) * 3 + (k_)] = clock64();                \
-    } while (0)
-#else
-#define NGP_BTR_I(s_, j_, l_, k_) ((void)0)
-#define NGP_BTR_W(s_, j_, l_, k_) ((void)0)
-#endif
-
-// one-thread-per-row epilogues of backward v2: all 64 accumulator columns of the row are requested from tensor
-// memory at once (one tcgen05.wait::ld instead of two dependent round trips)
-__device__ __forceinline__ void tmem_ld64(uint32_t taddr, uint32_t r[64]) {
-    tmem_ld16_issue(taddr, r);
-    tmem_ld16_issue(taddr + 16, r + 16);
-    tmem_ld16_issue(taddr + 32, r + 32);
-    tmem_ld16_issue(taddr + 48, r + 48);
-    tmem_ld_wait();
-}
-__device__ __forceinline__ void epilogue_hidden64(uint32_t tmem_row, uint8_t* dst, int row) {
-    uint32_t r[64];
-    tmem_ld64(tmem_row, r);
-#pragma unroll
-    for (int kc = 0; kc < 8; ++kc) {
-        const uint32_t* q = r + kc * 8;
-        *reinterpret_cast<uint4*>(dst + chunk_off(row, kc, 64)) =
-            make_uint4(pack_h2_relu(__uint_as_float(q[0]), __uint_as_float(q[1])),
-                       pack_h2_relu(__uint_as_float(q[2]), __uint_as_float(q[3])),
-                       pack_h2_relu(__uint_as_float(q[4]), __uint_as_float(q[5])),
-                       pack_h2_relu(__uint_as_float(q[6]), __uint_as_float(q[7])));
-    }
-}
-// dst = fp16(D) masked by relu'(act) (act = the post-ReLU forward activation of this row); dst may alias act
-__device__ __forceinline__ void epilogue_relu_bwd64(uint32_t tmem_row, const uint8_t* act, uint8_t* dst, int row) {
-    uint4 a[8];
-#pragma unroll
-    for (int kc = 0; kc < 8; ++kc) a[kc] = *reinterpret_cast<const uint4*>(act + chunk_off(row, kc, 64));
-    uint32_t r[64];
-    tmem_ld64(tmem_row, r);
-#pragma unroll
-    for (int kc = 0; kc < 8; ++kc) {
-        const uint32_t aw[4] = {a[kc].x, a[kc].y, a[kc].z, a[kc].w};
-        uint32_t o[4];
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-            const __half2 ah = *reinterpret_cast<const __half2*>(&aw[j]);
-            o[j] = pack_h2(__uint_as_float(r[kc * 8 + 2 * j]), __uint_as_float(r[kc * 8 + 2 * j + 1])) &
-                   __hgt2_mask(ah, __float2half2_rn(0.0f));
-        }
-        *reinterpret_cast<uint4*>(dst + chunk_off(row, kc, 64)) = make_uint4(o[0], o[1], o[2], o[3]);
-    }
-}
-
-struct RowInB {          // one thread = one sample row
-    uint4 e[4];          // embedding row (32 fp16)
-    float dx, dy, dz, dsig, dr[3];
-    uint4 hs[2];         // saved h (16 fp16)
-    uint2 rgb;           // saved fp16 rgb
-};
-__device__ __forceinline__ RowInB load_row_b(const __half* __restrict__ emb, const float* __restrict__ dirs,
-                                             const float* __restrict__ dsigmas, const __half* __restrict__ drgbs,
-                                             const __half* __restrict__ save, int64_t n_max, int64_t i, bool valid) {
-    RowInB r;
-#pragma unroll
-    for (int q = 0; q < 4; ++q) r.e[q] = make_uint4(0, 0, 0, 0);
-    r.hs[0] = r.hs[1] = make_uint4(0, 0, 0, 0);
-    r.rgb = make_uint2(0, 0);
-    r.dx = 0.f; r.dy = 0.f; r.dz = 1.f; r.dsig = 0.f; r.dr[0] = r.dr[1] = r.dr[2] = 0.f;
-    if (valid) {
-#pragma unroll
-        for (int q = 0; q < 4; ++q) r.e[q] = __ldg(reinterpret_cast<const uint4*>(emb + i * 32) + q);
-        r.dx = __ldg(dirs + i * 3 + 0);
-        r.dy = __ldg(dirs + i * 3 + 1);
-        r.dz = __ldg(dirs + i * 3 + 2);
-        r.dsig = __ldg(dsigmas + i);
-#pragma unroll
-        for (int c = 0; c < 3; ++c) r.dr[c] = __half2float(drgbs[i * 3 + c]);
-        r.hs[0] = __ldg(reinterpret_cast<const uint4*>(save + i * 16));
-        r.hs[1] = __ldg(reinterpret_cast<const uint4*>(save + i * 16) + 1);
-        r.rgb = __ldg(reinterpret_cast<const uint2*>(save_rgb_ptr(save, n_max) + i * 4));
-    }
-    return r;
-}
-
-// Every MMA of a tile has fixed operands (slot buffers + weights).  Its two 64-bit shared-memory descriptors live in
-// CONSTANT memory (filled by the host once, from the kernel's shared-memory base address): with compile-time indices
-// they are fetched straight into uniform registers (ULDC), so issuing an MMA costs a handful of instructions instead
-// of the ~35 dependent integer ops + four R2UR moves of descriptors built in ordinary registers.
-constexpr int kOpsPerTile = 62;
-__constant__ ulonglong2 c_b2_desc[kSlotsB][kOpsPerTile];
-// table offsets: L3 0 (2), L4 2 (4), dW5^T 6 (8), R1 14 (1), dW4 15 (8), R2 23 (4), R3 27 (4), dW3 31 (8), L1 39 (2),
-//                dW2^T 41 (8), R4 49 (1), R5 50 (4), dW1 54 (8)
-inline void build_b2_desc_table(uint32_t smem0, ulonglong2 (*tab)[kOpsPerTile]) {
-    for (int s = 0; s < kSlotsB; ++s) {
-        const uint32_t sb = smem0 + kAct + s * kSlotBytes;
-        const uint32_t aX3 = sb + kSX3, aH3 = sb + kSH3, aH4 = sb + kSH4, aD4 = sb + kSD4, aDO = sb + kSDO, aDH = sb + kSDH;
-        const uint32_t aW1 = smem0 + kW1, aW2 = smem0 + kW2, aW3 = smem0 + kW3, aW4 = smem0 + kW4, aW5 = smem0 + kW5;
-        int o = 0;
-        auto put = [&](const Operand& a, const Operand& b, int ksteps) {
-            for (int k = 0; k < ksteps; ++k) {
-                tab[s][o].x = smem_desc(a.addr + k * a.kstep, a.lbo, a.sbo);
-                tab[s][o].y = smem_desc(b.addr + k * b.kstep, b.lbo, b.sbo);
-                ++o;
-            }
-        };
-        put(op_kmajor(aX3, 32), op_kmajor(aW3, 32), 2);       // L3   D = X3 W3^T
-        put(op_kmajor(aH3, 64), op_kmajor(aW4, 64), 4);       // L4   D = H3 W4^T
-        put(op_mnmajor(aH4, 64), op_mnmajor(aDO, 16), 8);     //      dW5^T += H4^T dO
-        put(op_kmajor(aDO, 16), op_mnmajor(aW5, 64), 1);      // R1   D = dO W5
-        put(op_mnmajor(aD4, 64), op_mnmajor(aH3, 64), 8);     //      dW4 += dH4^T H3
-        put(op_kmajor(aD4, 64), op_mnmajor(aW4, 64), 4);      // R2   D = dH4 W4
-        put(op_kmajor(aH4, 64), op_mnmajor(aW3, 32), 4);      // R3   D = dH3 W3          (dH3 in H4buf)
-        put(op_mnmajor(aH4, 64), op_mnmajor(aX3, 32), 8);     //      dW3 += dH3^T X3
-        put(op_kmajor(aH3, 32), op_kmajor(aW1, 32), 2);       // L1   D = E W1^T          (E in H3buf)
-        put(op_mnmajor(aD4, 64), op_mnmajor(aDH, 16), 8);     //      dW2^T += H1^T dh    (H1 in dH4buf)
-        put(op_kmajor(aDH, 16), op_mnmajor(aW2, 64), 1);      // R4   D = dh W2
-        put(op_kmajor(aH4, 64), op_mnmajor(aW1, 32), 4);      // R5   D = dH1 W1          (dH1 in H4buf)
-        put(op_mnmajor(aH4, 64), op_mnmajor(aH3, 32), 8);     //      dW1 += dH1^T E
-    }
-}
-template <int S, int O, int CNT>
-__device__ __forceinline__ void issue_tab(uint32_t tmem_d, uint32_t idesc, uint32_t acc0) {   // whole warp, converged
-#pragma unroll
-    for (int k = 0; k < CNT; ++k) {
-        const ulonglong2 ab = c_b2_desc[S][O + k];
-        umma_f16_w(tmem_d, ab.x, ab.y, idesc, k > 0 ? 1u : acc0);
-    }
-}
-
-// the dX / recompute MMAs of round L for slot S; whole warp
-template <int S, int L>
-__device__ __forceinline__ void issue_dx(uint32_t tmem_base, uint32_t bar_acc) {
-    const uint32_t D = tmem_base + (uint32_t)S * 64u;
-    if constexpr (L == 0) issue_tab<S, 0, 2>(D, idesc_f16(kTile, 64), 0u);
-    if constexpr (L == 1) issue_tab<S, 2, 4>(D, idesc_f16(kTile, 64), 0u);
-    if constexpr (L == 2) issue_tab<S, 14, 1>(D, idesc_full(128, 64, 0, 1), 0u);
-    if constexpr (L == 3) issue_tab<S, 23, 4>(D, idesc_full(128, 64, 0, 1), 0u);
-    if constexpr (L == 4) issue_tab<S, 27, 4>(D, idesc_full(128, 32, 0, 1), 0u);
-    if constexpr (L == 5) issue_tab<S, 39, 2>(D, idesc_f16(kTile, 64), 0u);
-    if constexpr (L == 6) issue_tab<S, 49, 1>(D, idesc_full(128, 64, 0, 1), 0u);
-    if constexpr (L == 7) issue_tab<S, 50, 4>(D, idesc_full(128, 32, 0, 1), 0u);
-    umma_commit_w(bar_acc);
-}
-template <int L>
-__device__ __forceinline__ void issue_dx_slot(int s, uint32_t tmem_base, uint32_t bar_acc) {
-    static_assert(kSlotsB == 3, "one case per slot");
-    switch (s) {   // warp-uniform
-    case 0: issue_dx<0, L>(tmem_base, bar_acc); break;
-    case 1: issue_dx<1, L>(tmem_base, bar_acc); break;
-    default: issue_dx<2, L>(tmem_base, bar_acc); break;
-    }
-}
-// weight-gradient MMA number I (0: dW5^T, 1: dW4, 2: dW3, 3: dW2^T, 4: dW1) of slot S; whole warp
-template <int S, int I>
-__device__ __forceinline__ void issue_dw(uint32_t tmem_base, uint32_t accumulate, uint32_t bar_dwb) {
-    if constexpr (I == 0) issue_tab<S, 6, 8>(tmem_base + kB2DW5T, idesc_full(64, 16, 1, 1), accumulate);
-    if constexpr (I == 1) issue_tab<S, 15, 8>(tmem_base + kB2DW4, idesc_full(64, 64, 1, 1), accumulate);
-    if constexpr (I == 2) issue_tab<S, 31, 8>(tmem_base + kB2DW3, idesc_full(64, 32, 1, 1), accumulate);
-    if constexpr (I == 3) issue_tab<S, 41, 8>(tmem_base + kB2DW2T, idesc_full(64, 16, 1, 1), accumulate);
-    if constexpr (I == 4) issue_tab<S, 54, 8>(tmem_base + kB2DW1, idesc_full(64, 32, 1, 1), accumulate);
-    umma_commit_w(bar_dwb);
-}
-
-__device__ __forceinline__ void named_barrier_128(int id) {   // the four warps of one slot
-    asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory");
-}
-
-__global__ void __launch_bounds__(kThreadsB2, 1)
-mlp_bwd_v2_kernel(const __half* __restrict__ emb, const float* __restrict__ dirs, ngp_mlp_weights w,
-                  const __half* __restrict__ save, const float* __restrict__ dsigmas, const __half* __restrict__ drgbs,
-                  __half* __restrict__ demb, float* __restrict__ grad_w, int64_t n_max, const int32_t* __restrict__ n_dev,
-                  int32_t* __restrict__ found_inf, uint32_t* __restrict__ probe_smem_base) {
-    extern __shared__ __align__(128) uint8_t smem[];
-    if (probe_smem_base != nullptr) {   // set-up launch: where this kernel's dynamic shared memory starts
-        if (threadIdx.x == 0) *probe_smem_base = smem_u32(smem);
-        return;
-    }
-    const int64_t n = n_dev ? min(n_max, max((int64_t)*n_dev, (int64_t)0)) : n_max;
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-
-    stage_weight(smem + kW1, w.w1, 64, 64, 32, kThreadsB2);
-    stage_weight(smem + kW2, w.w2, 16, 16, 64, kThreadsB2);
-    stage_weight(smem + kW3, w.w3, 64, 64, 32, kThreadsB2);
-    stage_weight(smem + kW4, w.w4, 64, 64, 64, kThreadsB2);
-    stage_weight(smem + kW5, w.w5, 3, 16, 64, kThreadsB2);
-    const uint32_t smem0 = smem_u32(smem);
-    const uint32_t bar0 = smem0 + kBarB2;
-    // Weight-gradient MMA number m of a slot (m = 5 * tile + kind) uses request barrier rdw[s][m & 1] and completion
-    // barrier dwb[s][m & 1], in their phase (m >> 1) & 1: a slot may have TWO requests (and two completions)
-    // outstanding, and a single parity-tracked barrier cannot be two phases ahead of its waiter.  It never has three:
-    // request m + 2 is only made after completion m has been waited for.
-    auto bar_acc = [&](int s) { return bar0 + 8u * (uint32_t)s; };                             // dX MMA of the round done
-    auto bar_rdw = [&](int s, int b) { return bar0 + 8u * (uint32_t)(kSlotsB + 2 * s + b); };       // operands written
-    auto bar_dwb = [&](int s, int b) { return bar0 + 8u * (uint32_t)(3 * kSlotsB + 2 * s + b); };   // dW MMA done
-    const uint32_t bar_fin = bar0 + 8u * (uint32_t)(5 * kSlotsB);
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + kBarB2 + 8 * (5 * kSlotsB + 1));
-    if (tid == 0) {
-        for (int s = 0; s < kSlotsB; ++s) {
-            mbar_init(bar_acc(s), 1);
-            for (int b = 0; b < 2; ++b) {
-                mbar_init(bar_rdw(s, b), 128);
-                mbar_init(bar_dwb(s, b), 1);
+            for (int k = 0; k < 2; ++k) {
+                const float ds = r16(dsig[k] * expf(fminf(fmaxf(h0[k], -15.0f), 15.0f)));
+                a32[8 + 2 * k] = r16(a32[8 + 2 * k]) + ds;
             }
         }
-        mbar_init(bar_fin, 1);
-        fence_barrier_init();
-    }
-    if (warp == kIssuerB2) tmem_alloc(smem_u32(tmem_slot), kTmemColsB2);
-    fence_proxy_async();
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-
-    const int64_t n_tiles = (n + kTile - 1) / kTile;
-    const int64_t G = gridDim.x;
-    // tile j of slot s (this CTA): blockIdx.x + (kSlotsB * j + s) * G
-    auto slot_count = [&](int s) -> int64_t {
-        const int64_t first = (int64_t)blockIdx.x + s * G;
-        return first < n_tiles ? (n_tiles - 1 - first) / (kSlotsB * G) + 1 : 0;
-    };
-
-    if (warp == kIssuerB2) {
-        // ============ weight-gradient MMA issue: the whole warp, converged; one elected lane issues ============
-        const int64_t c0 = slot_count(0), c1 = slot_count(1), c2 = slot_count(2);
-        static_assert(kSlotsB == 3, "slot counts are held in three scalars");
-        // Requests are served in a fixed order (MMA kind, then slot): everything — slot, kind, hence every
-        // descriptor's address in constant memory — is then a compile-time constant of fully unrolled code.  No slot
-        // waits for such an MMA less than a full round after asking for it, so the order costs nothing.
-        for (int64_t j = 0; j < c0; ++j) {   // slot 0 starts first: it has at least as many tiles as any other
+        uint32_t dhf[4];
 #pragma unroll
-            for (int i = 0; i < 5; ++i) {
+        for (int q = 0; q < 4; ++q) dhf[q] = pack_h2(a32[8 + 2 * q], a32[9 + 2 * q]);
+        store_frag(smem + kDH, 16, 0, dhf, r0, t);
+        fence_proxy_async();
+        __syncthreads();
+        // R4: dH1pre = dh W2 ;  dW2^T += H1^T dh
+        wgmma_fence();
+        wgmma_rs_n64<1>(acc, dhf, desc_mnmajor(aW2, 64, 0), 0u);
 #pragma unroll
-                for (int s = 0; s < kSlotsB; ++s) {
-                    if (j >= (s == 0 ? c0 : s == 1 ? c1 : c2)) continue;
-                    const int64_t m = 5 * j + i;              // this slot's MMA number
-                    const int mb = (int)(m & 1);
-                    mbar_wait_bounded(bar_rdw(s, mb), (uint32_t)((m >> 1) & 1));
-                    tc_fence_after();
-                    [[maybe_unused]] constexpr int kRoundOf[5] = {2, 3, 4, 6, 7};
-                    NGP_BTR_I(s, j, kRoundOf[i], 0);
-                    // an accumulator is first written by slot 0's first tile (slot 0 leads every pass of this loop)
-                    const uint32_t accumulate = (s > 0 || j > 0) ? 1u : 0u;
-                    if (s == 0) {
-                        if (i == 0) issue_dw<0, 0>(tmem_base, accumulate, bar_dwb(0, mb));
-                        if (i == 1) issue_dw<0, 1>(tmem_base, accumulate, bar_dwb(0, mb));
-                        if (i == 2) issue_dw<0, 2>(tmem_base, accumulate, bar_dwb(0, mb));
-                        if (i == 3) issue_dw<0, 3>(tmem_base, accumulate, bar_dwb(0, mb));
-                        if (i == 4) issue_dw<0, 4>(tmem_base, accumulate, bar_dwb(0, mb));
-                    } else if (s == 1) {
-                        if (i == 0) issue_dw<1, 0>(tmem_base, accumulate, bar_dwb(1, mb));
-                        if (i == 1) issue_dw<1, 1>(tmem_base, accumulate, bar_dwb(1, mb));
-                        if (i == 2) issue_dw<1, 2>(tmem_base, accumulate, bar_dwb(1, mb));
-                        if (i == 3) issue_dw<1, 3>(tmem_base, accumulate, bar_dwb(1, mb));
-                        if (i == 4) issue_dw<1, 4>(tmem_base, accumulate, bar_dwb(1, mb));
-                    } else {
-                        if (i == 0) issue_dw<2, 0>(tmem_base, accumulate, bar_dwb(2, mb));
-                        if (i == 1) issue_dw<2, 1>(tmem_base, accumulate, bar_dwb(2, mb));
-                        if (i == 2) issue_dw<2, 2>(tmem_base, accumulate, bar_dwb(2, mb));
-                        if (i == 3) issue_dw<2, 3>(tmem_base, accumulate, bar_dwb(2, mb));
-                        if (i == 4) issue_dw<2, 4>(tmem_base, accumulate, bar_dwb(2, mb));
-                    }
-                    NGP_BTR_I(s, j, kRoundOf[i], 1);
+        for (int kk = 0; kk < 4; ++kk) wgmma_ss_n16<1, 1>(gW2T, desc_mnmajor(aH1, 64, kk), desc_mnmajor(aDH, 16, kk), 1u);
+        wgmma_commit();
+        wgmma_wait_all();
+        relu_bwd_frags(acc, smem + kH1, smem + kDH1, r0, t, f);
+        fence_proxy_async();
+        __syncthreads();
+        // R5: dE = dH1 W1 ;  dW1 += dH1^T E
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) wgmma_rs_n32<1>(a32, f[kk], desc_mnmajor(aW1, 32, kk), kk > 0 ? 1u : 0u);
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) wgmma_ss_n32<1, 1>(gW1, desc_mnmajor(aDH1, 64, kk), desc_mnmajor(aE, 32, kk), 1u);
+        wgmma_commit();
+        wgmma_wait_all();
+#pragma unroll
+        for (int k = 0; k < 2; ++k) {
+            if (!vv[k]) continue;
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                const float a = a32[4 * j + 2 * k], b = a32[4 * j + 2 * k + 1];
+                if constexpr (sizeof(TEmb) == 2) {
+                    *reinterpret_cast<uint32_t*>(demb + ii[k] * 32 + 8 * j + 2 * t) = pack_h2(a, b);
+                } else {   // fp16-rounded like the autocast graph, stored as fp32
+                    *reinterpret_cast<float2*>(demb + ii[k] * 32 + 8 * j + 2 * t) = make_float2(r16(a), r16(b));
                 }
             }
         }
-        umma_commit_w(bar_fin);   // every weight-gradient MMA of this CTA has completed when this arrives
-        __syncwarp();
-    } else {
-        // ======================= slot warpgroup: one thread per sample row =======================
-        const int s = warp >> 2, row = tid & 127;
-        const bool issuer = (warp & 3) == 0;         // warp 0 of the slot issues the slot's dX / recompute MMAs
-        uint8_t* sb = smem + kAct + s * kSlotBytes;
-        const uint32_t tmem_row = tmem_base + (uint32_t)s * 64u + ((uint32_t)((warp & 3) * 32) << 16);
-        const uint32_t acc = bar_acc(s);
-        uint32_t acc_phase = 0;
-        uint32_t m_hand = 0, m_wait = 0;   // weight-gradient MMAs of this slot requested / waited for so far
-        [[maybe_unused]] int64_t jt = 0;   // tile counter of this slot (trace builds)
-        // operands of round L are in shared memory and D has been read: barrier over the slot's 128 threads, then
-        // warp 0 issues round L's MMA; everybody waits for its commit
-#define NGP_B2_ROUND(L)                                   \
-        fence_proxy_async();                              \
-        tc_fence_before();                                \
-        named_barrier_128(1 + s);                         \
-        if (issuer) {                                     \
-            tc_fence_after();                             \
-            issue_dx_slot<L>(s, tmem_base, acc);   \
-        }                                                 \
-        NGP_BTR_W(s, jt, L, 2);                           \
-        mbar_wait_bounded(acc, acc_phase);                \
-        acc_phase ^= 1;                                   \
-        tc_fence_after();                                 \
-        NGP_BTR_W(s, jt, L, 0);
-        auto hand_to_dw = [&]() {   // (after fence_proxy_async + tc_fence_before of the round) operands of a dW MMA
-            mbar_arrive(bar_rdw(s, (int)(m_hand & 1u)));
-            ++m_hand;
-        };
-        auto wait_dw = [&]() {      // the oldest outstanding dW MMA of this slot has completed
-            mbar_wait_bounded(bar_dwb(s, (int)(m_wait & 1u)), (m_wait >> 1) & 1u);
-            ++m_wait;
-            tc_fence_after();
-        };
-        int64_t tile = (int64_t)blockIdx.x + s * G;
-        RowInB cur = load_row_b(emb, dirs, dsigmas, drgbs, save, n_max, tile * kTile + row,
-                                tile < n_tiles && tile * kTile + row < n);
-        bool dw1_pending = false;   // dW1 of the previous tile (reads H3buf, H4buf) not yet known to be done
-        for (; tile < n_tiles; tile += kSlotsB * G) {
-            const int64_t i = tile * kTile + row;
-            const bool valid = i < n;
-            const uint4 e0 = cur.e[0], e1 = cur.e[1], e2 = cur.e[2], e3 = cur.e[3];
-            const float dsig = cur.dsig;
-            const float h0 = __low2float(*reinterpret_cast<const __half2*>(&cur.hs[0].x));
-            {   // X3 = [SH((d/|d| + 1)/2) | h],  dL/do = dL/drgb * rgb (1 - rgb) in fp16 like the autocast graph
-                const float inv = 1.0f / sqrtf(cur.dx * cur.dx + cur.dy * cur.dy + cur.dz * cur.dz);
-                float sh[16];
-                sh16((cur.dx * inv + 1.0f) / 2.0f, (cur.dy * inv + 1.0f) / 2.0f, (cur.dz * inv + 1.0f) / 2.0f, sh);
-                uint8_t* x3 = sb + kSX3;
-                *reinterpret_cast<uint4*>(x3 + chunk_off(row, 0, 32)) =
-                    make_uint4(pack_h2(sh[0], sh[1]), pack_h2(sh[2], sh[3]), pack_h2(sh[4], sh[5]), pack_h2(sh[6], sh[7]));
-                *reinterpret_cast<uint4*>(x3 + chunk_off(row, 1, 32)) =
-                    make_uint4(pack_h2(sh[8], sh[9]), pack_h2(sh[10], sh[11]), pack_h2(sh[12], sh[13]), pack_h2(sh[14], sh[15]));
-                *reinterpret_cast<uint4*>(x3 + chunk_off(row, 2, 32)) = cur.hs[0];
-                *reinterpret_cast<uint4*>(x3 + chunk_off(row, 3, 32)) = cur.hs[1];
-                const __half2 a = *reinterpret_cast<const __half2*>(&cur.rgb.x);
-                const __half2 b = *reinterpret_cast<const __half2*>(&cur.rgb.y);
-                const float rgbv[3] = {__low2float(a), __high2float(a), __low2float(b)};
-                float d_o[3];
-#pragma unroll
-                for (int c = 0; c < 3; ++c) d_o[c] = cur.dr[c] * rgbv[c] * (1.0f - rgbv[c]);
-                *reinterpret_cast<uint4*>(sb + kSDO + chunk_off(row, 0, 16)) =
-                    make_uint4(pack_h2(d_o[0], d_o[1]), pack_h2(d_o[2], 0.0f), 0u, 0u);
-                *reinterpret_cast<uint4*>(sb + kSDO + chunk_off(row, 1, 16)) = make_uint4(0u, 0u, 0u, 0u);
-            }
-            NGP_B2_ROUND(0)                                              // L3: D = X3 W3^T
-            if (dw1_pending) wait_dw();                                  // dW1 of the previous tile read H3buf / H4buf
-            epilogue_hidden64(tmem_row, sb + kSH3, row);
-            NGP_BTR_W(s, jt, 0, 1);
-            NGP_B2_ROUND(1)                                              // L4: D = H3 W4^T
-            epilogue_hidden64(tmem_row, sb + kSH4, row);
-            NGP_BTR_W(s, jt, 1, 1);
-            NGP_B2_ROUND(2)                                              // R1: D = dO W5
-            hand_to_dw();                                                //     dW5^T += H4^T dO        (background)
-            epilogue_relu_bwd64(tmem_row, sb + kSH4, sb + kSD4, row);   //     dH4 = D relu'(H4) -> dH4buf
-            NGP_BTR_W(s, jt, 2, 1);
-            NGP_B2_ROUND(3)                                              // R2: D = dH4 W4
-            hand_to_dw();                                                //     dW4 += dH4^T H3         (background)
-            wait_dw();                                                   //     dW5^T done: H4buf is free
-            epilogue_relu_bwd64(tmem_row, sb + kSH3, sb + kSH4, row);   //     dH3 = D relu'(H3) -> H4buf
-            NGP_BTR_W(s, jt, 3, 1);
-            NGP_B2_ROUND(4)                                              // R3: D = dH3 W3
-            hand_to_dw();                                                //     dW3 += dH3^T X3         (background)
-            wait_dw();                                                   //     dW4 done: H3buf and dH4buf are free
-            {
-                float g[16];
-                tmem_ld16(tmem_row + 16, g);                             // D[:, 16:32] = dL/dh from the rgb net
-                // + TruncExp backward on h[:,0] (networks.py:26-30), fp16
-                const float ds = __half2float(__float2half_rn(dsig * expf(fminf(fmaxf(h0, -15.0f), 15.0f))));
-                g[0] = __half2float(__float2half_rn(g[0])) + ds;
-                *reinterpret_cast<uint4*>(sb + kSDH + chunk_off(row, 0, 16)) =
-                    make_uint4(pack_h2(g[0], g[1]), pack_h2(g[2], g[3]), pack_h2(g[4], g[5]), pack_h2(g[6], g[7]));
-                *reinterpret_cast<uint4*>(sb + kSDH + chunk_off(row, 1, 16)) =
-                    make_uint4(pack_h2(g[8], g[9]), pack_h2(g[10], g[11]), pack_h2(g[12], g[13]), pack_h2(g[14], g[15]));
-            }
-            *reinterpret_cast<uint4*>(sb + kSH3 + chunk_off(row, 0, 32)) = e0;   // E for the sigma-net recompute
-            *reinterpret_cast<uint4*>(sb + kSH3 + chunk_off(row, 1, 32)) = e1;
-            *reinterpret_cast<uint4*>(sb + kSH3 + chunk_off(row, 2, 32)) = e2;
-            *reinterpret_cast<uint4*>(sb + kSH3 + chunk_off(row, 3, 32)) = e3;
-            {   // the next tile of this slot (its registers are free now that E is staged): three rounds ahead of use
-                const int64_t in = (tile + kSlotsB * G) * kTile + row;
-                cur = load_row_b(emb, dirs, dsigmas, drgbs, save, n_max, in, in < n);
-            }
-            NGP_BTR_W(s, jt, 4, 1);
-            NGP_B2_ROUND(5)                                              // L1: D = E W1^T
-            epilogue_hidden64(tmem_row, sb + kSD4, row);                //     H1 -> dH4buf
-            NGP_BTR_W(s, jt, 5, 1);
-            NGP_B2_ROUND(6)                                              // R4: D = dh W2
-            hand_to_dw();                                                //     dW2^T += H1^T dh        (background)
-            wait_dw();                                                   //     dW3 done: H4buf (dH3) and X3buf are free
-            epilogue_relu_bwd64(tmem_row, sb + kSD4, sb + kSH4, row);   //     dH1 = D relu'(H1) -> H4buf
-            NGP_BTR_W(s, jt, 6, 1);
-            NGP_B2_ROUND(7)                                              // R5: D = dH1 W1
-            hand_to_dw();                                                //     dW1 += dH1^T E (waited for in the next L3)
-            wait_dw();                                                   //     dW2^T done: dH4buf (H1) and DHbuf are free
-            dw1_pending = true;
-            {
-                float v[32];
-                tmem_ld32(tmem_row, v);                                  // D[:, 0:32] = dL/dE
-                if (valid) {
-                    uint4* o = reinterpret_cast<uint4*>(demb + i * 32);
-#pragma unroll
-                    for (int q = 0; q < 4; ++q)
-                        o[q] = make_uint4(pack_h2(v[8 * q], v[8 * q + 1]), pack_h2(v[8 * q + 2], v[8 * q + 3]),
-                                          pack_h2(v[8 * q + 4], v[8 * q + 5]), pack_h2(v[8 * q + 6], v[8 * q + 7]));
-                }
-            }
-            NGP_BTR_W(s, jt, 7, 1);
-            ++jt;
-        }
-#undef NGP_B2_ROUND
+        __syncthreads();   // every buffer is restaged by the next tile
     }
 
-    // ---- flush the weight-gradient accumulators (as mlp_bwd_kernel): M = 64 rows on TMEM lanes (m%16) + 32*(m/16)
-    if (warp < 4 && slot_count(0) > 0) {
-        mbar_wait_bounded(bar_fin, 0);
-        tc_fence_after();
-        const uint32_t trow = tmem_base + ((uint32_t)((warp & 3) * 32) << 16);
-        const int m = warp * 16 + lane;
-        const bool has_row = lane < 16;
-        float v[16];
-        bool bad = false;
-        auto chk = [&]() {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) bad = bad || !(fabsf(v[j]) < INFINITY);
-        };
-#pragma unroll
-        for (int g = 0; g < 4; ++g) {   // dW4 [64 out x 64 in]
-            tmem_ld16(trow + kB2DW4 + g * 16, v);
-            if (has_row) {
-                chk();
-#pragma unroll
-                for (int j = 0; j < 16; ++j) atomicAdd(grad_w + (NGP_MLP_W1 + NGP_MLP_W2 + NGP_MLP_W3) + m * 64 + g * 16 + j, v[j]);
-            }
-        }
-#pragma unroll
-        for (int g = 0; g < 2; ++g) {   // dW1, dW3 [64 out x 32 in]
-            tmem_ld16(trow + kB2DW1 + g * 16, v);
-            if (has_row) {
-                chk();
-#pragma unroll
-                for (int j = 0; j < 16; ++j) atomicAdd(grad_w + m * 32 + g * 16 + j, v[j]);
-            }
-            tmem_ld16(trow + kB2DW3 + g * 16, v);
-            if (has_row) {
-                chk();
-#pragma unroll
-                for (int j = 0; j < 16; ++j) atomicAdd(grad_w + (NGP_MLP_W1 + NGP_MLP_W2) + m * 32 + g * 16 + j, v[j]);
-            }
-        }
-        tmem_ld16(trow + kB2DW2T, v);   // dW2^T [64 in x 16 out] -> W2 is [16 out x 64 in]
-        if (has_row) {
-            chk();
-#pragma unroll
-            for (int j = 0; j < 16; ++j) atomicAdd(grad_w + NGP_MLP_W1 + j * 64 + m, v[j]);
-        }
-        tmem_ld16(trow + kB2DW5T, v);   // dW5^T [64 in x 16 (3 used)] -> W5 is [3 out x 64 in]
-        if (has_row) {
-            chk();
-#pragma unroll
-            for (int j = 0; j < 3; ++j) atomicAdd(grad_w + (NGP_MLP_W1 + NGP_MLP_W2 + NGP_MLP_W3 + NGP_MLP_W4) + j * 64 + m, v[j]);
-        }
-        if (bad && found_inf != nullptr) *found_inf = 1;
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == kIssuerB2) tmem_dealloc(tmem_base, kTmemColsB2);
-}
-
-// backward implementation for fp16 embeddings + saved activations: 0 = auto (v2), 1 = v1 (mlp_bwd_kernel), 2 = v2;
-// the environment variable NGP_MLP_BWD overrides it (A/B runs)
-int g_bwd_impl = 0;
-
-int launch_bwd_v2(const void* emb, const float* dirs, const ngp_mlp_weights* w, const void* save, const float* dsigmas,
-                  const void* drgbs, void* demb, float* grad_w, int64_t n, const int32_t* n_dev, int32_t* found_inf,
-                  cudaStream_t st) {
-    // (the descriptor table lives in constant memory, i.e. per device: one flag per device of this process)
-    static bool configured_dev[64] = {};
-    int dev_id = 0;
-    if (cudaGetDevice(&dev_id) != cudaSuccess || dev_id < 0 || dev_id >= 64) dev_id = 0;
-    if (!configured_dev[dev_id]) {
-        // the set-up below synchronises the stream: if the very first call of the process happens under stream capture,
-        // this launch uses the v1 kernel (-2) and the set-up waits for the first eager call
-        cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
-        if (cudaStreamIsCapturing(st, &cap) != cudaSuccess || cap != cudaStreamCaptureStatusNone) {
-            cudaGetLastError();
-            return -2;
-        }
-        // one-time set-up (the first launch of a process is an eager one in every warm-up):
-        // ask the kernel where its dynamic shared memory starts, build the descriptor table, upload it
-        cudaError_t e = cudaFuncSetAttribute(mlp_bwd_v2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemB2);
-        uint32_t* d_base = nullptr;
-        uint32_t h_base = 0;
-        if (e == cudaSuccess) e = cudaMalloc(&d_base, sizeof(uint32_t));
-        if (e == cudaSuccess) {
-            mlp_bwd_v2_kernel<<<1, kThreadsB2, kSmemB2, st>>>(nullptr, nullptr, *w, nullptr, nullptr, nullptr, nullptr, nullptr,
-                                                            0, nullptr, nullptr, d_base);
-            e = cudaGetLastError();
-        }
-        if (e == cudaSuccess) e = cudaMemcpyAsync(&h_base, d_base, sizeof(uint32_t), cudaMemcpyDeviceToHost, st);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-        if (e == cudaSuccess) {
-            static ulonglong2 tab[kSlotsB][kOpsPerTile];
-            build_b2_desc_table(h_base, tab);
-            e = cudaMemcpyToSymbolAsync(c_b2_desc, tab, sizeof(tab), 0, cudaMemcpyHostToDevice, st);
-        }
-        if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-        if (d_base) cudaFree(d_base);
-        if (e != cudaSuccess) {
-            cudaGetLastError();
-            ngp::set_error("mlp_bwd_v2_kernel: set-up: %s", cudaGetErrorString(e));
-            return (int)e;
-        }
-        configured_dev[dev_id] = true;
-    }
-    const int64_t n_tiles = (n + kTile - 1) / kTile;
-    const int64_t max_ctas = (int64_t)ngp::sm_count();   // 212 KB of shared memory + all 512 TMEM columns per CTA
-    const unsigned grid = (unsigned)(n_tiles < max_ctas ? n_tiles : max_ctas);
-    mlp_bwd_v2_kernel<<<grid, kThreadsB2, kSmemB2, st>>>((const __half*)emb, dirs, *w, (const __half*)save, dsigmas,
-                                                        (const __half*)drgbs, (__half*)demb, grad_w, n, n_dev,
-                                                        found_inf, nullptr);
-    NGP_LAUNCHED("mlp_bwd_v2_kernel");
-    return 0;
+    // ---- flush the weight-gradient accumulators: thread element 4j + 2k + c is (row r0 + 8k, column 8j + 2t + c)
+    if ((int64_t)blockIdx.x >= n_tiles) return;
+    bool bad = false;   // non-finite weight gradient (GradScaler's inf check, raised at the source)
+    constexpr int o2 = NGP_MLP_W1, o3 = o2 + NGP_MLP_W2, o4 = o3 + NGP_MLP_W3, o5 = o4 + NGP_MLP_W4;
+    flush_acc<64>(gW4, r0, t, bad, [&](int m, int c) { return grad_w + o4 + m * 64 + c; });
+    flush_acc<32>(gW3, r0, t, bad, [&](int m, int c) { return grad_w + o3 + m * 32 + c; });
+    flush_acc<32>(gW1, r0, t, bad, [&](int m, int c) { return grad_w + m * 32 + c; });
+    flush_acc<16>(gW2T, r0, t, bad, [&](int m, int c) { return grad_w + o2 + c * 64 + m; });   // W2 is [16 out x 64 in]
+    // W5 is [3 out x 64 in]; columns 3..7 hold products with the zero padding of dO: finite unless dO is not
+    flush_acc<8>(gW5T, r0, t, bad, [&](int m, int c) { return c < 3 ? grad_w + o5 + c * 64 + m : (float*)nullptr; });
+    if (bad && found_inf != nullptr) *found_inf = 1;
 }
 
 template <typename TEmb, bool kSaved>
 int launch_bwd(const void* emb, const float* dirs, const ngp_mlp_weights* w, const void* save, const float* dsigmas,
                const void* drgbs, void* demb, float* grad_w, int64_t n, const int32_t* n_dev, int32_t* found_inf,
                cudaStream_t st) {
-    static bool configured = false;
-    if (!configured) {
-        cudaError_t e = cudaFuncSetAttribute(mlp_bwd_kernel<TEmb, kSaved>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                             kSmemBytesBwd);
+    auto kernel = mlp_bwd_kernel<TEmb, kSaved>;
+    static int per_sm[64] = {};   // set up once per device of this process
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) dev = 0;
+    if (per_sm[dev] == 0) {
+        cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBwd);
         if (e != cudaSuccess) {
             ngp::set_error("mlp_bwd_kernel: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
             return (int)e;
         }
-        configured = true;
+        per_sm[dev] = ctas_per_sm(kernel, kSmemBwd);
     }
     const int64_t n_tiles = (n + kTile - 1) / kTile;
-    const int64_t max_ctas = (int64_t)ngp::sm_count() * 2;  // 108 KB smem + 256 TMEM columns per CTA
+    const int64_t max_ctas = (int64_t)ngp::sm_count() * per_sm[dev];
     const unsigned grid = (unsigned)(n_tiles < max_ctas ? n_tiles : max_ctas);
-    mlp_bwd_kernel<TEmb, kSaved><<<grid, kThreadsBwd, kSmemBytesBwd, st>>>((const TEmb*)emb, dirs, *w, (const __half*)save,
-                                                                       dsigmas, (const __half*)drgbs, (TEmb*)demb,
-                                                                       grad_w, n, n_dev, found_inf);
+    kernel<<<grid, kThreads, kSmemBwd, st>>>((const TEmb*)emb, dirs, *w, (const __half*)save, dsigmas,
+                                             (const __half*)drgbs, (TEmb*)demb, grad_w, n, n_dev, found_inf);
     NGP_LAUNCHED("mlp_bwd_kernel");
     return 0;
 }
 
-// forward implementation: 0 = auto (v2 where it applies), 1 = v1 (shared-memory activations), 2 = v2 (TMEM activations)
-int g_fwd_impl = 0;
-
 template <typename TEmb>
 int launch_fwd(const void* emb, const float* dirs, const ngp_mlp_weights* w, float* sigmas, void* rgbs, void* save,
                int64_t n, const int32_t* n_dev, cudaStream_t st) {
-    // the environment variable NGP_MLP_FWD overrides ngp_mlp_set_impl (A/B runs of unmodified scripts)
-    static const int env_impl = [] { const char* e = getenv("NGP_MLP_FWD"); return e ? atoi(e) : -1; }();
-    const int impl = env_impl >= 0 ? env_impl : g_fwd_impl;
-    if (sizeof(TEmb) == 2 && impl != 1) {
-        const int rc = ngp::mlp_fwd_v2_launch(emb, dirs, w, sigmas, rgbs, save, n, n_dev, st);
-        if (rc != -2) return rc;   // -2: not applicable (tiny n / no tensor-map entry point) -> v1 below
-        if (impl == 2 && n >= kTile) return -1;   // explicitly requested: do not fall back silently
-    }
-    static bool configured = false;
-    if (!configured) {
-        cudaError_t e = cudaFuncSetAttribute(mlp_fwd_kernel<TEmb>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes);
-        if (e != cudaSuccess) {
-            ngp::set_error("mlp_fwd_kernel: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
-            return (int)e;
-        }
-        configured = true;
-    }
+    auto kernel = mlp_fwd_kernel<TEmb>;
+    static int per_sm[64] = {};
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) dev = 0;
+    if (per_sm[dev] == 0) per_sm[dev] = ctas_per_sm(kernel, kSmemFwd);
     const int64_t n_tiles = (n + kTile - 1) / kTile;
-    const int64_t max_ctas = (int64_t)ngp::sm_count() * 4;  // 52 KB smem + 64 TMEM columns per CTA
+    const int64_t max_ctas = (int64_t)ngp::sm_count() * per_sm[dev];
     const unsigned grid = (unsigned)(n_tiles < max_ctas ? n_tiles : max_ctas);
-    mlp_fwd_kernel<TEmb><<<grid, kThreads, kSmemBytes, st>>>((const TEmb*)emb, dirs, *w, sigmas, (__half*)rgbs,
-                                                            (__half*)save, n, n_dev);
+    kernel<<<grid, kThreads, kSmemFwd, st>>>((const TEmb*)emb, dirs, *w, sigmas, (__half*)rgbs, (__half*)save, n, n_dev);
     NGP_LAUNCHED("mlp_fwd_kernel");
     return 0;
 }
 
 }  // namespace
 
-#ifdef NGP_MLP_TRACE
-extern "C" int ngp_debug_mlp_trace(long long* out_host) {
-    return (int)cudaMemcpyFromSymbol(out_host, g_mlp_trace, sizeof(long long) * 256);
-}
-extern "C" int ngp_debug_mlp_bwd_trace(long long* iss_host, long long* wrk_host) {
-    cudaError_t e = cudaMemcpyFromSymbol(iss_host, g_bwd_iss, sizeof(g_bwd_iss));
-    if (e == cudaSuccess) e = cudaMemcpyFromSymbol(wrk_host, g_bwd_wrk, sizeof(g_bwd_wrk));
-    return (int)e;
-}
-#endif
-
 extern "C" {
-
-int ngp_mlp_set_impl(int fwd_impl) {
-    NGP_REQUIRE(fwd_impl >= 0 && fwd_impl <= 2, "fwd_impl must be 0 (auto), 1 (v1) or 2 (v2)");
-    g_fwd_impl = fwd_impl;
-    return 0;
-}
-
-int ngp_mlp_set_bwd_impl(int bwd_impl) {
-    NGP_REQUIRE(bwd_impl >= 0 && bwd_impl <= 2, "bwd_impl must be 0 (auto), 1 (v1) or 2 (v2)");
-    g_bwd_impl = bwd_impl;
-    return 0;
-}
 
 int64_t ngp_mlp_save_bytes(int64_t n) {
     // [n x 16] fp16 h (sigma-net output) + [n x 4] fp16 rgb (3 used): with them the backward skips layers 2 and 5
@@ -1355,16 +616,9 @@ int ngp_mlp_bwd_dyn(const void* emb, int emb_dtype, const float* dirs, const ngp
     NGP_REQUIRE((reinterpret_cast<uintptr_t>(demb) & 15) == 0, "demb must be 16-byte aligned");
     NGP_REQUIRE((reinterpret_cast<uintptr_t>(save) & 15) == 0, "save must be 16-byte aligned");
     cudaStream_t st = ngp::as_stream(stream);
-    if (emb_dtype == NGP_F16) {
-        static const int env_impl = [] { const char* e = getenv("NGP_MLP_BWD"); return e ? atoi(e) : -1; }();
-        const int impl = env_impl >= 0 ? env_impl : g_bwd_impl;
-        if (save && impl != 1 && n >= kTile) {
-            const int rc = launch_bwd_v2(emb, dirs, w, save, dsigmas, drgbs_f16, demb, grad_w, n, n_dev, found_inf_or_null, st);
-            if (rc != -2) return rc;   // -2: not set up and the stream is capturing -> v1 below
-        }
+    if (emb_dtype == NGP_F16)
         return save ? launch_bwd<__half, true>(emb, dirs, w, save, dsigmas, drgbs_f16, demb, grad_w, n, n_dev, found_inf_or_null, st)
                     : launch_bwd<__half, false>(emb, dirs, w, save, dsigmas, drgbs_f16, demb, grad_w, n, n_dev, found_inf_or_null, st);
-    }
     return save ? launch_bwd<float, true>(emb, dirs, w, save, dsigmas, drgbs_f16, demb, grad_w, n, n_dev, found_inf_or_null, st)
                 : launch_bwd<float, false>(emb, dirs, w, save, dsigmas, drgbs_f16, demb, grad_w, n, n_dev, found_inf_or_null, st);
 }

@@ -3,7 +3,7 @@
 // Semantics: modules/spherical_harmonics.py:16-42, modules/volume_train.py:22-48 (+ its Taichi
 // autodiff transpose, volume_train.py:160-173) and modules/volume_render_test.py:19-54.
 //
-// B200 mapping.  The reference composites with one thread per ray walking up to 1024 samples
+// GPU mapping.  The reference composites with one thread per ray walking up to 1024 samples
 // serially through a global T scratch array.  Here one WARP owns a ray: lanes take consecutive
 // samples (coalesced 128-byte loads), transmittance is a warp prefix product carried across
 // 32-sample chunks, early termination is a ballot, and the per-ray sums are shuffle reductions.

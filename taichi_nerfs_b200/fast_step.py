@@ -4,7 +4,7 @@ Same math as NGPTrainer.step / the reference's loop body (train.py:184-201) — 
 the C-ABI kernels, enqueued in a fixed order on fixed buffers:
 
   [ray-batch sampler] -> ray_aabb -> single-pass march (capacity buffers, one atomic row reservation per ray) ->
-  hash fwd (+AABB normalisation) -> tcgen05 MLP fwd -> fused per-ray head (composite fwd + background + MSE +
+  hash fwd (+AABB normalisation) -> fused MLP fwd -> fused per-ray head (composite fwd + background + MSE +
   composite bwd) -> MLP bwd -> hash bwd -> [all-reduce] -> check_finite -> device-side LR/bias-correction update
   -> fused Adam (+fp16 shadow, grad zero) -> device-side GradScaler update
 
@@ -94,7 +94,7 @@ class StaticTrainStep:
         # several ranks, opt-in: all-reduce gradient slices behind the backward kernels that complete them (F = 2 layout)
         import os
         # (opt-in, NGP_AR_OVERLAP=1: on 2 GPUs the three grouped scatter launches + concurrent NCCL kernels cost more
-        # than the all-reduce they hide — profiles/r2_bench_2gpu_*.json)
+        # than the all-reduce they hide)
         default_ar = ((trainer.world_size > 1 or os.environ.get("NGP_AR_FORCE") == "1") and enc._clayout.feat_dim == 2
                       and os.environ.get("NGP_AR_OVERLAP", "0") == "1")
         self.overlap_allreduce = bool(overlap_allreduce if overlap_allreduce is not None else default_ar)

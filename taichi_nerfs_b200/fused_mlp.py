@@ -1,4 +1,4 @@
-"""Autograd front end of the fused tcgen05 NGP MLP (csrc/mlp.cu).
+"""Autograd front end of the fused wgmma NGP MLP (csrc/mlp.cu).
 
 Used by ``modules.networks.NGP.forward`` whenever the stock architecture is configured (32-d
 embedding, 64-wide sigma net with 16 outputs, 2x64 rgb net): one kernel launch replaces the five

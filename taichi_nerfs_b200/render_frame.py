@@ -32,7 +32,7 @@ def render_frame(model, rays_o, rays_d, exp_step_factor=0.0, T_threshold=1e-4, m
     opacity = torch.empty(n, device=dev, dtype=torch.float32)
     enc = model.pos_encoder
     half = hasattr(enc, "table_f16")
-    fused = bool(model._fusable(rays_o))     # stock architecture: hash + tcgen05 MLP kernels on the raw sample rows
+    fused = bool(model._fusable(rays_o))     # stock architecture: hash + fused MLP kernels on the raw sample rows
     if fused:
         table = enc.table_f16() if half else enc.hash_table.detach().contiguous()
         W = [w.detach() for w in mlp_weights(model)]
@@ -105,7 +105,7 @@ class FrameRenderer:
     """Compacting test-time renderer: the whole frame is ONE CUDA graph of rounds with device-side control.
 
     round = [bookkeeping] -> persistent-warp march over the list of live rays (<= limit samples per ray, resume point
-    kept per ray) -> hash encode -> tcgen05 MLP -> composite onto the per-ray accumulators + block-level compaction of
+    kept per ray) -> hash encode -> fused MLP -> composite onto the per-ray accumulators + block-level compaction of
     the rays that are still alive (transmittance above the threshold, still inside the box) into the next round's list.
     Rays that have hit an opaque surface leave the list, so — unlike ``render_frame`` — samples behind it are neither
     marched nor shaded.  The host reads nothing until the frame is done (one 32-byte state read), where the reference
@@ -142,8 +142,7 @@ class FrameRenderer:
         self.coarse = None
         import os
         # The empty-space leap of the round march is opt-in (NGP_FRAME_LEAP=1): bit-exact (tests), but its exact
-        # super-cell box test costs more than the steps it skips on the Lego-sized box — 29 ms per 800x800 frame with
-        # it, 5.5 ms without (profiles/r2_frame800_leap_ab.txt); the earlier dilated variant bought 1 %.
+        # super-cell box test cost more than the steps it skips on the Lego-sized box when it was measured.
         use_leap = use_leap and os.environ.get("NGP_FRAME_LEAP", "0") == "1"
         if use_leap and model.cascades == 1 and model.grid_size in (32, 64, 128) and self.esf == 0.0:
             self.coarse = z(max((model.grid_size // 8) ** 3 // 32, 1), dtype=i32)

@@ -109,8 +109,7 @@ class NGPTrainer:
         # sync_master() (called before state_dict / checkpoints).
         import os
         P = self.slices[0][1]
-        # (opt-in, NGP_SHARDED_ADAM=1: on 2 GPUs its four collectives cost more than the bytes they save,
-        # profiles/r2_bench_2gpu_*.json)
+        # (opt-in, NGP_SHARDED_ADAM=1: on 2 GPUs its four collectives cost more than the bytes they save)
         want = (sharded_optimizer if sharded_optimizer is not None
                 else os.environ.get("NGP_SHARDED_ADAM", "0") == "1")
         self.sharded = bool((want or self.p2p is not None) and self.world_size > 1 and self._shadow_full is not None

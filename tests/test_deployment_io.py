@@ -76,13 +76,11 @@ def test_deployment_npy_and_bin_round_trip(tmp_path):
         load_deployment_model(NGP(scale=0.5), blob)                            # stock architecture: shapes differ
 
 
-REF = "/root/reference/deployment/InstantNGP/taichi_ngp/compiled"
-
-
-@pytest.mark.skipif(not os.path.exists(os.path.join(REF, "hash_embedding.bin")), reason="reference checkout not available")
 def test_shipped_lego_files_load_into_the_model():
     from modules.networks import NGP
     from modules.utils import load_deployment_model, read_aot_array
+    from oracle import kat_lego
+    REF = kat_lego.stage()   # the shipped model's six .bin files, rebuilt from tests/golden/
     m = NGP(**DEPLOY_CFG)
     extra = load_deployment_model(m, REF)
     assert extra['pose'].size == 12 and extra['model.directions'].size == 600 * 300 * 3

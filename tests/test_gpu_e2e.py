@@ -27,7 +27,7 @@ def test_state_dict_keys_match_reference():
 
 
 def test_fused_mlp_path_equals_torch_path():
-    """NGP.forward through the tcgen05 kernel vs the reference's nn.Linear graph under autocast."""
+    """NGP.forward through the fused MLP kernel vs the reference's nn.Linear graph under autocast."""
     from modules.networks import NGP
     torch.manual_seed(0)
     m = NGP(scale=0.5, max_res=1024, half_opt=True).cuda()
@@ -288,14 +288,14 @@ def test_static_step_with_device_sampled_batches(lego_bitfield, use_graph):
 
 def test_shipped_lego_model_renders_on_gpu():
     """Known-answer test on the CUDA path: the reference's shipped, trained Lego deployment model (L=4 F=4 dense
-    grid, 16-wide MLPs; staged under oracle/_ref/ by __graft_entry__.build()) loaded with load_deployment_model and
+    grid, 16-wide MLPs; rebuilt under oracle/_ref/ from tests/golden/) loaded with load_deployment_model and
     rendered through render(test_time=True) must reproduce the oracle's golden image of the same rays
     (tests/golden/lego_kat.png, made by oracle/kat_lego.py)."""
     import os
     import __graft_entry__ as g
     from conftest import GOLDEN
     if not g.stage_lego_fixture():
-        pytest.skip("shipped Lego weights not staged (needs one build() in the container that has /root/reference)")
+        pytest.skip("shipped Lego weights could not be staged")
     from PIL import Image
     from modules.networks import NGP
     from modules.rendering import render
@@ -406,11 +406,11 @@ def test_module_path_has_gradscaler_semantics(lego_bitfield):
 
 def test_psnr_vs_teacher():
     """"PSNR vs ref" protocol (SURVEY.md §8c): the stock fp16 model trained for 1500 graph steps on 200x200 views of the
-    reference's shipped trained Lego model must reach >= 25 dB on held-out teacher views (measured: see
-    profiles/r2_psnr.json; an untrained model scores ~9 dB)."""
+    reference's shipped trained Lego model must reach >= 25 dB on held-out teacher views (an untrained model scores
+    ~9 dB)."""
     import __graft_entry__ as g
     if not g.stage_lego_fixture():
-        pytest.skip("shipped Lego weights not staged (needs one build() in the container that has /root/reference)")
+        pytest.skip("shipped Lego weights could not be staged")
     from taichi_nerfs_b200.psnr import train_vs_teacher
     r = train_vs_teacher(torch.device('cuda'), steps=1500, train_views=32, test_views=2, downsample=0.25)
     assert r is not None

@@ -382,7 +382,7 @@ def test_mlp_bwd_tcgen05_matches_oracle(ops, oracle, emb_half, n, saved):
     demb, gw = ops.mlp_bwd(T(emb), T(dirs), [T(w) for w in ws], T(dsig), T(drgb), save=save)
     demb, gw = N(demb).astype(np.float32), N(gw)
     demb_ref = demb_ref.astype(np.float32)
-    # Error model (measured: profiles/r2_mlp_bwd_error.txt).  Every intermediate gradient is rounded to fp16 on both
+    # Error model (scripts/measure_mlp_bwd_error.py).  Every intermediate gradient is rounded to fp16 on both
     # sides and the tensor core sums K in a different order, so individual roundings flip by one fp16 ulp: the bulk of
     # the elements agrees to ~2e-5 of the tensor's max (asserted on the 99.9th percentile at 1e-4 = 5x measured).  The
     # few large deviations are not rounding noise but ReLU-mask flips: a hidden pre-activation within an ulp of zero is

@@ -1,5 +1,5 @@
-"""Known-answer test against the reference's shipped trained Lego deployment model (build container only:
-the 44 MB weight file lives under /root/reference and does not travel to the GPU box)."""
+"""Known-answer test against the reference's shipped trained Lego deployment model (stored shrunk under tests/golden/,
+rebuilt by oracle.kat_lego.stage())."""
 import json
 import os
 
@@ -9,11 +9,6 @@ import pytest
 from conftest import GOLDEN
 from oracle import kat_lego
 
-needs_ref = pytest.mark.skipif(not os.path.exists(os.path.join(kat_lego.REF_DIR, "hash_embedding.bin")),
-                               reason="reference checkout (trained deployment model) not available")
-
-
-@needs_ref
 def test_oracle_renders_the_shipped_lego_model():
     rgb, opacity, spr, counts = kat_lego.render(step=3)
     st = kat_lego.stats(rgb, opacity, spr)
@@ -32,9 +27,9 @@ def test_oracle_renders_the_shipped_lego_model():
     assert tv < 0.2   # uniform-random colours give ~0.67
 
 
-@needs_ref
 def test_deployment_bin_container_and_layout():
     from taichi_nerfs_b200.layout import make_hash_layout
+    kat_lego.stage()
     emb = kat_lego.read_bin(os.path.join(kat_lego.REF_DIR, "hash_embedding.bin"))
     assert emb.dtype == np.float32 and emb.size == make_hash_layout(2 ** 21, 4, 32, 128, 4).total_param_size
     assert kat_lego.read_bin(os.path.join(kat_lego.REF_DIR, "sigma_weights.bin")).size == 512

@@ -2,7 +2,7 @@
 seeds (:39-42), model_config (:86-117), mark_invisible_cells (:129), loss scale 2**16 | 2**19 (:137-141),
 Adam(lr, eps=1e-15) + cosine annealing to lr/30 (:143-163), density-grid update every 16 steps with a
 256-step warm-up (:57-58,178-182), log line every 1000 steps (:203-219), results/model.pth (:232-235),
-test-split PSNR (:237-304).  The step body runs on the sm_100a kernels through NGPTrainer (fused Adam,
+test-split PSNR (:237-304).  The step body runs on the sm_90a kernels through NGPTrainer (fused Adam,
 no host sync for the inf check); under torchrun every rank trains on its own rays and the flat gradient
 buffer is all-reduced once per step over NCCL.
 """
