@@ -71,6 +71,31 @@ def forward(model, rays_o, rays_d, noise, exp_step_factor=0.0, T_threshold=1e-4,
     return rgb_out.astype(np.float32), cache
 
 
+def render_test(model, rays_o, rays_d, exp_step_factor=0.0, T_threshold=1e-4, max_samples=1024):
+    """render(test_time=True) of the reference (modules/rendering.py:61-158) in one pass: the test-time march (no
+    jitter, at most max_samples per ray) of every ray, the network on every sample, then ONE composite_test call over
+    each ray's whole sample list.  Compositing stops at the first sample where T <= T_threshold, so this equals the
+    reference's chunked loop whenever that loop does not stop a ray early at max_samples (tests/test_oracle.py).
+    Returns dict(rgb [N,3] background included, depth [N], opacity [N], S = samples marched, n_term [N] = samples per
+    ray up to and including the one where T falls to the threshold, rays_a, sigmas, deltas)."""
+    n = rays_o.shape[0]
+    hits = O.ray_aabb_intersect(rays_o, rays_d, model.scale)
+    rays_a, xyzs, dirs, deltas, ts, S = O.raymarching_train(rays_o, rays_d, hits, model.bitfield,
+                                                           np.zeros(n, np.float32), model.cascades, model.scale,
+                                                           exp_step_factor, model.grid_size, max_samples)
+    lo, hi = np.float32(-model.scale), np.float32(model.scale)
+    xn = ((xyzs - lo) / (hi - lo)).astype(np.float32)
+    sigmas, rgbs = O.mlp_fwd(O.hash_encode_fwd(xn, model.table_for_kernel(), model.layout), dirs, model.ws)
+    opacity, depth = np.zeros(n, np.float32), np.zeros(n, np.float32)
+    rgb = np.zeros((n, 3), np.float32)
+    O.composite_test(sigmas, rgbs, deltas, ts, rays_a[:, 1:].astype(np.int64), rays_a[:, 0].astype(np.int64),
+                     T_threshold, opacity, depth, rgb)
+    n_term = O.composite_train_fwd(sigmas, rgbs, deltas, ts, rays_a, T_threshold)[0]  # same loop, counts the samples
+    bg = np.float32(1.0 if exp_step_factor == 0 else 0.0)  # rendering.py:152-156
+    return dict(rgb=(rgb + bg * (1 - opacity)[:, None]).astype(np.float32), depth=depth, opacity=opacity, S=S,
+                n_term=n_term, rays_a=rays_a, sigmas=sigmas, deltas=deltas)
+
+
 def backward(model, cache, rgb_out, rgb_gt, loss_scale):
     """Returns (loss, grad_table fp32 [P], grad_mlp fp32 [9408]) — gradients of loss*loss_scale."""
     n = rgb_out.shape[0]

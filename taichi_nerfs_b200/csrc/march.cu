@@ -222,6 +222,9 @@ struct RoundArgs {
     const int32_t* __restrict__ alive;      // live ray ids of this round
     const int32_t* __restrict__ n_alive;    // their number (device)
     float* __restrict__ t_cur;              // per ray: where the march resumes (in/out); +inf = left the box
+    int32_t* __restrict__ n_marched;        // per ray: samples emitted in earlier rounds of the frame (in/out), or
+                                            // null: no cap over the frame
+    int max_samples;                        // per-ray cap over the whole frame (the one-shot march's max_samples)
     int limit;                              // samples per ray this round (reduced so that all live rays fit `capacity`)
 };
 
@@ -256,9 +259,14 @@ __device__ __forceinline__ void march_one_ray(const float* __restrict__ rays_o, 
     const float t2 = hits_t[r * 2 + 1];
     float t;
     float t_resume = INFINITY;   // kMode 3: where the next round continues; stays +inf when the ray leaves the box
+    int marched_before = 0;
     if (kMode == 3) {
         t = round.t_cur[r];
         if (!(0.0f < t)) t = -1.0f;
+        if (round.n_marched != nullptr) {
+            marched_before = round.n_marched[r];
+            limit = max(0, min(limit, round.max_samples - marched_before));   // the frame's per-ray cap
+        }
     } else if (kMode == 2 && noise == nullptr) {  // test time: no jitter, strict 0 < t (ray_march.py:226)
         t = hits_t[r * 2 + 0];
         if (!(0.0f < t)) t = -1.0f;
@@ -462,7 +470,10 @@ __device__ __forceinline__ void march_one_ray(const float* __restrict__ rays_o, 
             rays_a[slot * 3 + 0] = (int32_t)r;
             rays_a[slot * 3 + 1] = s0;
             rays_a[slot * 3 + 2] = emitted;
-            round.t_cur[r] = t_resume;
+            // a ray that has reached max_samples is done, like the one-shot march: +inf takes it off the live list
+            const bool capped = round.n_marched != nullptr && marched_before + emitted >= round.max_samples;
+            if (round.n_marched != nullptr) round.n_marched[r] = marched_before + emitted;
+            round.t_cur[r] = capped ? INFINITY : t_resume;
         }
         __syncwarp();
         for (int k = lane; k < emitted; k += 32) {
@@ -743,22 +754,26 @@ int ngp_build_coarse_occupancy(const uint8_t* density_bitfield, int grid_size, u
     return 0;
 }
 
-int ngp_raymarching_round(const float* rays_o, const float* rays_d, const float* hits_t,
-                          const uint8_t* density_bitfield, int cascades, int grid_size, float scale,
-                          float exp_step_factor, int limit, const int32_t* alive, int32_t* state, float* t_cur,
-                          int32_t* rays_a, float* xyzs, float* dirs, float* deltas, float* ts, int64_t n_rays,
-                          int64_t capacity, const uint32_t* coarse_or_null, void* stream) {
+int ngp_raymarching_round_capped(const float* rays_o, const float* rays_d, const float* hits_t,
+                                 const uint8_t* density_bitfield, int cascades, int grid_size, float scale,
+                                 float exp_step_factor, int limit, int max_samples, const int32_t* alive,
+                                 int32_t* state, float* t_cur, int32_t* n_marched, int32_t* rays_a, float* xyzs,
+                                 float* dirs, float* deltas, float* ts, int64_t n_rays, int64_t capacity,
+                                 const uint32_t* coarse_or_null, void* stream) {
     NGP_REQUIRE(n_rays >= 0 && capacity >= 1, "bad size");
     if (n_rays == 0) return 0;
     NGP_REQUIRE(rays_o && rays_d && hits_t && density_bitfield && alive && state && t_cur && rays_a && xyzs && dirs &&
                     deltas && ts, "null pointer");
     NGP_REQUIRE(limit >= 1 && limit <= kMaxFrameSamples, "limit must be in [1, 1024]");
+    NGP_REQUIRE(n_marched == nullptr || max_samples >= 1, "max_samples must be >= 1");
     MarchParams p = make_params(density_bitfield, cascades, grid_size, scale, exp_step_factor);
     if (cascades == 1 && grid_size <= 128 && grid_size >= 32) p.coarse = coarse_or_null;
     RoundArgs ra;
     ra.alive = alive;
     ra.n_alive = state + 2;
     ra.t_cur = t_cur;
+    ra.n_marched = n_marched;
+    ra.max_samples = max_samples;
     ra.limit = limit;
     // persistent warps: a few CTAs per SM walk the live list (16 KB of shared memory and 128 threads per CTA)
     const int64_t want = (n_rays + kRaysPerBlock - 1) / kRaysPerBlock;
@@ -768,6 +783,16 @@ int ngp_raymarching_round(const float* rays_o, const float* rays_d, const float*
         rays_o, rays_d, hits_t, nullptr, p, limit, rays_a, state, xyzs, dirs, deltas, ts, n_rays, capacity, ra);
     NGP_LAUNCHED("march_train_warp_kernel<round>");
     return 0;
+}
+
+int ngp_raymarching_round(const float* rays_o, const float* rays_d, const float* hits_t,
+                          const uint8_t* density_bitfield, int cascades, int grid_size, float scale,
+                          float exp_step_factor, int limit, const int32_t* alive, int32_t* state, float* t_cur,
+                          int32_t* rays_a, float* xyzs, float* dirs, float* deltas, float* ts, int64_t n_rays,
+                          int64_t capacity, const uint32_t* coarse_or_null, void* stream) {
+    return ngp_raymarching_round_capped(rays_o, rays_d, hits_t, density_bitfield, cascades, grid_size, scale,
+                                        exp_step_factor, limit, 0, alive, state, t_cur, nullptr, rays_a, xyzs, dirs,
+                                        deltas, ts, n_rays, capacity, coarse_or_null, stream);
 }
 
 int ngp_raymarching_test(const float* rays_o, const float* rays_d, float* hits_t, const int64_t* alive_indices,

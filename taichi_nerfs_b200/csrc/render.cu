@@ -511,7 +511,8 @@ distortion_bwd_kernel(const float* __restrict__ dL_dloss, const float* __restric
 constexpr int kRoundWarps = 8;
 
 __global__ void frame_begin_kernel(const float* __restrict__ hits_t, float* __restrict__ t_cur,
-                                   int32_t* __restrict__ alive, int32_t* __restrict__ state,
+                                   int32_t* __restrict__ n_marched, int32_t* __restrict__ alive,
+                                   int32_t* __restrict__ state,
                                    float* __restrict__ opacity, float* __restrict__ depth, float* __restrict__ rgb,
                                    int64_t n) {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -524,6 +525,7 @@ __global__ void frame_begin_kernel(const float* __restrict__ hits_t, float* __re
     if (i >= n) return;
     const float t1 = hits_t[i * 2 + 0];
     t_cur[i] = 0.0f < t1 ? t1 : -1.0f;     // ray_march.py:226 (strict 0 < t); rays that miss the box never emit
+    n_marched[i] = 0;
     alive[i] = (int32_t)i;
     opacity[i] = 0.0f;
     depth[i] = 0.0f;
@@ -790,12 +792,12 @@ int ngp_composite_test(const float* sigmas, const void* rgbs, int rgbs_dtype, co
     return 0;
 }
 
-int ngp_frame_begin(const float* hits_t, float* t_cur, int32_t* alive, int32_t* state, float* opacity, float* depth,
-                    float* rgb, int64_t n_rays, void* stream) {
+int ngp_frame_begin(const float* hits_t, float* t_cur, int32_t* n_marched, int32_t* alive, int32_t* state,
+                    float* opacity, float* depth, float* rgb, int64_t n_rays, void* stream) {
     NGP_REQUIRE(n_rays >= 1 && n_rays < (1ll << 31), "n_rays out of range");
-    NGP_REQUIRE(hits_t && t_cur && alive && state && opacity && depth && rgb, "null pointer");
-    frame_begin_kernel<<<(unsigned)((n_rays + 255) / 256), 256, 0, ngp::as_stream(stream)>>>(hits_t, t_cur, alive, state,
-                                                                                           opacity, depth, rgb, n_rays);
+    NGP_REQUIRE(hits_t && t_cur && n_marched && alive && state && opacity && depth && rgb, "null pointer");
+    frame_begin_kernel<<<(unsigned)((n_rays + 255) / 256), 256, 0, ngp::as_stream(stream)>>>(
+        hits_t, t_cur, n_marched, alive, state, opacity, depth, rgb, n_rays);
     NGP_LAUNCHED("frame_begin_kernel");
     return 0;
 }

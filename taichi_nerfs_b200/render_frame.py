@@ -114,6 +114,7 @@ class FrameRenderer:
     samples are grouped into rounds.
     """
     SCHEDULE = (4, 8, 16, 32, 64, 128, 256, 512, 4)     # samples per live ray and round; sums to max_samples = 1024
+    MAX_SAMPLES = 1024     # per ray over the whole frame, extra rounds included (the one-shot march's max_samples)
 
     def __init__(self, model, n_rays, exp_step_factor=0.0, T_threshold=1e-4, rows_per_ray=6, use_graph=True,
                  use_leap=True):
@@ -134,6 +135,7 @@ class FrameRenderer:
         n, cap = self.n, self.cap
         self.rays_o, self.rays_d, self.hits = z(n, 3), z(n, 3), z(n, 2)
         self.t_cur, self.state = z(n), z(8, dtype=i32)
+        self.n_marched = z(n, dtype=i32)         # per ray: samples marched so far in this frame (capped at MAX_SAMPLES)
         self.alive = [z(n, dtype=i32), z(n, dtype=i32)]
         self.rays_a = z(n, 3, dtype=i32)
         self.xyzs, self.dirs, self.deltas, self.ts = z(cap, 3), z(cap, 3), z(cap), z(cap)
@@ -170,10 +172,11 @@ class FrameRenderer:
         L, m, st, p, check = self._load(), self.model, self._C.c_void_p(torch.cuda.current_stream().cuda_stream), self._p, self._check
         cur, nxt = self.alive[j & 1], self.alive[(j + 1) & 1]
         check(L.ngp_frame_round_begin(p(self.state), st))
-        check(L.ngp_raymarching_round(p(self.rays_o), p(self.rays_d), p(self.hits), p(m.density_bitfield), m.cascades,
-                                      m.grid_size, float(m.scale), self.esf, int(limit), p(cur), p(self.state),
-                                      p(self.t_cur), p(self.rays_a), p(self.xyzs), p(self.dirs), p(self.deltas),
-                                      p(self.ts), self.n, self.cap, p(self.coarse), st))
+        check(L.ngp_raymarching_round_capped(p(self.rays_o), p(self.rays_d), p(self.hits), p(m.density_bitfield),
+                                             m.cascades, m.grid_size, float(m.scale), self.esf, int(limit),
+                                             self.MAX_SAMPLES, p(cur), p(self.state), p(self.t_cur), p(self.n_marched),
+                                             p(self.rays_a), p(self.xyzs), p(self.dirs), p(self.deltas), p(self.ts),
+                                             self.n, self.cap, p(self.coarse), st))
         check(L.ngp_hash_encode_fwd_dyn(p(self.xyzs), p(self._table_t), self._C.byref(self._clayout), p(self.emb), self.tag,
                                         self.cap, p(self.state), self.aabb6, st))
         check(L.ngp_mlp_fwd_dyn(p(self.emb), self.tag, p(self.dirs), self._C.byref(self._wst), p(self.sig), p(self.rgbs),
@@ -185,8 +188,8 @@ class FrameRenderer:
     def _enqueue_frame(self):
         L, m, st, p, check = self._load(), self.model, self._C.c_void_p(torch.cuda.current_stream().cuda_stream), self._p, self._check
         check(L.ngp_ray_aabb_intersect(p(self.rays_o), p(self.rays_d), float(m.scale), p(self.hits), self.n, st))
-        check(L.ngp_frame_begin(p(self.hits), p(self.t_cur), p(self.alive[0]), p(self.state), p(self.opacity),
-                                p(self.depth), p(self.rgb), self.n, st))
+        check(L.ngp_frame_begin(p(self.hits), p(self.t_cur), p(self.n_marched), p(self.alive[0]), p(self.state),
+                                p(self.opacity), p(self.depth), p(self.rgb), self.n, st))
         if self.coarse is not None:   # 8^3-cell dilated occupancy: lets the march leap over empty space
             check(L.ngp_build_coarse_occupancy(p(m.density_bitfield), m.grid_size, p(self.coarse), st))
         for j, limit in enumerate(self.SCHEDULE):
@@ -222,7 +225,7 @@ class FrameRenderer:
         # live rays left for a further round, samples evaluated before the last round, ...]
         st = self.state.tolist()
         j = rounds
-        while st[3] > 0:               # rays that need more than the scheduled rounds (un-trained / foggy models)
+        while st[3] > 0:   # rays that need more than the scheduled rounds (un-trained / foggy models), up to MAX_SAMPLES
             self._table_t = tab
             self._enqueue_round(j, 512)
             st = self.state.tolist()

@@ -37,24 +37,43 @@ def test_ray_aabb_bit_exact(ops, oracle, rays_factory):
 
 
 # ---- a2 -------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("cfg", [
+MARCH_CFGS = [
     dict(scale=0.5, cascades=1, esf=0.0, occ="lego"),
     dict(scale=0.5, cascades=1, esf=0.0, occ="random"),
     dict(scale=16.0, cascades=6, esf=1 / 256, occ="random"),
     dict(scale=2.0, cascades=3, esf=1 / 256, occ="sparse"),
-])
-def test_march_train_bit_exact(ops, oracle, rays_factory, lego_bitfield, cfg):
-    n = 4099
-    rng = np.random.default_rng(21)
+]
+MARCH_IDS = ["lego", "random", "6casc_esf", "3casc_sparse"]
+
+
+def _march_inputs(cfg, n, seed, rng, rays_factory, lego_bitfield):
+    """Rays (inside the box unless the scene is the Lego one) and an occupancy bitfield of one march configuration."""
     radius = 1.4 if cfg["scale"] == 0.5 else 3.0
-    o, d = rays_factory(n, seed=21, radius=radius)
+    o, d = rays_factory(n, seed=seed, radius=radius)
     nbytes = cfg["cascades"] * 128 ** 3 // 8
     if cfg["occ"] == "lego":
         bits = lego_bitfield
+    elif cfg["occ"] == "full":
+        bits = np.full(nbytes, 255, np.uint8)
     elif cfg["occ"] == "random":
         bits = rng.integers(0, 256, nbytes, dtype=np.uint8)
     else:
         bits = (rng.random(nbytes) < 0.02).astype(np.uint8) * rng.integers(1, 256, nbytes, dtype=np.uint8)
+    return o, d, bits
+
+
+def _row_order(ra):
+    """rays_a [m, 3] -> (ray of every row, row index), rows listed slot by slot."""
+    k = ra[:, 2].astype(np.int64)
+    off = np.repeat(ra[:, 1].astype(np.int64) - (np.cumsum(k) - k), k)
+    return np.repeat(ra[:, 0], k), off + np.arange(int(k.sum()))
+
+
+@pytest.mark.parametrize("cfg", MARCH_CFGS)
+def test_march_train_bit_exact(ops, oracle, rays_factory, lego_bitfield, cfg):
+    n = 4099
+    rng = np.random.default_rng(21)
+    o, d, bits = _march_inputs(cfg, n, 21, rng, rays_factory, lego_bitfield)
     hits = oracle.ray_aabb_intersect(o, d, cfg["scale"])
     noise = rng.random(n, dtype=np.float32)
     ra, xyzs, dirs, deltas, ts, S = oracle.raymarching_train(o, d, hits, bits, noise, cfg["cascades"], cfg["scale"],
@@ -478,16 +497,28 @@ def test_deployment_model_config_trains():
 
 def test_march_frame_single_pass(ops, oracle, rays_factory, lego_bitfield):
     """Single-pass test-time march == oracle training march with zero noise, per ray (row order is arbitrary)."""
+    _check_frame_march(ops, oracle, rays_factory, lego_bitfield, MARCH_CFGS[0])
+
+
+@pytest.mark.parametrize("cfg", MARCH_CFGS[1:], ids=MARCH_IDS[1:])
+def test_march_frame_single_pass_configs(ops, oracle, rays_factory, lego_bitfield, cfg):
+    """The same at the other march configurations (cascades, exp_step_factor, occupancy)."""
+    _check_frame_march(ops, oracle, rays_factory, lego_bitfield, cfg)
+
+
+def _check_frame_march(ops, oracle, rays_factory, lego_bitfield, cfg):
     n = 5003
-    o, d = rays_factory(n, seed=40)
-    hits = oracle.ray_aabb_intersect(o, d, 0.5)
-    ra, xyzs, dirs, deltas, ts, S = oracle.raymarching_train(o, d, hits, lego_bitfield, np.zeros(n, np.float32), 1, 0.5,
-                                                            0.0, 128, 1024)
+    o, d, bits = _march_inputs(cfg, n, 40, np.random.default_rng(40), rays_factory, lego_bitfield)
+    sc, casc, esf = cfg["scale"], cfg["cascades"], cfg["esf"]
+    hits = oracle.ray_aabb_intersect(o, d, sc)
+    ra, xyzs, dirs, deltas, ts, S = oracle.raymarching_train(o, d, hits, bits, np.zeros(n, np.float32), casc, sc,
+                                                            esf, 128, 1024)
+    assert S > 0
     cap = S + 100
     counter = torch.zeros(2, device=DEV, dtype=torch.int32)
     g_ra = torch.zeros(n, 3, device=DEV, dtype=torch.int32)
     bufs = [torch.zeros(cap, 3, device=DEV), torch.zeros(cap, 3, device=DEV), torch.zeros(cap, device=DEV), torch.zeros(cap, device=DEV)]
-    ops.raymarching_frame(T(o), T(d), T(hits), T(lego_bitfield), 1, 0.5, 0.0, 128, 1024, counter, g_ra, *bufs)
+    ops.raymarching_frame(T(o), T(d), T(hits), T(bits), casc, sc, esf, 128, 1024, counter, g_ra, *bufs)
     assert N(counter).tolist() == [S, 0]
     g_ra = N(g_ra)
     assert np.array_equal(g_ra[:, 0], ra[:, 0]) and np.array_equal(g_ra[:, 2], ra[:, 2])
@@ -500,7 +531,7 @@ def test_march_frame_single_pass(ops, oracle, rays_factory, lego_bitfield):
     # capacity overflow: rays are dropped and counted, never written out of bounds
     counter.zero_()
     small = [torch.zeros(S // 3, 3, device=DEV), torch.zeros(S // 3, 3, device=DEV), torch.zeros(S // 3, device=DEV), torch.zeros(S // 3, device=DEV)]
-    ops.raymarching_frame(T(o), T(d), T(hits), T(lego_bitfield), 1, 0.5, 0.0, 128, 1024, counter, T(ra * 0), *small)
+    ops.raymarching_frame(T(o), T(d), T(hits), T(bits), casc, sc, esf, 128, 1024, counter, T(ra * 0), *small)
     assert N(counter)[1] > 0
 
 
@@ -637,30 +668,44 @@ def test_fused_grid_update_no_occupied_cells_and_erode(ops, oracle):
 
 
 # ---- compacting renderer: round march (resume points, empty-space leap) --------------------------------------------
+# garden scale, every cell occupied, rays from inside the box: every ray has more than max_samples candidate positions
+GARDEN_FULL = dict(scale=16.0, cascades=6, esf=1 / 256, occ="full")
+
+
 @pytest.mark.parametrize("leap", [False, True])
-def test_round_march_equals_full_march(ops, lego_bitfield, rays_factory, leap):
+def test_round_march_equals_full_march(ops, oracle, lego_bitfield, rays_factory, leap):
     """The per-round march of the compacting frame renderer (persistent warps over a live list, <= limit samples per
     ray and round, resume at t_cur, optional 256-position leap over empty space guided by the dilated coarse occupancy)
-    must emit, ray by ray, exactly the samples of the one-shot march (bit-exact t, delta, xyz), whatever the rounds."""
+    must emit, ray by ray, exactly the samples of the oracle's one-shot march with zero noise (bit-exact t, delta, xyz and
+    count), whatever the rounds.  Lego rays stay below max_samples, so the entry point without the cap gives them all."""
+    _check_round_march(ops, oracle, lego_bitfield, rays_factory, MARCH_CFGS[0], leap, capped=False)
+
+
+@pytest.mark.parametrize("leap", [False, True])
+@pytest.mark.parametrize("cfg", MARCH_CFGS + [GARDEN_FULL], ids=MARCH_IDS + ["6casc_full_capped"])
+def test_round_march_capped_equals_full_march(ops, oracle, lego_bitfield, rays_factory, cfg, leap):
+    """The round march as the frame renderer runs it, with the per-ray count that caps a ray at max_samples over all
+    rounds, at every march configuration.  The leap applies to one cascade with a constant step only: elsewhere the
+    kernel must ignore the coarse occupancy it is given."""
+    _check_round_march(ops, oracle, lego_bitfield, rays_factory, cfg, leap, capped=True)
+
+
+def _check_round_march(ops, oracle, lego_bitfield, rays_factory, cfg, leap, capped):
     import ctypes as C
     from taichi_nerfs_b200 import _lib
     L = _lib.load()
     n = 6000
-    o, d = rays_factory(n, seed=77)
-    o, d = T(o), T(d)
-    bits = T(lego_bitfield)
-    hits = ops.ray_aabb_intersect(o, d, 0.5)
-    zeros = torch.zeros(n, device="cuda")
-    counter, rays_a = ops.raymarching_train_count(o, d, hits, bits, zeros, 1, 0.5, 0.0, 128, 1024)
-    S = int(counter[0])
-    xyz_ref, dirs_ref = torch.empty(S, 3, device="cuda"), torch.empty(S, 3, device="cuda")
-    dl_ref, ts_ref = torch.empty(S, device="cuda"), torch.empty(S, device="cuda")
-    ops.raymarching_train_write(o, d, hits, bits, zeros, 1, 0.5, 0.0, 128, counter, rays_a, xyz_ref, dirs_ref, dl_ref, ts_ref)
-    ra = N(rays_a)
+    o_np, d_np, bits_np = _march_inputs(cfg, n, 77, np.random.default_rng(77), rays_factory, lego_bitfield)
+    sc, casc, esf = cfg["scale"], cfg["cascades"], cfg["esf"]
+    hits_np = oracle.ray_aabb_intersect(o_np, d_np, sc)
+    ra, xyz_ref, dirs_ref, dl_ref, ts_ref, S = oracle.raymarching_train(o_np, d_np, hits_np, bits_np,
+                                                                       np.zeros(n, np.float32), casc, sc, esf, 128, 1024)
+    o, d, bits, hits = T(o_np), T(d_np), T(bits_np), T(hits_np)
     p = lambda t: C.c_void_p(t.data_ptr())  # noqa: E731
     st = C.c_void_p(torch.cuda.current_stream().cuda_stream)
     cap = 64 * n
     t_cur = torch.where(hits[:, 0] > 0, hits[:, 0], torch.full_like(hits[:, 0], -1.0)).contiguous()
+    n_marched = torch.zeros(n, device="cuda", dtype=torch.int32)
     alive = torch.arange(n, device="cuda", dtype=torch.int32)
     state = torch.zeros(8, device="cuda", dtype=torch.int32)
     r_a = torch.zeros(n, 3, device="cuda", dtype=torch.int32)
@@ -669,14 +714,15 @@ def test_round_march_equals_full_march(ops, lego_bitfield, rays_factory, leap):
     coarse = None
     if leap:
         coarse = torch.zeros(128, device="cuda", dtype=torch.int32)
-        _lib.check(L.ngp_build_coarse_occupancy(p(bits), 128, p(coarse), st))
+        _lib.check(L.ngp_build_coarse_occupancy(p(bits), 128, p(coarse), st))    # from cascade 0
         c = N(coarse).view(np.uint32)
         # bit s = any occupied cell among the 512 Morton-consecutive cells (64 bytes) of super-cell s
-        want = np.packbits(lego_bitfield.reshape(4096, 64).any(1), bitorder="little").view(np.uint32)
+        want = np.packbits(bits_np[:128 ** 3 // 8].reshape(4096, 64).any(1), bitorder="little").view(np.uint32)
         np.testing.assert_array_equal(c, want)
-        occupied_sc = sum(bin(int(w)).count("1") for w in c)
-        assert 0 < occupied_sc < 4096 * 0.4, occupied_sc            # the Lego grid leaves most super-cells empty
-    got = [[] for _ in range(n)]
+        if cfg["occ"] == "lego":
+            occupied_sc = sum(bin(int(w)).count("1") for w in c)
+            assert 0 < occupied_sc < 4096 * 0.4, occupied_sc            # the Lego grid leaves most super-cells empty
+    rows_ray, rows_t, rows_dl, rows_xyz = [], [], [], []
     schedule = [4, 8, 16, 3, 64, 128, 256, 512]
     rounds = 0
     while not bool(((t_cur == float("inf")) | (t_cur < 0)).all()) and rounds < 64:
@@ -684,28 +730,36 @@ def test_round_march_equals_full_march(ops, lego_bitfield, rays_factory, leap):
         rounds += 1
         state.zero_()
         state[2] = n                                                  # every ray stays on the live list
-        _lib.check(L.ngp_raymarching_round(p(o), p(d), p(hits), p(bits), 1, 128, 0.5, 0.0, limit, p(alive), p(state),
-                                           p(t_cur), p(r_a), p(xyz), p(dirs), p(dl), p(ts), n, cap,
-                                           None if coarse is None else p(coarse), st))
+        pc = None if coarse is None else p(coarse)
+        if capped:
+            _lib.check(L.ngp_raymarching_round_capped(p(o), p(d), p(hits), p(bits), casc, 128, sc, esf, limit, 1024,
+                                                      p(alive), p(state), p(t_cur), p(n_marched), p(r_a), p(xyz),
+                                                      p(dirs), p(dl), p(ts), n, cap, pc, st))
+        else:
+            _lib.check(L.ngp_raymarching_round(p(o), p(d), p(hits), p(bits), casc, 128, sc, esf, limit, p(alive),
+                                               p(state), p(t_cur), p(r_a), p(xyz), p(dirs), p(dl), p(ts), n, cap, pc, st))
         rows = int(state[0])
         eff = max(1, min(limit, cap // n))
-        r_np, ts_np, dl_np, xyz_np = N(r_a), N(ts)[:rows], N(dl)[:rows], N(xyz)[:rows]
+        r_np = N(r_a)
         assert (r_np[:, 2] <= eff).all() and int(r_np[:, 2].sum()) == rows
-        for ray, s0, k in r_np:
-            if k:
-                got[ray].append((ts_np[s0:s0 + k], dl_np[s0:s0 + k], xyz_np[s0:s0 + k]))
+        ray_of, idx = _row_order(r_np)
+        assert np.array_equal(np.sort(idx), np.arange(rows))          # the reserved ranges tile [0, rows)
+        rows_ray.append(ray_of)
+        rows_t.append(N(ts)[idx])
+        rows_dl.append(N(dl)[idx])
+        rows_xyz.append(N(xyz)[idx])
     done = (t_cur == float("inf")) | (t_cur < 0)
-    assert bool(done.all()), "every ray must have left the box"
-    ts_r, dl_r, xyz_r = N(ts_ref), N(dl_ref), N(xyz_ref)
-    total = 0
-    for ray, s0, k in ra:
-        if k == 0:
-            assert not got[ray]
-            continue
-        t_all = np.concatenate([g[0] for g in got[ray]])
-        assert t_all.shape[0] == k, (ray, t_all.shape[0], k)
-        np.testing.assert_array_equal(t_all, ts_r[s0:s0 + k])
-        np.testing.assert_array_equal(np.concatenate([g[1] for g in got[ray]]), dl_r[s0:s0 + k])
-        np.testing.assert_array_equal(np.concatenate([g[2] for g in got[ray]]), xyz_r[s0:s0 + k])
-        total += k
-    assert total == S and S > 50000
+    assert bool(done.all()), "every ray must have left the box or reached max_samples"
+    if capped:
+        np.testing.assert_array_equal(N(n_marched), ra[:, 2])          # per-ray sample count == the capped march's
+    # rows of all rounds, stably grouped by ray (rounds in order) == the oracle's rows, which are in ray order
+    order = np.argsort(np.concatenate(rows_ray), kind="stable")
+    for got, want in ((rows_t, ts_ref), (rows_dl, dl_ref), (rows_xyz, xyz_ref)):
+        got = np.concatenate(got)[order]
+        assert got.shape == want.shape
+        assert np.array_equal(got.view(np.uint32), want.view(np.uint32))
+    assert S > 30000
+    if not capped:
+        assert ra[:, 2].max() < 1024
+    if cfg["occ"] == "full":
+        assert (ra[:, 2] == 1024).mean() > 0.9            # the per-ray cap is what ends these rays

@@ -394,6 +394,73 @@ def test_composite_test_equals_train_when_chunked(oracle):
     np.testing.assert_allclose(depth, dep, atol=1e-5)
 
 
+def _reference_test_loop(oracle, model, o, d, esf, thr, max_samples=1024):
+    """numpy restatement of the reference's test-time loop (modules/rendering.py:61-158): march <= step samples per
+    live ray (raymarching_test resumes at hits_t[:, 0]), shade them, composite_test onto the accumulators, drop the
+    rays it marks dead; step = max(min(n_rays // n_alive, 64), min_samples)."""
+    n = o.shape[0]
+    hits = oracle.ray_aabb_intersect(o, d, model.scale)
+    opacity, depth, rgb = np.zeros(n, np.float32), np.zeros(n, np.float32), np.zeros((n, 3), np.float32)
+    alive = np.arange(n, dtype=np.int64)
+    samples = total = 0
+    min_samples = 1 if esf == 0 else 4
+    lo, hi = np.float32(-model.scale), np.float32(model.scale)
+    while samples < max_samples and alive.size:
+        step = max(min(n // alive.size, 64), min_samples)
+        samples += step
+        ri, valid, dl, tt, cnt = oracle.raymarching_test(o, d, hits, alive, model.bitfield, model.cascades,
+                                                         model.scale, esf, model.grid_size, step)
+        v = valid.astype(bool)
+        if not v.any():
+            break
+        ri, dl, tt = ri[v], dl[v], tt[v]
+        cnt = cnt.astype(np.int64)
+        pack = np.stack([np.cumsum(cnt) - cnt, cnt], 1)
+        xyzs = o[ri] + tt[:, None] * d[ri]                       # rendering.py:109-111, fp32
+        xn = ((xyzs - lo) / (hi - lo)).astype(np.float32)
+        sig, rgbs = oracle.mlp_fwd(oracle.hash_encode_fwd(xn, model.table_for_kernel(), model.layout), d[ri], model.ws)
+        oracle.composite_test(sig, rgbs, dl, tt, pack, alive, thr, opacity, depth, rgb)
+        alive = alive[alive >= 0]
+        total += int(cnt.sum())
+    bg = np.float32(1.0 if esf == 0 else 0.0)
+    return dict(rgb=rgb + bg * (1 - opacity)[:, None], depth=depth, opacity=opacity, total_samples=total)
+
+
+@pytest.mark.parametrize("thr", [1e-4, 0.25])
+@pytest.mark.parametrize("scene", ["lego", "3casc_esf"])
+def test_render_test_equals_reference_loop(oracle, lego_bitfield, rays_factory, scene, thr):
+    """oracle render_test (one march of every ray, one composite_test per ray) == the reference's chunked loop on rays
+    that stay below max_samples: compositing is sequential per ray and stops at the first sample with T <= threshold,
+    however the samples are chunked.  The chunks restart from T = 1 - opacity, hence fp32 rounding, not bits."""
+    from oracle.train_step import OracleModel, render_test
+    rng = np.random.default_rng(16)
+    lay = make_hash_layout(2 ** 19, 16, 16, 1024, 2)
+    table = (rng.uniform(-1, 1, (lay.total_entries, 2)) * 6).astype(np.float32)     # dense-ish medium
+    if scene == "lego":
+        sc, casc, esf, bits = 0.5, 1, 0.0, lego_bitfield
+        o, d = rays_factory(256, seed=16)
+    else:
+        sc, casc, esf = 2.0, 3, 1 / 256
+        bits = (rng.random(casc * 128 ** 3 // 8) < 0.05).astype(np.uint8) * rng.integers(1, 256, casc * 128 ** 3 // 8,
+                                                                                          dtype=np.uint8)
+        o, d = rays_factory(256, seed=16, radius=1.5)
+    ws = _rand_weights(rng)
+    ws[1] *= 3                                                                          # larger density logits
+    model = OracleModel(lay, table, ws, bits, scale=sc, cascades=casc, half=True)
+    got = render_test(model, o, d, esf, thr)
+    want = _reference_test_loop(oracle, model, o, d, esf, thr)
+    counts = got["rays_a"][:, 2]
+    assert counts.max() < 1024 and got["S"] == counts.sum() > 0
+    n_term = got["n_term"]
+    stopped = n_term < counts                                  # rays whose transmittance fell to the threshold
+    assert 0.05 < stopped.mean() < 0.95, stopped.mean()        # both kinds of ray are present
+    assert (n_term <= counts).all()
+    for k in ("rgb", "depth", "opacity"):
+        np.testing.assert_allclose(got[k], want[k], atol=1e-5, err_msg=k)
+    # the loop marches whole chunks: at least every sample up to termination, at most every sample
+    assert n_term.sum() <= want["total_samples"] <= got["S"]
+
+
 # ------------------------------------------------------------------------------------------------
 def test_packbits_and_morton(oracle):
     rng = np.random.default_rng(15)
