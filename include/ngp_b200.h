@@ -53,6 +53,22 @@ typedef struct ngp_hash_layout {
     uint32_t resolutions[NGP_MAX_LEVELS]; /* ceil(scale)+1                         */
 } ngp_hash_layout;
 
+/*
+ * Tri-plane layout (modules/triplane.py of the reference): three max_res x max_res planes of F features,
+ * plane fd starting at fd*max_res^2*F (triplane.py:24,85), entry (u, v) of a plane at (u + v*max_res)*F.
+ * `scales`/`resolutions` are the per-level fp32 scale base_res*exp(l*log_b) - 1 and ceil(scale) + 1
+ * (triplane.py:27-33), derived on the host exactly like the hash levels'.
+ */
+#define NGP_TRIPLANE_MAX_RES 16384
+typedef struct ngp_triplane_layout {
+    int32_t  n_levels;               /* L, 1..NGP_MAX_LEVELS                      */
+    int32_t  feat_dim;               /* F: features per level, 2 or 4             */
+    int32_t  max_res;                /* plane side, 2..NGP_TRIPLANE_MAX_RES       */
+    int32_t  reserved;
+    float    scales[NGP_MAX_LEVELS];      /* base_res*exp(l*log_b) - 1     (f32)   */
+    uint32_t resolutions[NGP_MAX_LEVELS]; /* ceil(scale)+1                         */
+} ngp_triplane_layout;
+
 /* Weights of the tiny NGP MLP (modules/networks.py:111-132): no biases.
  * Row-major [out, in] exactly like torch.nn.Linear.weight, fp32 master copy. */
 typedef struct ngp_mlp_weights {
@@ -147,6 +163,27 @@ int ngp_hash_encode_bwd(const float* xyz, const void* dout, int dout_dtype,
 int ngp_hash_encode_bwd_input(const float* xyz, const void* table, const void* dout, int dtype,
                               const ngp_hash_layout* layout, float* dx,
                               int64_t n, void* stream);
+
+/* ---- tri-plane encoding ---------------------------------------------------- */
+/* forward: replaces triplane_encoder_kernel, modules/triplane.py:35-98.  xyz [n,3] in [0,1] ->
+ * out fp32 [n, L*F], column j*L + level (feature-major, triplane.py:43-45).  The max_res-grid
+ * coordinate is clamped to [0, max_res-1] (the reference's bounds check is commented out,
+ * triplane.py:88-89); the clamp is the identity for positions in [0,1].
+ * `aabb6` (HOST pointer, 6 floats: xyz_min[3], xyz_max-xyz_min[3]; may be NULL) folds NGP.density's
+ * normalisation (modules/networks.py:144) into the load, bit-identical to normalising first.
+ * `table` (and `grad_table`) must be aligned to one entry (4*F bytes). */
+int ngp_triplane_encode_fwd(const float* xyz, const float* table, const ngp_triplane_layout* layout,
+                            float* out, int64_t n, const float* aabb6, void* stream);
+/* the same with the row count read on the device: rows [0, min(n_max, *n_dev)) (the compacting frame
+ * renderer's round, see ngp_hash_encode_fwd_dyn); rows >= that count are not written. */
+int ngp_triplane_encode_fwd_dyn(const float* xyz, const float* table, const ngp_triplane_layout* layout,
+                                float* out, int64_t n_max, const int32_t* n_dev, const float* aabb6,
+                                void* stream);
+/* backward wrt the table: replaces triplane_encoder_kernel.grad (Taichi autodiff, triplane.py:186-197):
+ * grad_table[entry(fd,c)] += dout * w_c[fd] * prod_{fd' != fd} lf[fd'], ACCUMULATED into the caller's fp32
+ * buffer.  xyz in [0,1] (no aabb).  There is no dL/dxyz (the reference returns None, :197). */
+int ngp_triplane_encode_bwd(const float* xyz, const float* table, const float* dout,
+                            const ngp_triplane_layout* layout, float* grad_table, int64_t n, void* stream);
 
 /* ---- sync-free ("_dyn") variants used by the graph-captured training step -------------------
  * Same kernels as above, but the number of valid rows is read ON THE DEVICE: rows [0, min(n_max,*n_dev))

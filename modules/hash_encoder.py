@@ -2,6 +2,8 @@
 (HashEncoder :147-285).  The table is one flat fp32 Parameter of L-level (offset, size) slabs."""
 from __future__ import annotations
 
+import ctypes
+
 import torch
 
 from taichi_nerfs_b200 import ops
@@ -73,3 +75,20 @@ class HashEncoder(torch.nn.Module):
 
     def forward(self, positions):
         return _HashEncode.apply(positions.float().contiguous(), self.hash_table.contiguous(), self)
+
+    # ---- kernel-level interface (NGP's grid update and the frame renderers) -------------------------------------
+    emb_dtype = torch.float32
+
+    def kernel_table(self):
+        """The tensor the encode kernel reads (its pointer is tracked by FrameRenderer's graph)."""
+        return self.hash_table.detach().contiguous()
+
+    def encode_world(self, xyzs_w, aabb):
+        """[N, out_dim] embedding of world positions, aabb = (xyz_min[3], xyz_max-xyz_min[3]) normalised in the
+        kernel; no autograd."""
+        return ops.hash_encode_fwd(xyzs_w, self.kernel_table(), self._clayout, self.out_dim, aabb=aabb)
+
+    def enqueue_encode_dyn(self, lib, xyzs, table, emb, n_max, n_dev, aabb6, stream):
+        """Raw launch of the device-counted encode (FrameRenderer's rounds): pointers in, rc out."""
+        return lib.ngp_hash_encode_fwd_dyn(xyzs, table, ctypes.byref(self._clayout), emb, ops.F32, n_max, n_dev, aabb6,
+                                           stream)

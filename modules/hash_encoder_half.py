@@ -3,6 +3,8 @@ modules/hash_encoder_half.py of the reference (HashEncoder :218-368): fp32 maste
 [entries, F], gathers from an fp16 copy with fp16 accumulation, fp32 gradient accumulation."""
 from __future__ import annotations
 
+import ctypes
+
 import torch
 
 from taichi_nerfs_b200 import ops
@@ -91,3 +93,20 @@ class HashEncoder(torch.nn.Module):
     def forward(self, positions):
         out = _HashEncodeHalf.apply(positions.float().contiguous(), self.hash_table, self)
         return out.view(-1, self.out_dim)
+
+    # ---- kernel-level interface (NGP's grid update and the frame renderers) -------------------------------------
+    emb_dtype = torch.float16
+
+    def kernel_table(self):
+        """The tensor the encode kernel reads (its pointer is tracked by FrameRenderer's graph)."""
+        return self.table_f16()
+
+    def encode_world(self, xyzs_w, aabb):
+        """[N, out_dim] embedding of world positions, aabb = (xyz_min[3], xyz_max-xyz_min[3]) normalised in the
+        kernel; no autograd."""
+        return ops.hash_encode_fwd(xyzs_w, self.kernel_table(), self._clayout, self.out_dim, aabb=aabb)
+
+    def enqueue_encode_dyn(self, lib, xyzs, table, emb, n_max, n_dev, aabb6, stream):
+        """Raw launch of the device-counted encode (FrameRenderer's rounds): pointers in, rc out."""
+        return lib.ngp_hash_encode_fwd_dyn(xyzs, table, ctypes.byref(self._clayout), emb, ops.F16, n_max, n_dev, aabb6,
+                                           stream)

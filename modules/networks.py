@@ -87,10 +87,13 @@ class NGP(nn.Module):
                 from .hash_encoder import HashEncoder
             self.pos_encoder = HashEncoder(max_params=2 ** log2_T, base_res=base_res, max_res=max_res,
                                            levels=levels, feature_per_level=feature_per_level)
+        elif pos_encoder_type == 'triplane':
+            # networks.py:101-107: levels, feature_per_level, log2_T and half_opt do not apply to the tri-plane
+            from .triplane import TriPlaneEncoder
+            self.pos_encoder = TriPlaneEncoder(base_res=16, max_res=max_res, levels=8, feature_per_level=4)
         else:
-            # 'triplane' is an experimental alternative in the reference (modules/triplane.py) and is
-            # outside the hot path this repository accelerates (SURVEY.md §2.2: out of scope).
-            raise NotImplementedError(f"pos_encoder_type={pos_encoder_type!r} is out of scope here")
+            raise NotImplementedError(f"pos_encoder_type={pos_encoder_type!r}")
+        self.pos_encoder_type = pos_encoder_type
 
         self.xyz_encoder = MLP(input_dim=self.pos_encoder.out_dim, output_dim=xyz_net_out_dim,
                                net_depth=xyz_net_depth, net_width=xyz_net_width, bias_enabled=False)
@@ -102,7 +105,8 @@ class NGP(nn.Module):
 
     # -- network ----------------------------------------------------------------------------------
     def _fusable(self, x):
-        """True when the stock architecture is in use, so the fused sm_90a MLP kernel applies."""
+        """True when the stock architecture is in use, so the fused sm_90a MLP kernel applies.  Which encode kernel
+        runs with it is the encoder's business (encode_world / enqueue_encode_dyn: hash or tri-plane)."""
         return (x.is_cuda and _fused_mlp_available()
                 and self.pos_encoder.out_dim == 32
                 and self.xyz_encoder.net_depth == 1 and self.xyz_encoder.net_width == 64
@@ -214,14 +218,13 @@ class NGP(nn.Module):
                         self.density_bitfield, count_grid=count)
 
     def _density_eval(self, xyzs_w):
-        """sigma at world positions for the grid update: hash encode (AABB normalisation folded into the kernel) +
+        """sigma at world positions for the grid update: the encoder's kernel (AABB normalisation folded into it) +
         sigma net, straight on the kernels for the stock architecture, NGP.density otherwise."""
         if not self._fusable(xyzs_w):
             return self.density(xyzs_w).float().contiguous()
         from taichi_nerfs_b200 import ops
         from taichi_nerfs_b200.fused_mlp import mlp_weights
         enc = self.pos_encoder
-        table = enc.table_f16() if hasattr(enc, 'table_f16') else enc.hash_table.detach().contiguous()
         aabb = self.__dict__.get('_aabb6')
         if aabb is None:
             aabb = self.__dict__['_aabb6'] = (self.xyz_min.flatten().tolist()
@@ -232,7 +235,7 @@ class NGP(nn.Module):
             dirs = torch.zeros(n, 3, device=xyzs_w.device, dtype=torch.float32)
             dirs[:, 2] = 1.0                       # the sigma head does not depend on the direction
             self.__dict__['_unit_dirs'] = dirs
-        emb = ops.hash_encode_fwd(xyzs_w, table, enc._clayout, enc.out_dim, aabb=aabb)
+        emb = enc.encode_world(xyzs_w, aabb)
         sigmas, _ = ops.mlp_fwd(emb, dirs[:n], [w.detach() for w in mlp_weights(self)])
         return sigmas
 

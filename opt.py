@@ -18,8 +18,9 @@ _FLAGS = [
     ('--model_name', dict(type=str, default='ngp', choices=['ngp'], help='which model to train/test')),
     ('--scale', dict(type=float, default=0.5, help='scene scale (whole scene must lie in [-scale, scale]^3')),
     ('--half_opt', dict(action='store_true', default=False, help='whether to use half optimization')),
-    ('--encoder_type', dict(type=str, default='hash', choices=['hash'],
-                        help='which encoder to use (the reference\'s experimental triplane encoder is out of scope)')),
+    ('--encoder_type', dict(type=str, default='hash', choices=['hash', 'triplane'],
+                        help='which encoder to use: the multiresolution hash grid or the tri-plane encoder (fp32 '
+                             'planes; not with --half_opt, --graph_step or --deployment)')),
     ('--sh_degree', dict(type=int, default=2, help='degree of spherical harmonics (svox only; unused)')),
     ('--grid_size', dict(type=int, default=256, help='size of voxel grid in each dimension (svox only; unused)')),
     ('--grid_radius', dict(type=float, default=0.0125, help='radius of voxel grid points (svox only; unused)')),
@@ -52,4 +53,11 @@ def get_opts(prefix_args=None):
     parser = argparse.ArgumentParser()
     for flag, kw in _FLAGS:
         parser.add_argument(flag, **kw)
-    return parser.parse_args(prefix_args)
+    hparams = parser.parse_args(prefix_args)
+    if hparams.encoder_type == 'triplane':
+        for flag, why in (('half_opt', 'the tri-plane table is fp32 (an fp16 plane table is not supported)'),
+                          ('graph_step', 'the graph-captured step runs the hash encoder only'),
+                          ('deployment', 'the deployment export (mobile demo format) is hash-only')):
+            if getattr(hparams, flag):
+                parser.error(f"--encoder_type triplane does not combine with --{flag}: {why}")
+    return hparams

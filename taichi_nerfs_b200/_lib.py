@@ -10,7 +10,7 @@ import ctypes as C
 import os
 import threading
 
-from .layout import CHashLayout
+from .layout import CHashLayout, CTriplaneLayout
 
 _PKG = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_PKG, "lib", "libngp_b200.so")
@@ -32,6 +32,7 @@ class NgpError(RuntimeError):
 def _declare(lib):
     i64, i32, f32, vp, ci = C.c_int64, C.c_int32, C.c_float, C.c_void_p, C.c_int
     lay = C.POINTER(CHashLayout)
+    tri = C.POINTER(CTriplaneLayout)
     mw = C.POINTER(MlpWeights)
     sigs = {
         "ngp_version": (ci, []),
@@ -48,6 +49,9 @@ def _declare(lib):
         "ngp_hash_encode_fwd_dyn": (ci, [vp, vp, lay, vp, ci, i64, vp, vp, vp]),
         "ngp_hash_encode_bwd_dyn": (ci, [vp, vp, ci, lay, vp, i64, vp, vp, vp]),
         "ngp_hash_encode_bwd_levels": (ci, [vp, vp, ci, lay, vp, i64, vp, vp, ci, ci, vp, vp]),
+        "ngp_triplane_encode_fwd": (ci, [vp, vp, tri, vp, i64, vp, vp]),
+        "ngp_triplane_encode_fwd_dyn": (ci, [vp, vp, tri, vp, i64, vp, vp, vp]),
+        "ngp_triplane_encode_bwd": (ci, [vp, vp, vp, tri, vp, i64, vp]),
         "ngp_mlp_fwd_dyn": (ci, [vp, ci, vp, mw, vp, vp, vp, i64, vp, vp]),
         "ngp_mlp_bwd_dyn": (ci, [vp, ci, vp, mw, vp, vp, vp, vp, vp, i64, vp, vp, vp]),
         "ngp_adam_step_dyn": (ci, [vp, vp, vp, vp, vp, vp, vp, f32, f32, f32, ci, i64, vp]),

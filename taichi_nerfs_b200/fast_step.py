@@ -37,6 +37,9 @@ class StaticTrainStep:
         enc = m.pos_encoder
         if not m._fusable(next(m.parameters())):
             raise _lib.NgpError("StaticTrainStep needs the stock NGP architecture (fused MLP)")
+        if not hasattr(enc, "hash_table"):
+            raise _lib.NgpError("StaticTrainStep runs the hash encoder's kernels; the graph-captured step does not "
+                                "support the tri-plane encoder (train it without --graph_step)")
         dev = next(m.parameters()).device
         self.dev, self.n = dev, int(n_rays)
         self.cap = C_ = int(n_rays) * int(samples_per_ray_capacity)

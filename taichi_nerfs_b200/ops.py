@@ -133,6 +133,32 @@ def hash_encode_bwd_input(xyz, table, dout, clayout):
     return dx
 
 
+# ---- tri-plane encoder -----------------------------------------------------------------------------
+def triplane_encode_fwd(xyz, table, clayout, aabb=None, out=None):
+    """xyz [n,3] fp32 in [0,1] (or world positions with aabb = (xyz_min[3], xyz_max-xyz_min[3]), normalised in the
+    kernel) -> fp32 [n, L*F] in the reference's feature-major column order."""
+    _need_cuda(xyz, table, out)
+    if xyz.dtype != torch.float32 or table.dtype != torch.float32:
+        raise TypeError("triplane_encode_fwd: positions and the plane table must be fp32")
+    n = xyz.shape[0]
+    if out is None:
+        out = torch.empty(n, clayout.n_levels * clayout.feat_dim, device=xyz.device, dtype=torch.float32)
+    a6 = None if aabb is None else (C.c_float * 6)(*[float(v) for v in aabb])
+    check(load().ngp_triplane_encode_fwd(_ptr(xyz), _ptr(table), C.byref(clayout), _ptr(out), n, a6, _stream()),
+          "triplane_encode_fwd")
+    return out
+
+
+def triplane_encode_bwd(xyz, table, dout, clayout, grad_table):
+    """grad_table (fp32 [P]) += dL/dtable for dout fp32 [n, L*F]; xyz in [0,1]."""
+    _need_cuda(xyz, table, dout, grad_table)
+    if dout.dtype != torch.float32 or grad_table.dtype != torch.float32:
+        raise TypeError("triplane_encode_bwd: dout and grad_table must be fp32")
+    check(load().ngp_triplane_encode_bwd(_ptr(xyz), _ptr(table), _ptr(dout), C.byref(clayout), _ptr(grad_table),
+                                         xyz.shape[0], _stream()), "triplane_encode_bwd")
+    return grad_table
+
+
 # ---- a6 ------------------------------------------------------------------------------------------
 def dir_encode(dirs):
     _need_cuda(dirs)

@@ -19,8 +19,10 @@ DENSITY_THRESHOLD = 0.01 * 1024 / 3 ** 0.5   # train.py:180
 
 def train_vs_teacher(device, steps: int = 3000, batch: int = 8192, train_views: int = 48, test_views: int = 4,
                      downsample: float = 0.5, seed: int = 23, half_opt: bool = True, graph: bool = True,
-                     teacher=None, log=None):
-    """Returns {"psnr": mean dB over the held-out views, "psnr_views": [...], "steps": ..., "steps_per_s": ...,
+                     teacher=None, log=None, pos_encoder_type: str = 'hash'):
+    """pos_encoder_type='triplane' trains the reference's tri-plane model instead (fp32 planes: half_opt does not
+    apply and the loss scale is 2**19, as train.py without --half_opt; the graph-captured step is hash-only, so pass
+    graph=False).  Returns {"psnr": mean dB over the held-out views, "psnr_views": [...], "steps": ..., "steps_per_s": ...,
     "rays_per_s": ..., "model": the trained NGP} or None when the teacher fixture is not staged."""
     from datasets.ray_utils import get_rays
     from datasets.teacher import TeacherLego, load_teacher
@@ -39,7 +41,9 @@ def train_vs_teacher(device, steps: int = 3000, batch: int = 8192, train_views: 
     test_ds.build_image_bank(teacher)
 
     torch.manual_seed(seed)
-    model = NGP(scale=0.5, max_res=1024, half_opt=half_opt).to(device)
+    if pos_encoder_type == 'triplane':
+        half_opt = False
+    model = NGP(scale=0.5, max_res=1024, half_opt=half_opt, pos_encoder_type=pos_encoder_type).to(device)
     model.mark_invisible_cells(train_ds.K, train_ds.poses, train_ds.img_wh)
     trainer = NGPTrainer(model, lr=1e-2, max_steps=steps)
     fast = None

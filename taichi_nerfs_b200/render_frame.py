@@ -31,10 +31,8 @@ def render_frame(model, rays_o, rays_d, exp_step_factor=0.0, T_threshold=1e-4, m
     depth = torch.empty(n, device=dev, dtype=torch.float32)
     opacity = torch.empty(n, device=dev, dtype=torch.float32)
     enc = model.pos_encoder
-    half = hasattr(enc, "table_f16")
-    fused = bool(model._fusable(rays_o))     # stock architecture: hash + fused MLP kernels on the raw sample rows
+    fused = bool(model._fusable(rays_o))     # stock architecture: encoder + fused MLP kernels on the raw sample rows
     if fused:
-        table = enc.table_f16() if half else enc.hash_table.detach().contiguous()
         W = [w.detach() for w in mlp_weights(model)]
     aabb = model.xyz_min.flatten().tolist() + (model.xyz_max - model.xyz_min).flatten().tolist()
     total = 0
@@ -83,7 +81,7 @@ def render_frame(model, rays_o, rays_d, exp_step_factor=0.0, T_threshold=1e-4, m
             rgb[b:e] = 0
             continue
         if fused:
-            emb = ops.hash_encode_fwd(xyzs, table, enc._clayout, enc.out_dim, aabb=aabb)  # normalisation in-kernel
+            emb = enc.encode_world(xyzs, aabb)  # hash or tri-plane kernel, normalisation in-kernel
             sigmas, rgbs = ops.mlp_fwd(emb, dirs, W)
         else:   # any other NGP configuration (e.g. the reference's L=4 F=4 deployment model): module forward
             with torch.autocast('cuda', dtype=torch.float16):
@@ -127,9 +125,8 @@ class FrameRenderer:
         self.dev, self.n = dev, int(n_rays)
         self.cap = int(n_rays) * int(rows_per_ray)
         self.esf, self.T_thr = float(exp_step_factor), float(T_threshold)
-        self.half = hasattr(enc, "table_f16")
-        self.tag = F16 if self.half else F32
-        edt = torch.float16 if self.half else torch.float32
+        edt = enc.emb_dtype     # fp16 (half_opt hash) or fp32 (fp32 hash, tri-plane) embedding
+        self.tag = F16 if edt == torch.float16 else F32
         f32, i32 = torch.float32, torch.int32
         z = lambda *s, dtype=f32: torch.zeros(*s, device=dev, dtype=dtype)  # noqa: E731
         n, cap = self.n, self.cap
@@ -153,7 +150,6 @@ class FrameRenderer:
         self._w_keep = [w.detach().float().contiguous() for w in mlp_weights(model)]
         self._wst = MlpWeights(*[w.data_ptr() for w in self._w_keep])
         self._w_ptrs = [w.data_ptr() for w in mlp_weights(model)]
-        self._clayout = enc._clayout
         self.rays_o[:] = torch.tensor([1.2, 0.3, 0.5], device=dev)      # valid placeholder rays for the capture
         self.rays_d[:] = -self.rays_o
         self.graph = None
@@ -165,8 +161,7 @@ class FrameRenderer:
         return None if t is None else self._C.c_void_p(t.data_ptr())
 
     def _table(self):
-        enc = self.model.pos_encoder
-        return enc.table_f16() if self.half else enc.hash_table.detach()
+        return self.model.pos_encoder.kernel_table()
 
     def _enqueue_round(self, j, limit):
         L, m, st, p, check = self._load(), self.model, self._C.c_void_p(torch.cuda.current_stream().cuda_stream), self._p, self._check
@@ -177,8 +172,8 @@ class FrameRenderer:
                                              self.MAX_SAMPLES, p(cur), p(self.state), p(self.t_cur), p(self.n_marched),
                                              p(self.rays_a), p(self.xyzs), p(self.dirs), p(self.deltas), p(self.ts),
                                              self.n, self.cap, p(self.coarse), st))
-        check(L.ngp_hash_encode_fwd_dyn(p(self.xyzs), p(self._table_t), self._C.byref(self._clayout), p(self.emb), self.tag,
-                                        self.cap, p(self.state), self.aabb6, st))
+        check(m.pos_encoder.enqueue_encode_dyn(L, p(self.xyzs), p(self._table_t), p(self.emb), self.cap, p(self.state),
+                                               self.aabb6, st))
         check(L.ngp_mlp_fwd_dyn(p(self.emb), self.tag, p(self.dirs), self._C.byref(self._wst), p(self.sig), p(self.rgbs),
                                 None, self.cap, p(self.state), st))
         check(L.ngp_composite_round(p(self.sig), p(self.rgbs), 1, p(self.deltas), p(self.ts), p(self.rays_a),
@@ -217,7 +212,7 @@ class FrameRenderer:
         tab = self._table()
         if self.graph is not None and tab.data_ptr() == self._table_ptr:
             self.graph.replay()
-        else:   # eager enqueue (no graph, or the fp16 shadow table was re-allocated since the capture)
+        else:   # eager enqueue (no graph, or the table the encoder reads was re-allocated since the capture)
             self._table_t = tab
             self._enqueue_frame()
         rounds = len(self.SCHEDULE)

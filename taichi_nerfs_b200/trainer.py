@@ -78,7 +78,8 @@ class NGPTrainer:
                 self.flat_param[off:off + s].copy_(p.data.reshape(-1))
             p.data = self.flat_param[off:off + s].view_as(p)
             off += s + q
-            if p is getattr(model.pos_encoder, 'hash_table', None):
+            if (p is getattr(model.pos_encoder, 'hash_table', None)
+                    or p is getattr(model.pos_encoder, 'plane_embedding', None)):
                 model.pos_encoder.grad_sink = self.flat_grad[off - s - q:off - q]
         self.found_inf = torch.zeros(1, device=dev, dtype=torch.int32)
         # device-side optimizer scalars (shared with StaticTrainStep): iteration counter, [lr/bc1, sqrt(bc2), 1/(scale*world),
@@ -112,6 +113,9 @@ class NGPTrainer:
         # (opt-in, NGP_SHARDED_ADAM=1: on 2 GPUs its four collectives cost more than the bytes they save)
         want = (sharded_optimizer if sharded_optimizer is not None
                 else os.environ.get("NGP_SHARDED_ADAM", "0") == "1")
+        if (want or p2p_optimizer) and hasattr(model.pos_encoder, 'plane_embedding'):
+            raise ValueError("NGPTrainer: the sharded and peer-memory optimizers shard the fp16 hash table; a tri-plane "
+                             "model uses the all-reduce of the flat gradient (sharded_optimizer / p2p_optimizer off)")
         self.sharded = bool((want or self.p2p is not None) and self.world_size > 1 and self._shadow_full is not None
                             and P % (4 * self.world_size) == 0 and self.slices[0][0] == 0)
         if self.sharded:

@@ -88,6 +88,8 @@ def main(prefix_args=None):
     if hparams.graph_step:
         if hparams.distortion_loss_w > 0 or not model._fusable(next(model.parameters())):
             raise ValueError("--graph_step needs the stock NGP architecture and --distortion_loss_w 0")
+        if getattr(model, 'pos_encoder_type', 'hash') != 'hash':
+            raise ValueError("--graph_step runs the hash encoder only; train a tri-plane model without it")
         from taichi_nerfs_b200.fast_step import StaticTrainStep
         fast = StaticTrainStep(trainer, hparams.batch_size, exp_step_factor=exp_step_factor)
 
