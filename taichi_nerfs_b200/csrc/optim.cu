@@ -18,12 +18,15 @@ struct AdamArgs {
     int zero_grad;
 };
 
+// The FMA contractions are spelled out: left to nvcc they differed between the fp32- and fp16-gradient instantiations
+// (v * beta2 rounded first in one, ((1-beta2)*gg)*gg in the other), so the multi-GPU fp16 path drifted by an ulp from
+// the single-GPU path on identical gradients.  These are the contractions the fp32 instantiation had.
 __device__ __forceinline__ void adam1(float& p, float& g, float& m, float& v, const AdamArgs& a) {
-    const float gg = g * a.inv_scale;
-    m = m + (gg - m) * (1.0f - a.beta1);                 // exp_avg.lerp_(grad, 1-beta1)
-    v = v * a.beta2 + (1.0f - a.beta2) * gg * gg;        // exp_avg_sq.mul_(beta2).addcmul_(g,g,1-beta2)
-    const float denom = sqrtf(v) / a.bc2_sqrt + a.eps;
-    p = p - a.lr_over_bc1 * (m / denom);
+    const float gg = __fmul_rn(g, a.inv_scale);
+    m = __fmaf_rn(__fsub_rn(gg, m), 1.0f - a.beta1, m);                           // exp_avg.lerp_(grad, 1-beta1)
+    v = __fmaf_rn(v, a.beta2, __fmul_rn(__fmul_rn(1.0f - a.beta2, gg), gg));       // .mul_(beta2).addcmul_(g,g,1-beta2)
+    const float denom = __fadd_rn(__fdiv_rn(sqrtf(v), a.bc2_sqrt), a.eps);
+    p = __fmaf_rn(-a.lr_over_bc1, __fdiv_rn(m, denom), p);
 }
 
 // TGrad = float: the gradient is read from (and zeroed in) `grad`.  TGrad = __half: the gradient comes from the fp16
