@@ -10,8 +10,9 @@
 // shared memory), WARP w handles LEVEL w and each lane walks a chunk of 16 consecutive samples.
 // Consecutive samples of a ray are <= 1 finest-level cell apart, so (a) the forward re-gathers the
 // 8 corners only when the cell changes (37x fewer loads at level 0, ~1x at the finest levels),
-// (b) the backward accumulates w*dy in registers and issues its 8 vector atomics only at cell
-// changes, and (c) all lanes of a warp stay inside one level's table slab (L1/L2 locality).
+// (b) the backward accumulates w*dy in registers and issues its vector atomics only at cell
+// changes, for the corners the new cell does not share with the old one, and (c) all lanes of a
+// warp stay inside one level's table slab (L1/L2 locality).
 // The fp16 table (21.8 MiB) and the fp32 gradient (43.6 MiB) together exceed the H100's 50 MB L2; how much of
 // the gathers and atomics L2 serves has not been measured on the H100.  Results are staged in shared memory
 // ([level][sample], chunk stride 17 words = conflict-free) and written with coalesced stores in
@@ -114,6 +115,44 @@ __device__ __forceinline__ void corner_weights(const float pos[3], float w[8]) {
     for (int c = 0; c < 4; ++c) axy[c] = f_mul(ax[c & 1], ay[c >> 1]);
 #pragma unroll
     for (int c = 0; c < 8; ++c) w[c] = f_mul(axy[c & 3], az[c >> 2]);
+}
+
+// Corner reuse between consecutive cells.  When a lane moves from cell pg to cell g and every per-axis offset
+// g - pg is in {-1, 0, 1}, corner c' of g is corner c' + (g - pg) of pg whenever that lies in {0, 1}^3: the same grid
+// coordinate, so the same table entry on dense and hashed levels alike.  Corner masks are 8-bit sets over c = x + 2y + 4z.
+struct CellStep {
+    uint32_t carried;  // corners of the new cell that are corners of the old one
+    uint32_t stays;    // corners of the old cell that are corners of the new one (the others leave)
+    int32_t d[3];
+};
+
+__device__ __forceinline__ CellStep cell_step(const uint32_t pg[3], const uint32_t g[3]) {
+    constexpr uint32_t kLow[3] = {0x55u, 0x33u, 0x0Fu};  // corners with bit d clear; the complement has it set
+    CellStep s;
+    s.carried = s.stays = 0xFFu;
+#pragma unroll
+    for (int d = 0; d < 3; ++d) {
+        s.d[d] = (int32_t)(g[d] - pg[d]);
+        const uint32_t lo = kLow[d], hi = ~kLow[d] & 0xFFu;
+        s.carried &= s.d[d] == 0 ? 0xFFu : s.d[d] == 1 ? lo : s.d[d] == -1 ? hi : 0u;
+        s.stays &= s.d[d] == 0 ? 0xFFu : s.d[d] == 1 ? hi : s.d[d] == -1 ? lo : 0u;
+    }
+    return s;
+}
+
+// moves the carried corners' values to their places in the new cell, axis by axis (compile-time indices, selects);
+// the slots of corners that are not carried are left holding stale values
+__device__ __forceinline__ void shift_corners(float2 a[8], const CellStep& s) {
+#pragma unroll
+    for (int d = 0; d < 3; ++d) {
+#pragma unroll
+        for (int c = 0; c < 8; ++c) {
+            if (c & (1 << d)) continue;
+            const float2 lo = a[c], hi = a[c | (1 << d)];
+            a[c] = s.d[d] == 1 ? hi : lo;
+            a[c | (1 << d)] = s.d[d] == -1 ? lo : hi;
+        }
+    }
 }
 
 template <typename T>
@@ -253,7 +292,10 @@ __global__ void __launch_bounds__(kThreads) hash_fwd_kernel(const float* __restr
 // ---- backward wrt table ------------------------------------------------------------------------------
 // Consecutive samples of a ray stay in the same cell for 1/(res*dt) steps (37 at level 0 down to ~1
 // at the finest levels), so a lane accumulates w*dy for its 16-sample chunk in registers and issues
-// the 8 vector atomics only when the cell changes: ~2.3x fewer L2 atomics on Lego-shape rays.
+// the 8 vector atomics only when the cell changes: ~2.3x fewer L2 atomics on Lego-shape rays.  When the
+// new cell is a neighbour of the old one, only the corners that leave are scattered and the shared ones
+// keep accumulating (cell_step): another 25 % fewer atomics on the lego_half sample stream
+// (scripts/hash_corner_reuse.py).  The forward does not carry corners: there it saved loads but not time.
 template <typename T>
 __global__ void __launch_bounds__(kThreads) hash_bwd_kernel(const float* __restrict__ xyz,
                                                             const T* __restrict__ dout,
@@ -314,19 +356,22 @@ __global__ void __launch_bounds__(kThreads) hash_bwd_kernel(const float* __restr
     bool pending = false;
     bool bad = false;   // a non-finite contribution: raised at the source, so that no separate pass over the 45 MB
                         // gradient buffer is needed for GradScaler's inf check (optional, found_inf may be NULL)
-    auto flush = [&]() {
+    // scatters the corners of cell pg in `leaving` (the others are carried into the next cell)
+    auto flush = [&](uint32_t leaving) {
         uint32_t idx[8];
         corner_indices(m, pg, idx);
 #pragma unroll
-        for (int c = 0; c < 8; ++c) bad = bad || !(fabsf(acc[c].x) < INFINITY) || !(fabsf(acc[c].y) < INFINITY);
+        for (int c = 0; c < 8; ++c)
+            if ((leaving >> c) & 1u) bad = bad || !(fabsf(acc[c].x) < INFINITY) || !(fabsf(acc[c].y) < INFINITY);
 #pragma unroll
         for (int c = 0; c < 8; c += 2) {
-            if ((idx[c] ^ idx[c + 1]) == 1u) {  // x-neighbours in one aligned 16-byte block: one L2 atomic
+            const bool out0 = (leaving >> c) & 1u, out1 = (leaving >> (c + 1)) & 1u;
+            if (out0 && out1 && (idx[c] ^ idx[c + 1]) == 1u) {  // x-neighbours in one aligned 16-byte block: one L2 atomic
                 const float2 lo = (idx[c] & 1u) ? acc[c + 1] : acc[c], hi = (idx[c] & 1u) ? acc[c] : acc[c + 1];
                 atomicAdd(reinterpret_cast<float4*>(g2 + (idx[c] & ~1u)), make_float4(lo.x, lo.y, hi.x, hi.y));
             } else {
-                atomicAdd(g2 + idx[c], acc[c]);  // red.global.add.v2.f32
-                atomicAdd(g2 + idx[c + 1], acc[c + 1]);
+                if (out0) atomicAdd(g2 + idx[c], acc[c]);  // red.global.add.v2.f32
+                if (out1) atomicAdd(g2 + idx[c + 1], acc[c + 1]);
             }
         }
     };
@@ -344,12 +389,19 @@ __global__ void __launch_bounds__(kThreads) hash_bwd_kernel(const float* __restr
         float pos[3];
         grid_pos<kHalf>(x, m, g, pos);
         if (!pending || g[0] != pg[0] || g[1] != pg[1] || g[2] != pg[2]) {
-            if (pending) flush();
+            uint32_t carried = 0u;
+            if (pending) {
+                const CellStep st = cell_step(pg, g);
+                flush(~st.stays & 0xFFu);
+                shift_corners(acc, st);
+                carried = st.carried;
+            }
             pg[0] = g[0];
             pg[1] = g[1];
             pg[2] = g[2];
 #pragma unroll
-            for (int c = 0; c < 8; ++c) acc[c] = make_float2(0.0f, 0.0f);
+            for (int c = 0; c < 8; ++c)
+                if (!((carried >> c) & 1u)) acc[c] = make_float2(0.0f, 0.0f);
             pending = true;
         }
         float w[8];
@@ -360,7 +412,7 @@ __global__ void __launch_bounds__(kThreads) hash_bwd_kernel(const float* __restr
             acc[c].y += w[c] * dy.y;
         }
     }
-    if (pending) flush();
+    if (pending) flush(0xFFu);
     if (bad && found_inf != nullptr) *found_inf = 1;
 }
 
