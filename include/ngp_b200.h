@@ -206,6 +206,12 @@ int ngp_hash_encode_bwd_dyn(const float* xyz, const void* dout, int dout_dtype, 
 int ngp_hash_encode_bwd_levels(const float* xyz, const void* dout, int dout_dtype, const ngp_hash_layout* layout,
                                float* grad_table, int64_t n_max, const int32_t* n_dev, const float* aabb6,
                                int level_begin, int level_end, int32_t* found_inf_or_null, void* stream);
+/* The level groups the F = 2 table backward above scatters one launch at a time, for an L2 of l2_bytes (the
+ * backward passes the current device's when n_max >= 2^20 rows, else 0: one group): consecutive groups covering [level_begin, level_end), each one's fp32
+ * gradient slice at most half of l2_bytes unless it is a single level.  Writes the group boundaries
+ * bounds[0] = level_begin < ... < bounds[G] = level_end (room for NGP_MAX_LEVELS + 1) and returns G, or < 0. */
+int ngp_hash_bwd_level_groups(const ngp_hash_layout* layout, int level_begin, int level_end, int64_t l2_bytes,
+                              int32_t* bounds);
 int ngp_mlp_fwd_dyn(const void* emb, int emb_dtype, const float* dirs, const ngp_mlp_weights* w, float* sigmas,
                     void* rgbs_f16, void* save, int64_t n_max, const int32_t* n_dev, void* stream);
 int ngp_mlp_bwd_dyn(const void* emb, int emb_dtype, const float* dirs, const ngp_mlp_weights* w, const void* save,

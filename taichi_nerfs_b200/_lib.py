@@ -49,6 +49,7 @@ def _declare(lib):
         "ngp_hash_encode_fwd_dyn": (ci, [vp, vp, lay, vp, ci, i64, vp, vp, vp]),
         "ngp_hash_encode_bwd_dyn": (ci, [vp, vp, ci, lay, vp, i64, vp, vp, vp]),
         "ngp_hash_encode_bwd_levels": (ci, [vp, vp, ci, lay, vp, i64, vp, vp, ci, ci, vp, vp]),
+        "ngp_hash_bwd_level_groups": (ci, [lay, ci, ci, i64, vp]),
         "ngp_triplane_encode_fwd": (ci, [vp, vp, tri, vp, i64, vp, vp]),
         "ngp_triplane_encode_fwd_dyn": (ci, [vp, vp, tri, vp, i64, vp, vp, vp]),
         "ngp_triplane_encode_bwd": (ci, [vp, vp, vp, tri, vp, i64, vp]),

@@ -13,10 +13,14 @@
 // (b) the backward accumulates w*dy in registers and issues its vector atomics only at cell
 // changes, for the corners the new cell does not share with the old one, and (c) all lanes of a
 // warp stay inside one level's table slab (L1/L2 locality).
-// The fp16 table (21.8 MiB) and the fp32 gradient (43.6 MiB) together exceed the H100's 50 MB L2; how much of
-// the gathers and atomics L2 serves has not been measured on the H100.  Results are staged in shared memory
+// The fp32 gradient (43.6 MiB) and the streams of one launch exceed the H100's 50 MB L2, and the scatter is sensitive
+// to that (scripts/hash_l2_probe.py: the same requests into an 8x smaller gradient run 1.58x faster; the forward's
+// gathers only 1.04x).  So a large backward scatters one level group at a time, each group's gradient slice at most
+// half the L2, with evict-first loads of dL/dout and evict-last atomics.  Results are staged in shared memory
 // ([level][sample], chunk stride 17 words = conflict-free) and written with coalesced stores in
 // the reference's [n, L*F] row-major layout.
+#include <atomic>
+
 #include "common.cuh"
 
 namespace {
@@ -153,6 +157,39 @@ __device__ __forceinline__ void shift_corners(float2 a[8], const CellStep& s) {
             a[c | (1 << d)] = s.d[d] == -1 ? lo : hi;
         }
     }
+}
+
+// Per-instruction L2 eviction priorities (PTX createpolicy + .L2::cache_hint; no persisting-L2 set-aside is needed)
+__device__ __forceinline__ uint64_t l2_evict_first() {
+    uint64_t p;
+    asm("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
+    return p;
+}
+__device__ __forceinline__ uint64_t l2_evict_last() {
+    uint64_t p;
+    asm("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p));
+    return p;
+}
+__device__ __forceinline__ uint64_t l2_evict_normal() {
+    uint64_t p;
+    asm("createpolicy.fractional.L2::evict_normal.b64 %0, 1.0;" : "=l"(p));
+    return p;
+}
+__device__ __forceinline__ uint4 ldg_hint(const uint4* p, uint64_t pol) {
+    uint4 v;
+    asm("ld.global.nc.L2::cache_hint.v4.u32 {%0, %1, %2, %3}, [%4], %5;"
+        : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w)
+        : "l"(p), "l"(pol));
+    return v;
+}
+__device__ __forceinline__ void red_add_hint(float2* p, float2 v, uint64_t pol) {
+    asm volatile("red.global.add.L2::cache_hint.v2.f32 [%0], {%1, %2}, %3;" ::"l"(p), "f"(v.x), "f"(v.y), "l"(pol)
+                 : "memory");
+}
+__device__ __forceinline__ void red_add_hint(float4* p, float4 v, uint64_t pol) {
+    asm volatile("red.global.add.L2::cache_hint.v4.f32 [%0], {%1, %2, %3, %4}, %5;" ::"l"(p), "f"(v.x), "f"(v.y),
+                 "f"(v.z), "f"(v.w), "l"(pol)
+                 : "memory");
 }
 
 template <typename T>
@@ -302,9 +339,10 @@ __global__ void __launch_bounds__(kThreads) hash_bwd_kernel(const float* __restr
                                                             const __grid_constant__ ngp_hash_layout lay,
                                                             float* __restrict__ grad_table, int64_t n_max,
                                                             const Dyn dyn, int level_begin, int level_end,
-                                                            int32_t* __restrict__ found_inf) {
-    // blockDim.x = 32 * (level_end - level_begin): warp w scatters level level_begin + w (the multi-GPU step launches
-    // the levels in groups so that a finished group's table slice is all-reduced while the next group runs)
+                                                            int32_t* __restrict__ found_inf, int grouped) {
+    // blockDim.x = 32 * (level_end - level_begin): warp w scatters level level_begin + w.  The host launches one level
+    // group at a time (bwd_level_groups), so only the group's dL/dout columns are staged: tile row w = level
+    // level_begin + w.
     using V2 = typename Vec2<T>::type;
     const int64_t n = effective_n(dyn, n_max);
     constexpr bool kHalf = sizeof(T) == 2;
@@ -326,21 +364,28 @@ __global__ void __launch_bounds__(kThreads) hash_bwd_kernel(const float* __restr
         }
         reinterpret_cast<float4*>(sx)[r + r / kChunk] = make_float4(v[0], v[1], v[2], 0.0f);
     }
+    // grouped launches: dL/dout is read once, evict-first, so that it does not push the gradient slice being
+    // scattered out of L2.  A launch that is the only group keeps the default priorities: an evict-last gradient left
+    // in L2 after it slowed the small-batch step more than the hints sped the launch up.
+    const uint64_t stream_pol = grouped ? l2_evict_first() : l2_evict_normal();
     const V2* d2 = reinterpret_cast<const V2*>(dout) + base * L;
     constexpr int kVec = 16 / sizeof(V2);
     if (L % kVec == 0 && (reinterpret_cast<uintptr_t>(dout) & 15) == 0) {
-        const int groups = L / kVec;
+        // 16-byte loads over the aligned column blocks that cover [level_begin, level_end)
+        const int v0 = level_begin / kVec, groups = (level_end + kVec - 1) / kVec - v0;
         for (int k = threadIdx.x; k < rows * groups; k += nthreads) {
-            const int r = k / groups, l0 = (k - r * groups) * kVec;
-            const uint4 raw = __ldg(reinterpret_cast<const uint4*>(d2 + (int64_t)r * L + l0));
+            const int r = k / groups, l0 = (v0 + k - r * groups) * kVec;
+            const uint4 raw = ldg_hint(reinterpret_cast<const uint4*>(d2 + (int64_t)r * L + l0), stream_pol);
             const V2* v = reinterpret_cast<const V2*>(&raw);
 #pragma unroll
-            for (int q = 0; q < kVec; ++q) tile[(l0 + q) * kRow + r + r / kChunk] = v[q];
+            for (int q = 0; q < kVec; ++q)
+                if (l0 + q >= level_begin && l0 + q < level_end) tile[(l0 + q - level_begin) * kRow + r + r / kChunk] = v[q];
         }
     } else {
-        for (int k = threadIdx.x; k < rows * L; k += nthreads) {
-            const int r = k / L, l = k - r * L;
-            tile[l * kRow + r + r / kChunk] = d2[k];
+        const int nl = level_end - level_begin;
+        for (int k = threadIdx.x; k < rows * nl; k += nthreads) {
+            const int r = k / nl, l = k - r * nl;
+            tile[l * kRow + r + r / kChunk] = d2[(int64_t)r * L + level_begin + l];
         }
     }
     __syncthreads();
@@ -349,7 +394,10 @@ __global__ void __launch_bounds__(kThreads) hash_bwd_kernel(const float* __restr
     if (level >= L || level >= level_end) return;
     const LevelMeta m = level_meta(lay, level);
     float2* g2 = reinterpret_cast<float2*>(grad_table);
-    const V2* trow = tile + level * kRow + lane * (kChunk + 1);
+    const V2* trow = tile + (level - level_begin) * kRow + lane * (kChunk + 1);
+    // the group's gradient slice is sized to stay in L2 for the whole launch (bwd_level_groups); evict-last keeps it
+    // there against the streams
+    const uint64_t grad_pol = grouped ? l2_evict_last() : l2_evict_normal();
 
     uint32_t pg[3] = {0u, 0u, 0u};
     float2 acc[8];
@@ -368,10 +416,10 @@ __global__ void __launch_bounds__(kThreads) hash_bwd_kernel(const float* __restr
             const bool out0 = (leaving >> c) & 1u, out1 = (leaving >> (c + 1)) & 1u;
             if (out0 && out1 && (idx[c] ^ idx[c + 1]) == 1u) {  // x-neighbours in one aligned 16-byte block: one L2 atomic
                 const float2 lo = (idx[c] & 1u) ? acc[c + 1] : acc[c], hi = (idx[c] & 1u) ? acc[c] : acc[c + 1];
-                atomicAdd(reinterpret_cast<float4*>(g2 + (idx[c] & ~1u)), make_float4(lo.x, lo.y, hi.x, hi.y));
+                red_add_hint(reinterpret_cast<float4*>(g2 + (idx[c] & ~1u)), make_float4(lo.x, lo.y, hi.x, hi.y), grad_pol);
             } else {
-                if (out0) atomicAdd(g2 + idx[c], acc[c]);  // red.global.add.v2.f32
-                if (out1) atomicAdd(g2 + idx[c + 1], acc[c + 1]);
+                if (out0) red_add_hint(g2 + idx[c], acc[c], grad_pol);
+                if (out1) red_add_hint(g2 + idx[c + 1], acc[c + 1], grad_pol);
             }
         }
     };
@@ -573,6 +621,28 @@ Dyn make_dyn(const int32_t* n_dev, const float* aabb6) {
     return d;
 }
 
+// Share of the L2 that one level group's fp32 gradient slice may fill.  The rest holds what streams through during the
+// launch (dL/dout, xyz) and the lines in flight; DESIGN.md §4 has the measurements behind the value.
+constexpr int64_t kL2BudgetNum = 1, kL2BudgetDen = 2;
+// Launches of fewer rows stay one group: they scatter too few requests per gradient line for the residency to pay for
+// the extra launches (measured: the 393 k-row lego_fp32_1024 step got slower grouped, the 3.1 M-row lego_half and
+// 8.4 M-row garden16 steps faster).
+constexpr int64_t kGroupMinRows = 1 << 20;
+
+// L2 size of the current device, queried once per device.  Attribute queries are not stream operations, so this is
+// legal while a stream is being captured.
+int64_t device_l2_bytes() {
+    constexpr int kMaxDevices = 64;
+    static std::atomic<int> cached[kMaxDevices];
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess) return 0;
+    if (dev < kMaxDevices && cached[dev].load(std::memory_order_relaxed) > 0) return cached[dev].load(std::memory_order_relaxed);
+    int bytes = 0;
+    if (cudaDeviceGetAttribute(&bytes, cudaDevAttrL2CacheSize, dev) != cudaSuccess || bytes <= 0) return 0;
+    if (dev < kMaxDevices) cached[dev].store(bytes, std::memory_order_relaxed);
+    return bytes;
+}
+
 int check_layout(const ngp_hash_layout* lay) {
     NGP_REQUIRE(lay != nullptr, "null layout");
     NGP_REQUIRE(lay->n_levels >= 1 && lay->n_levels <= NGP_MAX_LEVELS, "n_levels out of range");
@@ -652,13 +722,43 @@ int ngp_hash_encode_bwd_levels(const float* xyz, const void* dout, int dout_dtyp
     }
     const unsigned grid = (unsigned)((n + kTile - 1) / kTile);
     if (int rc = configure_smem()) return rc;
-    const unsigned threads = 32u * (unsigned)(level_end - level_begin);
-    if (dout_dtype == NGP_F16)
-        hash_bwd_kernel<__half><<<grid, threads, smem_bytes(layout->n_levels, 4), st>>>(xyz, (const __half*)dout, *layout, grad_table, n, dyn, level_begin, level_end, found_inf_or_null);
-    else
-        hash_bwd_kernel<float><<<grid, threads, smem_bytes(layout->n_levels, 8), st>>>(xyz, (const float*)dout, *layout, grad_table, n, dyn, level_begin, level_end, found_inf_or_null);
-    NGP_LAUNCHED("hash_bwd_kernel");
+    // one launch per level group, in level order: each launch's scatter stays inside an L2-sized gradient slice
+    int32_t bounds[NGP_MAX_LEVELS + 1];
+    const int64_t l2 = n >= kGroupMinRows ? device_l2_bytes() : 0;
+    const int n_groups = ngp_hash_bwd_level_groups(layout, level_begin, level_end, l2, bounds);
+    for (int g = 0; g < n_groups; ++g) {
+        const int a = bounds[g], b = bounds[g + 1];
+        const unsigned threads = 32u * (unsigned)(b - a);
+        if (dout_dtype == NGP_F16)
+            hash_bwd_kernel<__half><<<grid, threads, smem_bytes(b - a, 4), st>>>(xyz, (const __half*)dout, *layout, grad_table, n, dyn, a, b, found_inf_or_null, n_groups > 1);
+        else
+            hash_bwd_kernel<float><<<grid, threads, smem_bytes(b - a, 8), st>>>(xyz, (const float*)dout, *layout, grad_table, n, dyn, a, b, found_inf_or_null, n_groups > 1);
+        NGP_LAUNCHED("hash_bwd_kernel");
+    }
     return 0;
+}
+
+int ngp_hash_bwd_level_groups(const ngp_hash_layout* layout, int level_begin, int level_end, int64_t l2_bytes,
+                              int32_t* bounds) {
+    // greedy: a group grows while its fp32 gradient slice stays within the budget; a level larger than the budget
+    // is a group of its own; l2_bytes <= 0 (unknown) gives one group
+    if (int rc = check_layout(layout)) return rc;
+    NGP_REQUIRE(level_begin >= 0 && level_begin < level_end && level_end <= layout->n_levels, "bad level range");
+    NGP_REQUIRE(bounds != nullptr, "null pointer");
+    const int64_t budget = l2_bytes * kL2BudgetNum / kL2BudgetDen;
+    int n_groups = 0;
+    int64_t used = 0;
+    bounds[0] = level_begin;
+    for (int l = level_begin; l < level_end; ++l) {
+        const int64_t bytes = (int64_t)layout->map_sizes[l] * layout->feat_dim * (int64_t)sizeof(float);
+        if (l > bounds[n_groups] && l2_bytes > 0 && used + bytes > budget) {
+            bounds[++n_groups] = l;
+            used = 0;
+        }
+        used += bytes;
+    }
+    bounds[++n_groups] = level_end;
+    return n_groups;
 }
 
 int ngp_hash_encode_bwd_input(const float* xyz, const void* table, const void* dout, int dtype,
