@@ -27,6 +27,7 @@ import torch
 
 from taichi_nerfs_b200.layout import make_hash_layout
 
+from composite_ref import _check_composite_bwd, np_composite_f64
 from hash_ref import (PAD, _aabb6, _check_scatter, _level_ranges, _level_slice, _normalise, _ray_points,
                       _world_points, n_dev_cases, np_hash_bwd_f64, rows_of)
 
@@ -653,54 +654,6 @@ def _long_rays(rng, half):
     n = counts.size
     rays_a = np.stack([rng.permutation(n), np.cumsum(counts) - counts, counts], 1).astype(np.int32)
     return rays_a, sig, rgbs, deltas, ts
-
-
-def np_composite_f64(sig, rgbs, deltas, ts, rays_a, thr, go, gd, gr, gw):
-    """fp64 restatement of the compositing (volume_train.py:22-48) and its transpose, per ray: w_s = a_s T_s while
-    T_s > thr.  Returns forward sums, dsigma, drgb and, for the tolerances, the sum of |terms| of every dsigma and the
-    conditioning factor N + 4 / min a of every ray (a = 1 - exp(-sigma delta) carries an absolute fp32 error)."""
-    S, n = sig.size, rays_a.shape[0]
-    out = dict(op=np.zeros(n), rgb=np.zeros((n, 3)), dep=np.zeros(n), dsig=np.zeros(S), drgb=np.zeros((S, 3)),
-               mag=np.zeros(S), w=np.zeros(S), k=np.zeros(S), kray=np.ones(n), active=np.zeros(S, bool))
-    c_all = rgbs.astype(np.float64)
-    for r, s0, cnt in rays_a:
-        if cnt == 0:
-            continue
-        sl = slice(s0, s0 + cnt)
-        x = sig[sl].astype(np.float64) * deltas[sl].astype(np.float64)
-        a = -np.expm1(-x)
-        Tn = np.exp(-np.cumsum(x))                   # T after each sample
-        Tb = np.concatenate([[1.0], Tn[:-1]])        # T before
-        act = Tb > thr
-        assert np.all(np.abs(np.log(Tb / thr)) > 1e-2), "a sample too close to the threshold for an fp64 reference"
-        w = np.where(act, a * Tb, 0.0)
-        c, t = c_all[sl], ts[sl].astype(np.float64)
-        G = c @ gr[r].astype(np.float64) + gd[r] * t + go[r] + gw[sl]
-        Gabs = np.abs(c) @ np.abs(gr[r]).astype(np.float64) + abs(gd[r]) * np.abs(t) + abs(go[r]) + np.abs(gw[sl])
-        later = np.concatenate([np.cumsum((w * G)[::-1])[::-1][1:], [0.0]])
-        later_abs = np.concatenate([np.cumsum((w * Gabs)[::-1])[::-1][1:], [0.0]])
-        d = deltas[sl].astype(np.float64)
-        out["dsig"][sl] = np.where(act, d * (Tn * G - later), 0.0)
-        # T_{s+1} = T_s (1 - a_s) is off by ~u T_s, not u T_{s+1}, where a_s rounds to 1 in fp32
-        out["mag"][sl] = d * (Tb * Gabs + later_abs)
-        out["drgb"][sl] = w[:, None] * gr[r].astype(np.float64)[None, :]
-        out["w"][sl], out["active"][sl] = w, act
-        out["op"][r], out["rgb"][r], out["dep"][r] = w.sum(), w @ c, w @ t
-        out["kray"][r] = cnt + 4.0 / a[act].min()
-        out["k"][sl] = out["kray"][r]
-    return out
-
-
-def _check_composite_bwd(dsig, drgbs, ref, half, what):
-    act = ref["active"]
-    assert not dsig[~act].any() and not drgbs[~act].any(), f"{what}: gradient of a sample after termination"
-    err = np.abs(dsig.astype(np.float64) - ref["dsig"])
-    tol = 8 * ref["k"] * U * ref["mag"]
-    bad = np.flatnonzero(err > tol)
-    assert bad.size == 0, f"{what}: dsigma of {bad.size} samples, first {bad[0]}: err {err[bad[0]]:.3e} tol {tol[bad[0]]:.3e}"
-    d = drgbs.astype(np.float64)
-    tol = 8 * ref["k"][:, None] * U * np.abs(ref["drgb"]) + (2.0 ** -11 * np.abs(ref["drgb"]) + 2.0 ** -24 if half else 0)
-    assert (np.abs(d - ref["drgb"]) <= tol).all(), f"{what}: drgb"
 
 
 @pytest.mark.gpu
