@@ -199,10 +199,11 @@ int ngp_hash_encode_fwd_dyn(const float* xyz, const void* table, const ngp_hash_
 int ngp_hash_encode_bwd_dyn(const float* xyz, const void* dout, int dout_dtype, const ngp_hash_layout* layout,
                             float* grad_table, int64_t n_max, const int32_t* n_dev, const float* aabb6,
                             void* stream);
-/* Same, restricted to the levels [level_begin, level_end): the levels own disjoint slices of grad_table, so a
- * multi-GPU step scatters them in groups and all-reduces a finished group's slice while the next group runs
- * (SURVEY.md §8e).  found_inf_or_null: set to 1 when a non-finite contribution is scattered - GradScaler's inf check
- * raised at the source instead of a separate pass over the gradient buffer (ngp_check_finite). */
+/* Same, restricted to the levels [level_begin, level_end): the levels own disjoint slices of grad_table, so a range
+ * can be scattered on its own; inside the range the launch scatters one L2-sized level group at a time
+ * (ngp_hash_bwd_level_groups below).  found_inf_or_null: set to 1 when a non-finite contribution is scattered -
+ * GradScaler's inf check raised at the source instead of a separate pass over the gradient buffer
+ * (ngp_check_finite). */
 int ngp_hash_encode_bwd_levels(const float* xyz, const void* dout, int dout_dtype, const ngp_hash_layout* layout,
                                float* grad_table, int64_t n_max, const int32_t* n_dev, const float* aabb6,
                                int level_begin, int level_end, int32_t* found_inf_or_null, void* stream);

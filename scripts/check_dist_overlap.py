@@ -1,6 +1,7 @@
-"""torchrun check (N >= 2 GPUs): every multi-GPU variant of the graph step (peer-memory optimizer = the default, NCCL
-sharded optimizer, fp16 transport, per-slice all-reduces behind the backward kernels) applies the same updates as the
-step with one monolithic fp32 all-reduce; parameters and occupancy grids stay identical on all ranks.
+"""torchrun check (N >= 2 GPUs): both multi-GPU exchanges of the graph step (the peer-memory optimizer step, the
+default on one NVLink box, and the fp16 NCCL all-reduce it falls back to), each with and without the optimizer overlap,
+apply the update of a single-rank trainer on the concatenated batch of all ranks; parameters and occupancy grids stay
+identical on all ranks.
 
     python -m torch.distributed.run --nproc-per-node 2 --master-addr 127.0.0.1 --master-port 29517 scripts/check_dist_overlap.py
 """
@@ -18,62 +19,73 @@ from oracle.train_step import make_rays  # noqa: E402   (ray generator only)
 from taichi_nerfs_b200.fast_step import StaticTrainStep  # noqa: E402
 from taichi_nerfs_b200.trainer import NGPTrainer  # noqa: E402
 
+if int(os.environ.get("WORLD_SIZE", "1")) < 2:
+    sys.exit("check_dist_overlap.py checks the multi-GPU step: run it under torchrun with --nproc-per-node >= 2")
 rank, world, local = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"]), int(os.environ["LOCAL_RANK"])
 torch.cuda.set_device(local)
 dist.init_process_group("nccl", device_id=torch.device("cuda", local))
+# a one-rank group per rank for the reference trainer (new_group is collective: every rank creates every group)
+solo = [dist.new_group([r]) for r in range(world)][rank]
 bits = np.load(os.path.join(ROOT, "tests", "golden", "lego_bitfield.npz"))["bitfield"]
 thr = 0.01 * 1024 / 3 ** 0.5
+N = 4096   # rays per rank
 
 
-def run(sharded, overlap_ar, overlap_opt, f16=False, p2p=False):
-    os.environ["NGP_GRAD_F16"] = "1" if f16 else "0"
+def batch(r, k):
+    """Rank r's rays, targets and marching noise of step k."""
+    o, d = make_rays(N, seed=100 * r + k)
+    g = torch.Generator(device="cuda").manual_seed(100 * r + k)
+    return (torch.from_numpy(o).cuda(), torch.from_numpy(d).cuda(), torch.rand(N, 3, device="cuda", generator=g),
+            torch.rand(N, device="cuda", generator=g))
+
+
+def run(overlap_opt, p2p=None, reference=False):
     torch.manual_seed(3)
     m = NGP(scale=0.5, max_res=1024, half_opt=True).cuda()
     with torch.no_grad():
         m.pos_encoder.hash_table.mul_(2e3)
         m.density_bitfield.copy_(torch.from_numpy(bits))
-    tr = NGPTrainer(m, lr=1e-2, sharded_optimizer=sharded, p2p_optimizer=p2p)
-    fs = StaticTrainStep(tr, 4096, samples_per_ray_capacity=64, overlap_allreduce=overlap_ar, overlap_optimizer=overlap_opt)
-    if p2p:
-        assert tr.p2p is not None and tr.sharded, "peer-memory optimizer unavailable (CUDA IPC / peer access failed)"
+    tr = NGPTrainer(m, lr=1e-2, process_group=solo if reference else None, p2p_optimizer=p2p)
+    n = N * world if reference else N
+    fs = StaticTrainStep(tr, n, samples_per_ray_capacity=64, overlap_optimizer=overlap_opt)
+    if reference:
+        assert tr.world_size == 1 and tr.p2p is None and tr.grad16 is None
+    elif p2p is False:
+        assert tr.p2p is None and tr.grad16 is not None
     else:
-        assert tr.sharded == (sharded and not overlap_ar) and tr.grad_f16 == (f16 and not sharded)
+        assert tr.p2p is not None, "peer-memory optimizer unavailable (CUDA IPC / peer access failed)"
     losses = []
     for k in range(4):
-        o, d = make_rays(4096, seed=100 * rank + k)          # every rank renders its own shard
-        g = torch.Generator(device="cuda").manual_seed(100 * rank + k)
-        losses.append(float(fs.step(torch.from_numpy(o).cuda(), torch.from_numpy(d).cuda(),
-                                    torch.rand(4096, 3, device="cuda", generator=g),
-                                    torch.rand(4096, device="cuda", generator=g))))
+        if reference:   # every rank's batch, in rank order
+            o, d, gt, noise = (torch.cat(parts) for parts in zip(*(batch(r, k) for r in range(world))))
+        else:           # every rank renders its own shard
+            o, d, gt, noise = batch(rank, k)
+        losses.append(float(fs.step(o, d, gt, noise)))
         if k == 1:
             fs.flush()
             m.update_density_grid(thr, warmup=False)
     fs.flush()
     torch.cuda.synchronize()
-    return m, tr, losses
+    tr.p2p_check()
+    return m, losses
 
 
-m1, t1, l1 = run(False, False, False)     # replicated Adam, one monolithic all-reduce (round 1)
-m2, t2, l2 = run(True, False, False)      # sharded optimizer: reduce-scatter, shard Adam, all-gather of the fp16 shadow
-m3, t3, l3 = run(True, False, True)       # + optimizer of step k beside the marching of step k+1
-m4, t4, l4 = run(False, True, False)      # opt-in: slice all-reduces behind the level groups of the hash backward
-m5, t5, l5 = run(False, False, True, f16=True)   # default at N > 1: fp16 gradient transport + optimizer overlap
-m6, t6, l6 = run(False, False, False, p2p=True)   # peer-memory optimizer step (csrc/p2p.cu), no NCCL in the step
-m7, t7, l7 = run(False, False, True, p2p=True)    # default at N > 1: + optimizer of step k beside the marching of k+1
-t6.p2p_check(), t7.p2p_check()
-for name, (ma, mb) in {"sharded vs replicated": (m1, m2), "sharded + optimizer overlap": (m1, m3),
-                       "slice all-reduce vs monolithic": (m1, m4), "fp16 transport vs fp32": (m1, m5),
-                       "peer-memory optimizer vs replicated": (m1, m6),
-                       "peer-memory optimizer + overlap": (m1, m7)}.items():
+m0, l0 = run(False, reference=True)   # one rank, the concatenated batch: no gradient exchange at all
+runs = {"peer-memory optimizer": run(False),
+        "peer-memory optimizer + overlap": run(True),            # the default at N > 1
+        "fp16 NCCL fallback": run(False, p2p=False),
+        "fp16 NCCL fallback + overlap": run(True, p2p=False)}
+for name, (m, _) in runs.items():
     # Adam's first updates are +-lr whatever the gradient's magnitude, so an entry whose gradient sum is ~0 moves in the
-    # opposite direction when the sum is rounded differently (atomic order; fp16 rounding of the transport variant, which
-    # flips more of them): a small fraction of entries may differ by a few lr, the rest agree to 2e-3
-    limit = 1e-2 if name.startswith("fp16 transport") else 2e-3
-    for pa, pb in zip(ma.parameters(), mb.parameters()):
+    # opposite direction when the sum is rounded differently (atomic order, summation order over the ranks; fp16
+    # rounding of the fallback's transport, which flips more of them): a small fraction of entries may differ by a few
+    # lr, the rest agree to 2e-3
+    limit = 1e-2 if name.startswith("fp16") else 2e-3
+    for pa, pb in zip(m0.parameters(), m.parameters()):
         bad = float(((pa - pb).abs() > 2e-3).float().mean())
         assert bad < limit, (name, bad)
 # replicas agree bit for bit: parameters and occupancy grids
-for m in (m1, m2, m3, m4, m5, m6, m7):
+for m, _ in runs.values():
     flat = torch.cat([p.detach().reshape(-1) for p in m.parameters()])
     ref = flat.clone()
     dist.broadcast(ref, 0)
@@ -83,5 +95,6 @@ for m in (m1, m2, m3, m4, m5, m6, m7):
     dist.broadcast(gr, 0)
     assert torch.equal(g, gr), "occupancy bitfields differ across ranks"
 if rank == 0:
-    print(f"dist check ok on {world} GPUs: losses {l1} / {l2} / {l3} / {l4} / {l5} / p2p {l6} / {l7}")
+    print(f"dist check ok on {world} GPUs: losses single-rank {l0} / "
+          + " / ".join(f"{name} {ls}" for name, (_, ls) in runs.items()))
 dist.destroy_process_group()

@@ -5,7 +5,7 @@ the C-ABI kernels, enqueued in a fixed order on fixed buffers:
 
   [ray-batch sampler] -> ray_aabb -> single-pass march (capacity buffers, one atomic row reservation per ray) ->
   hash fwd (+AABB normalisation) -> fused MLP fwd -> fused per-ray head (composite fwd + background + MSE +
-  composite bwd) -> MLP bwd -> hash bwd -> [all-reduce] -> check_finite -> device-side LR/bias-correction update
+  composite bwd) -> MLP bwd -> hash bwd -> [gradient exchange] -> check_finite -> device-side LR/bias-correction update
   -> fused Adam (+fp16 shadow, grad zero) -> device-side GradScaler update
 
 What makes it graph-capturable: the number of samples S stays on the device (kernels read it from the
@@ -31,7 +31,7 @@ def _p(t):
 class StaticTrainStep:
     def __init__(self, trainer, n_rays: int, samples_per_ray_capacity: int = 384, exp_step_factor: float = 0.0,
                  T_threshold: float = 1e-4, max_samples: int = 1024, use_graph: bool = True,
-                 dynamic_loss_scale: bool = True, overlap_optimizer: bool = False, overlap_allreduce=None):
+                 dynamic_loss_scale: bool = True, overlap_optimizer: bool = False):
         self.tr = trainer
         m = self.model = trainer.model
         enc = m.pos_encoder
@@ -93,21 +93,10 @@ class StaticTrainStep:
         self.overlap = bool(overlap_optimizer)
         self.pending = False             # gradients of the last step not applied yet (overlap mode only)
         self._side = torch.cuda.Stream(device=dev, priority=-1)
-        self._ar_stream = torch.cuda.Stream(device=dev)
-        # several ranks, opt-in: all-reduce gradient slices behind the backward kernels that complete them (F = 2 layout)
-        import os
-        # (opt-in, NGP_AR_OVERLAP=1: on 2 GPUs the three grouped scatter launches + concurrent NCCL kernels cost more
-        # than the all-reduce they hide)
-        default_ar = ((trainer.world_size > 1 or os.environ.get("NGP_AR_FORCE") == "1") and enc._clayout.feat_dim == 2
-                      and os.environ.get("NGP_AR_OVERLAP", "0") == "1")
-        self.overlap_allreduce = bool(overlap_allreduce if overlap_allreduce is not None else default_ar)
-        if self.overlap_allreduce and getattr(trainer, "p2p", None) is not None:
-            self.overlap_allreduce = False   # the peer-memory optimizer step needs no all-reduce at all
-        if self.overlap_allreduce and trainer.sharded:
-            trainer.sharded = False     # the slice all-reduces replace the reduce-scatter; Adam stays replicated
-        # one rank + dynamic loss scale: the backward kernels raise GradScaler's inf flag themselves (a non-finite
-        # contribution is seen where it is scattered), the optimizer consumes and clears it - no 45 MB check pass
-        self.inf_at_source = bool((trainer.world_size == 1 or trainer.sharded) and self.dynamic_loss_scale
+        # one rank or the peer-memory step + dynamic loss scale: the backward kernels raise GradScaler's inf flag
+        # themselves (a non-finite contribution is seen where it is scattered), the optimizer consumes and clears it -
+        # no 45 MB check pass (the NCCL fallback checks the reduced fp16 sum instead)
+        self.inf_at_source = bool((trainer.world_size == 1 or trainer.p2p is not None) and self.dynamic_loss_scale
                                   and enc._clayout.feat_dim == 2)
         if self.inf_at_source:
             trainer.found_inf.zero_()
@@ -198,55 +187,13 @@ class StaticTrainStep:
                                            int(level_begin), int(level_end),
                                            _p(self.tr.found_inf) if self.inf_at_source else None, st))
 
-    def _level_groups(self):
-        """Level groups of the multi-GPU backward, most expensive first: the hashed fine levels (all-distinct cells,
-        most atomics), the hashed coarse levels, the dense levels.  Each group owns a contiguous slice of the flat
-        gradient buffer (levels are laid out in order)."""
-        lay = self._clayout
-        L_, first_hashed = lay.n_levels, lay.begin_fast_hash_level
-        mid = first_hashed + (L_ - first_hashed) // 2
-        groups = [(mid, L_), (first_hashed, mid), (0, first_hashed)]
-        return [(a, b) for a, b in groups if b > a]
-
-    def _slice_of_levels(self, a, b):
-        lay, F = self._clayout, self._clayout.feat_dim
-        lo = lay.offsets[a] * F
-        hi = (lay.offsets[b] if b < lay.n_levels else self.P // F) * F
-        return lo, hi
-
-    def _enqueue_backward_overlapped(self):
-        """Multi-GPU backward: gradient slices are all-reduced on a side stream as soon as they are complete — the MLP
-        gradients while the hash scatter runs, each level group while the next group runs — so only the last (small,
-        dense-level) slice's all-reduce is exposed (SURVEY.md §8e)."""
-        import torch.distributed as dist
-        tr, main, ar = self.tr, torch.cuda.current_stream(), self._ar_stream
-        fg = tr.flat_grad
-        reduce = tr.world_size > 1     # (a single rank can still run the grouped launches: tests)
-
-        def allreduce_behind(lo, hi):
-            ar.wait_stream(main)
-            with torch.cuda.stream(ar):
-                dist.all_reduce(fg[lo:hi], group=tr.pg)
-        self._k_mlp_bwd()
-        if reduce:
-            allreduce_behind(self.P, fg.numel())                        # MLP weight gradients (37.6 KB)
-        for a, b in self._level_groups():
-            self._k_hash_bwd(a, b)
-            if reduce:
-                allreduce_behind(*self._slice_of_levels(a, b))
-        if reduce:
-            main.wait_stream(ar)
-
     def _enqueue_network(self):
         # counter[0] = number of valid sample rows, read on the device by every kernel
         self._k_hash_fwd()
         self._k_mlp_fwd()
         self._k_head()
-        if self.overlap_allreduce:
-            self._enqueue_backward_overlapped()
-        else:
-            self._k_mlp_bwd()
-            self._k_hash_bwd()
+        self._k_mlp_bwd()
+        self._k_hash_bwd()
 
     def _enqueue_sampler(self):
         """datasets/base.py:34-61 + ray_utils.py:51-80 + the marching jitter, keyed by (seed, batch counter, ray)."""
@@ -257,9 +204,8 @@ class StaticTrainStep:
                                           _p(self.gt), _p(self.noise), None, None, self.n, self._st()))
 
     def _enqueue_update(self):
-        # [all-reduce, unless the backward already reduced slice by slice] -> check_finite -> LR/bias scalars ->
-        # fused Adam -> GradScaler.update
-        self.tr.enqueue_update(allreduce=not self.overlap_allreduce, check_finite=not self.inf_at_source)
+        # [gradient exchange] -> check_finite -> LR/bias scalars -> fused Adam -> GradScaler.update
+        self.tr.enqueue_update(check_finite=not self.inf_at_source)
 
     def _enqueue(self, sampled=False, mode="sync"):
         if sampled:
@@ -341,7 +287,7 @@ class StaticTrainStep:
         else:
             self._enqueue(sampled, mode)
         self.pending = self.overlap
-        if getattr(self.tr, 'sharded', False):
+        if self.tr.p2p is not None:
             self.tr.master_stale = True     # (the Python side of the update does not run on a graph replay)
 
     def flush(self):
@@ -354,7 +300,7 @@ class StaticTrainStep:
             self.pending = False
             if self.tr._shadow is not None:
                 self.model.pos_encoder.adopt_shadow(self.tr._shadow)
-        self.tr.sync_master()   # sharded optimizer: the fp32 master table is complete again on every rank
+        self.tr.sync_master()   # peer-memory step: the fp32 master table is complete again on every rank
 
     def _finish_step(self):
         self.tr.step_count += 1

@@ -48,8 +48,8 @@ def inv_grad_scale(loss_scale: float, world: int) -> float:
 
 
 def optimizer_shard(n_table: int, rank: int, world: int):
-    """[begin, end) of the flat table parameter owned by ``rank`` in the sharded optimizer (NGPTrainer): equal shards,
-    each a multiple of 4 floats so that every shard stays 16-byte aligned for the float4 Adam sweep."""
+    """[begin, end) of the flat table parameter owned by ``rank`` in the peer-memory optimizer step (NGPTrainer): equal
+    shards, each a multiple of 4 floats so that every shard stays 16-byte aligned for the float4 Adam sweep."""
     if n_table % (4 * world) != 0:
         raise ValueError(f"table size {n_table} is not a multiple of 4 * world ({world})")
     shard = n_table // world

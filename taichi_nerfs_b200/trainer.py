@@ -8,9 +8,9 @@ the fp16 table re-cast by ONE fused pass over the flat parameter buffer (csrc/op
 bias-correction scalars and the iteration counter live in device memory (``scale_state``, ``hyper``, ``step_dev``),
 so nothing synchronises the host; the graph-captured step (fast_step.py) enqueues exactly the same kernels.
 
-Multi-GPU: rays are sharded across ranks (each rank renders its own batch); the only collective is
-one all-reduce (sum) of the flat gradient buffer per step, folded into the fused Adam as inv_scale /
-world_size (SURVEY.md §8e).
+Multi-GPU: rays are sharded across ranks (each rank renders its own batch) and the gradient sum is folded into the
+fused Adam as inv_scale / world_size (SURVEY.md §8e).  On one NVLink box the optimizer step is ONE peer-memory kernel
+(csrc/p2p.cu); otherwise the flat gradient is all-reduced once per step in fp16 over NCCL.
 """
 from __future__ import annotations
 
@@ -31,7 +31,7 @@ def _p(t):
 class NGPTrainer:
     def __init__(self, model, lr: float = 1e-2, max_steps: int = 20000, loss_scale: float | None = None,
                  betas=(0.9, 0.999), eps: float = 1e-15, process_group=None, dynamic_loss_scale: bool = True,
-                 sharded_optimizer: bool | None = None, p2p_optimizer: bool | None = None):
+                 p2p_optimizer: bool | None = None):
         self.model = model
         self.lr0 = lr
         self.max_steps = max_steps
@@ -51,15 +51,16 @@ class NGPTrainer:
         sizes = [p.numel() for p in self.params]
         pad = [(-s) % 4 for s in sizes]  # keep every slice 16-byte aligned for the float4 Adam kernel
         total = sum(s + q for s, q in zip(sizes, pad))
-        # Several ranks on one NVLink box (default; NGP_P2P_ADAM=0 or p2p_optimizer=False keeps NCCL): the gradient
-        # and the fp16 shadow live in a CUDA-IPC buffer that the peers map, and the optimizer step is ONE kernel that
-        # sums the owned 1/N of the gradient with peer loads, runs Adam on it and stores the new fp16 table slice into
-        # every rank's shadow with peer stores (csrc/p2p.cu).  None when unavailable (the NCCL paths below remain).
-        import os
+        # Several ranks on one NVLink box (p2p_optimizer: None = whenever available, False = the NCCL fallback): the
+        # gradient and the fp16 shadow live in a CUDA-IPC buffer that the peers map, and the optimizer step is ONE
+        # kernel that sums the owned 1/N of the gradient with peer loads, runs Adam on it and stores the new fp16 table
+        # slice into every rank's shadow with peer stores (csrc/p2p.cu).  None when unavailable (NCCL fallback below).
         self.p2p = None
         P_, enc_ = sizes[0], model.pos_encoder
-        want_p2p = p2p_optimizer if p2p_optimizer is not None else os.environ.get("NGP_P2P_ADAM", "1") != "0"
-        if (want_p2p and self.world_size > 1 and dev.type == "cuda" and hasattr(enc_, "adopt_shadow")
+        if p2p_optimizer and hasattr(enc_, 'plane_embedding'):
+            raise ValueError("NGPTrainer: the peer-memory optimizer shards the fp16 hash table; a tri-plane model uses "
+                             "the all-reduce of the flat gradient (p2p_optimizer off)")
+        if (p2p_optimizer is not False and self.world_size > 1 and dev.type == "cuda" and hasattr(enc_, "adopt_shadow")
                 and self.params[0] is enc_.hash_table and P_ % (4 * self.world_size) == 0):
             from .p2p import PeerRegion
             self.p2p = PeerRegion.create(total, dev, process_group)
@@ -103,35 +104,19 @@ class NGPTrainer:
             self._shadow = self._shadow_full[:enc.hash_table.numel()]
             enc.adopt_shadow(self._shadow)
 
-        # Several ranks, fp16 encoder: shard the optimizer over the hash table (the MLP weights stay replicated).
-        # Per step: reduce-scatter of the table gradient (each rank receives the sum for the entries it owns), Adam on
-        # the owned 1/N of the table, all-gather of the updated fp16 shadow (what the kernels read) — 0.75x the bytes
-        # of an all-reduce and 1/N of the Adam sweep.  The fp32 master of non-owned entries goes stale until
-        # sync_master() (called before state_dict / checkpoints).
-        import os
-        P = self.slices[0][1]
-        # (opt-in, NGP_SHARDED_ADAM=1: on 2 GPUs its four collectives cost more than the bytes they save)
-        want = (sharded_optimizer if sharded_optimizer is not None
-                else os.environ.get("NGP_SHARDED_ADAM", "0") == "1")
-        if (want or p2p_optimizer) and hasattr(model.pos_encoder, 'plane_embedding'):
-            raise ValueError("NGPTrainer: the sharded and peer-memory optimizers shard the fp16 hash table; a tri-plane "
-                             "model uses the all-reduce of the flat gradient (sharded_optimizer / p2p_optimizer off)")
-        self.sharded = bool((want or self.p2p is not None) and self.world_size > 1 and self._shadow_full is not None
-                            and P % (4 * self.world_size) == 0 and self.slices[0][0] == 0)
-        if self.sharded:
+        # Peer-memory step: the optimizer is sharded over the hash table (the MLP weights stay replicated); each rank
+        # owns 1/N of the table.  The fp32 master of non-owned entries goes stale until sync_master() (called before
+        # state_dict / checkpoints).
+        if self.p2p is not None:
             self.rank = torch.distributed.get_rank(process_group)
-            self.shard_lo, hi = parallel.optimizer_shard(P, self.rank, self.world_size)
+            self.shard_lo, hi = parallel.optimizer_shard(P_, self.rank, self.world_size)
             self.shard = hi - self.shard_lo
-            if self.p2p is None:   # staging buffers of the NCCL reduce-scatter / all-gather
-                self.grad_shard = torch.zeros(self.shard, device=dev, dtype=torch.float32)
-                self.shadow_shard = torch.zeros(self.shard, device=dev, dtype=torch.float16)
             self.master_stale = False
-        assert self.p2p is None or self.sharded
-        # Several ranks: the gradient travels in fp16 (half the all-reduce bytes).  That is the precision the
-        # reference's own gradients have under autocast (fp16 autograd); the loss scale keeps them in range and an
-        # overflow becomes inf = a skipped step + scale backoff, as with GradScaler.
-        self.grad_f16 = bool(self.world_size > 1 and not self.sharded and os.environ.get("NGP_GRAD_F16", "1") != "0")
-        self.grad16 = torch.zeros(total, device=dev, dtype=torch.float16) if self.grad_f16 else None
+        # Several ranks without peer memory: the gradient travels in fp16 (half the all-reduce bytes).  That is the
+        # precision the reference's own gradients have under autocast (fp16 autograd); the loss scale keeps them in
+        # range and an overflow becomes inf = a skipped step + scale backoff, as with GradScaler.
+        self.grad16 = (torch.zeros(total, device=dev, dtype=torch.float16)
+                       if self.world_size > 1 and self.p2p is None else None)
 
     # cosine annealing to lr/30 (train.py:159-163, CosineAnnealingLR(T_max=max_steps, eta_min=lr/30))
     def lr_at(self, step: int) -> float:
@@ -170,103 +155,55 @@ class NGPTrainer:
         (loss * scale).backward()
         return loss, results
 
-    def enqueue_update(self, allreduce: bool = True, check_finite: bool = True):
-        """[all-reduce] -> inf check -> LR / bias-correction scalars -> fused Adam (+fp16 shadow, grad zero) ->
-        GradScaler.update(), all on the current stream with device-side scalars (graph-capturable)."""
-        if self.sharded and allreduce:
-            return self._enqueue_update_sharded(check_finite)
-        if self.grad_f16 and allreduce:
-            return self._enqueue_update_f16()
-        L, st = load(), C.c_void_p(torch.cuda.current_stream().cuda_stream)
-        fg = self.flat_grad
-        if allreduce:
-            parallel.allreduce_gradients(fg, self.pg)
-        if check_finite:   # (False: the backward kernels already raised the flag at the source, fast_step.py)
-            check(L.ngp_check_finite(_p(fg), fg.numel(), _p(self.found_inf), st))   # after the sum: identical on every rank
-        # inv_scale: static (host constant) or the device value maintained by ngp_loss_scale_update (-1 sentinel)
-        inv = -1.0 if self.dynamic_loss_scale else parallel.inv_grad_scale(self.loss_scale, self.world_size)
-        check(L.ngp_adam_hyper_update(_p(self.step_dev), self.lr0, self.lr0 / 30, self.max_steps, self.betas[0],
-                                      self.betas[1], inv, _p(self.found_inf), _p(self.hyper), st))
-        # one launch over [hash table | MLP weights]
-        check(L.ngp_adam_step_dyn(_p(self.flat_param), _p(fg), _p(self.exp_avg), _p(self.exp_avg_sq),
-                                  _p(self._shadow_full), _p(self.found_inf), _p(self.hyper), self.betas[0],
-                                  self.betas[1], self.eps, 1, fg.numel(), st))
-        if self.dynamic_loss_scale:  # GradScaler.update(): adjusts the scale used by the NEXT step
-            check(L.ngp_loss_scale_update(_p(self.scale_state), _p(self.found_inf), 2.0, 0.5, 2000,
-                                          float(self.world_size), _p(self.hyper), 0 if check_finite else 1, st))
+    def enqueue_update(self, check_finite: bool = True):
+        """Gradient exchange -> inf check -> LR / bias-correction scalars -> fused Adam (+fp16 shadow, grad zero) ->
+        GradScaler.update(), all on the current stream with device-side scalars (graph-capturable).
 
-    def _enqueue_update_f16(self):
-        """Several ranks: pack the gradient to fp16 -> ONE all-reduce of half the bytes -> finite check on the reduced
-        buffer (identical on every rank; catches local inf/NaN and overflow alike) -> Adam reads the fp16 sum and zeroes
-        the fp32 accumulation buffer."""
+        The exchange: none on one rank.  Peer memory (csrc/p2p.cu): [local finite check] -> barrier (all backward
+        passes done; found_inf becomes the OR over the ranks) -> ONE kernel: peer-load sum of the owned gradient slice +
+        Adam on it + peer-store of the new fp16 table slice into every rank's shadow (the MLP weights: every rank, same
+        sums) -> barrier (everybody has read my gradient and written my shadow) -> clear the local gradient.  NCCL
+        fallback: pack the gradient to fp16 -> ONE all-reduce of half the bytes -> finite check on the reduced buffer
+        (always: identical on every rank, catches local inf/NaN and overflow alike) -> Adam reads the fp16 sum and
+        zeroes the fp32 accumulation buffer.
+
+        check_finite=False: the backward kernels already raised the inf flag at the source (fast_step.py)."""
         L, st = load(), C.c_void_p(torch.cuda.current_stream().cuda_stream)
-        fg, g16 = self.flat_grad, self.grad16
-        check(L.ngp_grad_pack_f16(_p(fg), _p(g16), fg.numel(), st))
-        parallel.allreduce_gradients(g16, self.pg)
-        check(L.ngp_check_finite_f16(_p(g16), g16.numel(), _p(self.found_inf), st))
+        R, fg, g16, P = self.p2p, self.flat_grad, self.grad16, self.slices[0][1]
+        if g16 is not None:
+            check(L.ngp_grad_pack_f16(_p(fg), _p(g16), fg.numel(), st))
+            parallel.allreduce_gradients(g16, self.pg)
+            check(L.ngp_check_finite_f16(_p(g16), g16.numel(), _p(self.found_inf), st))
+        elif check_finite:
+            check(L.ngp_check_finite(_p(fg), fg.numel(), _p(self.found_inf), st))
+        if R is not None:
+            R.barrier(self.found_inf)
+        # inv_scale: static (host constant) or the device value maintained by GradScaler.update() below (-1 sentinel)
         inv = -1.0 if self.dynamic_loss_scale else parallel.inv_grad_scale(self.loss_scale, self.world_size)
         check(L.ngp_adam_hyper_update(_p(self.step_dev), self.lr0, self.lr0 / 30, self.max_steps, self.betas[0],
                                       self.betas[1], inv, _p(self.found_inf), _p(self.hyper), st))
-        check(L.ngp_adam_step_dyn_g16(_p(self.flat_param), _p(g16), _p(fg), _p(self.exp_avg), _p(self.exp_avg_sq),
+        # one Adam launch over [hash table | MLP weights]
+        if R is not None:
+            check(L.ngp_adam_step_p2p(_p(self.flat_param), R.grad_tab, _p(self.exp_avg), _p(self.exp_avg_sq),
+                                      R.shadow_tab, R.rank, R.world, _p(self.found_inf), _p(self.hyper), self.betas[0],
+                                      self.betas[1], self.eps, self.shard_lo, self.shard_lo + self.shard, P,
+                                      fg.numel(), st))
+            R.barrier(None)
+            fg.zero_()
+            self.master_stale = True
+        elif g16 is not None:
+            check(L.ngp_adam_step_dyn_g16(_p(self.flat_param), _p(g16), _p(fg), _p(self.exp_avg), _p(self.exp_avg_sq),
+                                          _p(self._shadow_full), _p(self.found_inf), _p(self.hyper), self.betas[0],
+                                          self.betas[1], self.eps, fg.numel(), st))
+        else:
+            check(L.ngp_adam_step_dyn(_p(self.flat_param), _p(fg), _p(self.exp_avg), _p(self.exp_avg_sq),
                                       _p(self._shadow_full), _p(self.found_inf), _p(self.hyper), self.betas[0],
-                                      self.betas[1], self.eps, fg.numel(), st))
-        if self.dynamic_loss_scale:
+                                      self.betas[1], self.eps, 1, fg.numel(), st))
+        if self.dynamic_loss_scale:  # GradScaler.update(): adjusts the scale used by the NEXT step
+            # a flag raised at the source is not reset by the next step, so this launch clears it
+            raised_at_source = not check_finite and g16 is None
             check(L.ngp_loss_scale_update(_p(self.scale_state), _p(self.found_inf), 2.0, 0.5, 2000,
-                                          float(self.world_size), _p(self.hyper), 0, st))
-
-    def _enqueue_update_sharded(self, check_finite: bool):
-        """Sharded update (see __init__): inf flag (local check, max over ranks) -> reduce-scatter of the table gradient
-        + all-reduce of the MLP gradients -> Adam on the owned table shard and on the replicated MLP weights ->
-        all-gather of the fp16 shadow table -> GradScaler.update()."""
-        if self.p2p is not None:
-            return self._enqueue_update_p2p(check_finite)
-        import torch.distributed as dist
-        L, st = load(), C.c_void_p(torch.cuda.current_stream().cuda_stream)
-        fg, P, lo, hi = self.flat_grad, self.slices[0][1], self.shard_lo, self.shard_lo + self.shard
-        if check_finite:   # on the local gradient: a non-finite term on any rank makes the sum non-finite
-            check(L.ngp_check_finite(_p(fg), fg.numel(), _p(self.found_inf), st))
-        dist.all_reduce(self.found_inf, op=dist.ReduceOp.MAX, group=self.pg)
-        dist.reduce_scatter_tensor(self.grad_shard, fg[:P], op=dist.ReduceOp.SUM, group=self.pg)
-        dist.all_reduce(fg[P:], op=dist.ReduceOp.SUM, group=self.pg)
-        inv = -1.0 if self.dynamic_loss_scale else parallel.inv_grad_scale(self.loss_scale, self.world_size)
-        check(L.ngp_adam_hyper_update(_p(self.step_dev), self.lr0, self.lr0 / 30, self.max_steps, self.betas[0],
-                                      self.betas[1], inv, _p(self.found_inf), _p(self.hyper), st))
-        check(L.ngp_adam_step_dyn(_p(self.flat_param[lo:hi]), _p(self.grad_shard), _p(self.exp_avg[lo:hi]),
-                                  _p(self.exp_avg_sq[lo:hi]), _p(self.shadow_shard), _p(self.found_inf), _p(self.hyper),
-                                  self.betas[0], self.betas[1], self.eps, 0, self.shard, st))
-        check(L.ngp_adam_step_dyn(_p(self.flat_param[P:]), _p(fg[P:]), _p(self.exp_avg[P:]), _p(self.exp_avg_sq[P:]),
-                                  _p(self._shadow_full[P:]), _p(self.found_inf), _p(self.hyper), self.betas[0],
-                                  self.betas[1], self.eps, 1, fg.numel() - P, st))
-        fg[:P].zero_()     # the local table gradient (the Adam sweep only saw the reduced shard)
-        dist.all_gather_into_tensor(self._shadow_full[:P], self.shadow_shard, group=self.pg)
-        if self.dynamic_loss_scale:
-            check(L.ngp_loss_scale_update(_p(self.scale_state), _p(self.found_inf), 2.0, 0.5, 2000,
-                                          float(self.world_size), _p(self.hyper), 0 if check_finite else 1, st))
-        self.master_stale = True
-
-    def _enqueue_update_p2p(self, check_finite: bool):
-        """The sharded update without NCCL (csrc/p2p.cu): [local finite check] -> barrier (all backward passes done;
-        found_inf becomes the OR over the ranks) -> LR / bias-correction scalars -> ONE kernel: peer-load sum of the
-        owned gradient slice + Adam on it + peer-store of the new fp16 table slice into every rank's shadow (the MLP
-        weights: every rank, same sums) -> barrier (everybody has read my gradient and written my shadow) -> clear the
-        local gradient -> GradScaler.update()."""
-        L, st = load(), C.c_void_p(torch.cuda.current_stream().cuda_stream)
-        R, fg, P = self.p2p, self.flat_grad, self.slices[0][1]
-        if check_finite:
-            check(L.ngp_check_finite(_p(fg), fg.numel(), _p(self.found_inf), st))
-        R.barrier(self.found_inf)
-        inv = -1.0 if self.dynamic_loss_scale else parallel.inv_grad_scale(self.loss_scale, self.world_size)
-        check(L.ngp_adam_hyper_update(_p(self.step_dev), self.lr0, self.lr0 / 30, self.max_steps, self.betas[0],
-                                      self.betas[1], inv, _p(self.found_inf), _p(self.hyper), st))
-        check(L.ngp_adam_step_p2p(_p(self.flat_param), R.grad_tab, _p(self.exp_avg), _p(self.exp_avg_sq), R.shadow_tab,
-                                  R.rank, R.world, _p(self.found_inf), _p(self.hyper), self.betas[0], self.betas[1],
-                                  self.eps, self.shard_lo, self.shard_lo + self.shard, P, fg.numel(), st))
-        R.barrier(None)
-        fg.zero_()
-        if self.dynamic_loss_scale:
-            check(L.ngp_loss_scale_update(_p(self.scale_state), _p(self.found_inf), 2.0, 0.5, 2000,
-                                          float(self.world_size), _p(self.hyper), 0 if check_finite else 1, st))
-        self.master_stale = True
+                                          float(self.world_size), _p(self.hyper), int(raised_at_source), st))
 
     def p2p_check(self):
         """Host check (synchronises): raises if a peer barrier of this rank timed out (a rank fell out of step)."""
@@ -274,9 +211,9 @@ class NGPTrainer:
             raise RuntimeError("NGPTrainer: a peer barrier timed out — the ranks did not run the same steps")
 
     def sync_master(self):
-        """Sharded optimizer: make the fp32 master table complete on every rank again (before state_dict(), checkpoints
+        """Peer-memory step: make the fp32 master table complete on every rank again (before state_dict(), checkpoints
         or anything else that reads ``hash_table`` itself rather than the fp16 shadow)."""
-        if getattr(self, 'sharded', False) and self.master_stale:
+        if self.p2p is not None and self.master_stale:
             import torch.distributed as dist
             P, lo = self.slices[0][1], self.shard_lo
             own = self.flat_param[lo:lo + self.shard].clone()

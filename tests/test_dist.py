@@ -104,58 +104,6 @@ def test_two_rank_update_equals_single_process(tmp_path):
     assert np.mean(np.isclose(w0, wref, rtol=0, atol=2e-4)) > 0.999
 
 
-def _worker_sharded(rank, world, port, out_dir):
-    """The sharded optimizer's data flow (NGPTrainer._enqueue_update_sharded) with gloo collectives and the oracle's
-    Adam: local inf flag -> max over ranks; table gradient summed, every rank applies Adam to the entries it owns;
-    the updated fp16 shadow shards are all-gathered; MLP gradients all-reduced, MLP Adam replicated."""
-    os.environ["MASTER_ADDR"] = "127.0.0.1"
-    os.environ["MASTER_PORT"] = str(port)
-    os.environ["OMP_NUM_THREADS"] = "2"
-    dist.init_process_group("gloo", rank=rank, world_size=world)
-    from oracle import oracle as O
-    from taichi_nerfs_b200 import parallel
-    TS, model = _model16()
-    o, d, gt, nz = _batch()
-    b, e = parallel.shard_bounds(N_GLOBAL, rank, world)
-    rgb, cache = TS.forward(model, o[b:e], d[b:e], nz[b:e])
-    loss, g_table, g_mlp = TS.backward(model, cache, rgb, gt[b:e], LOSS_SCALE)
-    P = g_table.size
-    lo, hi = parallel.optimizer_shard(P, rank, world)
-    found = torch.tensor([int(O.check_finite(g_table) or O.check_finite(g_mlp))], dtype=torch.int32)
-    parallel.allreduce_found_inf(found)
-    # reduce-scatter == all-reduce followed by keeping the owned slice (gloo has no reduce_scatter_tensor)
-    gt_sum = torch.from_numpy(g_table.copy())
-    dist.all_reduce(gt_sum)
-    shard_grad = gt_sum.numpy()[lo:hi].copy()
-    gm = torch.from_numpy(g_mlp.copy())
-    dist.all_reduce(gm)
-    inv = parallel.inv_grad_scale(LOSS_SCALE, world)
-    assert int(found) == 0
-    model.step += 1
-    shadow_shard = np.zeros(hi - lo, np.float16)
-    O.adam_step(model.table[lo:hi], shard_grad, model.m[lo:hi], model.v[lo:hi], 1e-2, model.step, inv_scale=inv,
-                param_f16=shadow_shard)
-    off, goff = P, 0
-    for w in model.ws:
-        flat = w.reshape(-1)
-        g = np.ascontiguousarray(gm.numpy()[goff:goff + flat.size])
-        O.adam_step(flat, g, model.m[off:off + flat.size], model.v[off:off + flat.size], 1e-2, model.step, inv_scale=inv)
-        off += flat.size
-        goff += flat.size
-    # all-gather of the fp16 shadow (what the kernels read) and, for the comparison, of the fp32 master (sync_master)
-    parts = [torch.zeros(hi - lo, dtype=torch.float16) for _ in range(world)]
-    dist.all_gather(parts, torch.from_numpy(shadow_shard))
-    shadow = torch.cat(parts).numpy()
-    mparts = [torch.zeros(hi - lo) for _ in range(world)]
-    dist.all_gather(mparts, torch.from_numpy(model.table[lo:hi].copy()))
-    master = torch.cat(mparts).numpy()
-    np.save(os.path.join(out_dir, f"shadow_{rank}.npy"), shadow)
-    np.save(os.path.join(out_dir, f"master_{rank}.npy"), master)
-    np.save(os.path.join(out_dir, f"w_{rank}.npy"), np.concatenate([w.reshape(-1) for w in model.ws]))
-    dist.barrier()
-    dist.destroy_process_group()
-
-
 def _worker_p2p(rank, world, port, out_dir):
     """The peer-memory optimizer step (csrc/p2p.cu, NGPTrainer._enqueue_update_p2p) with two processes on the CPU: the
     'peer buffers' are files both ranks map (np.memmap) — gradient, fp16 shadow, flag block.  No collective touches the
@@ -262,24 +210,3 @@ def test_optimizer_shard_bounds():
         assert all((b - a) % 4 == 0 and a % 4 == 0 for a, b in cuts)
     with pytest.raises(ValueError):
         optimizer_shard(10, 0, 4)
-
-
-def test_two_rank_sharded_optimizer_equals_replicated(tmp_path):
-    """Sharded update (each rank owns half of the table) == the replicated update of
-    test_two_rank_update_equals_single_process, bit for bit; the gathered fp16 shadow is the cast of the master."""
-    world = 2
-    port = _free_port()
-    rep = tmp_path / "rep"
-    sh = tmp_path / "sh"
-    rep.mkdir()
-    sh.mkdir()
-    mp.spawn(_worker, args=(world, port, str(rep)), nprocs=world, join=True)
-    mp.spawn(_worker_sharded, args=(world, _free_port(), str(sh)), nprocs=world, join=True)
-    t_rep = np.load(rep / "table_0.npy")
-    m0, m1 = np.load(sh / "master_0.npy"), np.load(sh / "master_1.npy")
-    assert np.array_equal(m0, m1) and np.array_equal(m0, t_rep)
-    s0, s1 = np.load(sh / "shadow_0.npy"), np.load(sh / "shadow_1.npy")
-    assert np.array_equal(s0, s1) and np.array_equal(s0, t_rep.astype(np.float16))
-    assert np.array_equal(np.load(sh / "w_0.npy"), np.load(rep / "w_0.npy"))
-    assert np.array_equal(np.load(sh / "w_0.npy"), np.load(sh / "w_1.npy"))
-

@@ -456,43 +456,3 @@ def test_update_density_grid_is_sync_free_and_matches_reference_statistics():
         c.update_density_grid(thr, warmup=False)
     c.update_density_grid(thr, warmup=True)
     assert torch.equal(a.density_bitfield, c.density_bitfield) and torch.equal(a.density_grid, c.density_grid)
-
-
-def test_grouped_hash_backward_equals_single_launch(lego_bitfield):
-    """The multi-GPU step scatters the hash gradient in level groups (fine hashed, coarse hashed, dense) so that a
-    finished group's slice can be all-reduced behind the next group's kernel: the groups together must produce the
-    single launch's gradient (each level's atomics are unchanged, levels own disjoint slices)."""
-    from modules.networks import NGP
-    from oracle.train_step import make_rays
-    from taichi_nerfs_b200.fast_step import StaticTrainStep
-    from taichi_nerfs_b200.trainer import NGPTrainer
-
-    def run(grouped):
-        torch.manual_seed(3)
-        m = NGP(scale=0.5, max_res=1024, half_opt=True).cuda()
-        with torch.no_grad():
-            m.pos_encoder.hash_table.mul_(2e3)
-            m.density_bitfield.copy_(torch.from_numpy(lego_bitfield))
-        tr = NGPTrainer(m, lr=1e-2)
-        fs = StaticTrainStep(tr, 2048, samples_per_ray_capacity=64, use_graph=False, overlap_allreduce=grouped)
-        assert fs.overlap_allreduce == grouped
-        o, d = make_rays(2048, seed=21)
-        g = torch.Generator(device='cuda').manual_seed(0)
-        fs.rays_o.copy_(torch.from_numpy(o))
-        fs.rays_d.copy_(torch.from_numpy(d))
-        fs.gt.copy_(torch.rand(2048, 3, device='cuda', generator=g))
-        fs.noise.copy_(torch.rand(2048, device='cuda', generator=g))
-        from taichi_nerfs_b200._lib import check, load as L
-        check(L().ngp_step_reset(fs.counter.data_ptr(), fs.loss_sum.data_ptr(), tr.found_inf.data_ptr(), None, None))
-        fs._enqueue_march()
-        fs._enqueue_network()
-        torch.cuda.synchronize()
-        return tr.flat_grad.clone(), fs
-    g1, fs = run(False)
-    g2, _ = run(True)
-    groups = fs._level_groups()
-    assert groups[0][1] == 16 and groups[-1][0] == 0 and sum(b - a for a, b in groups) == 16
-    los = sorted(fs._slice_of_levels(a, b) for a, b in groups)
-    assert los[0][0] == 0 and los[-1][1] == fs.P and all(x[1] == y[0] for x, y in zip(los, los[1:]))
-    scale = float(g1.abs().max())
-    assert scale > 0 and float((g1 - g2).abs().max()) <= 1e-5 * scale
