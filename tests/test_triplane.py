@@ -8,6 +8,7 @@ import numpy as np
 import pytest
 
 from taichi_nerfs_b200.layout import make_hash_layout, make_triplane_layout
+from triplane_ref import triplane_numpy
 
 
 @pytest.fixture(scope="module")
@@ -15,48 +16,6 @@ def O():
     from oracle import triplane
     triplane.build()
     return triplane
-
-
-def triplane_numpy(xyz, table, lay, acc=np.float32, clamp=False):
-    """Vectorised restatement of triplane_encoder_kernel (triplane.py:35-98) for xyz in [0,1]: the geometry in fp32
-    exactly as the kernel computes it, the feature arithmetic in ``acc`` (fp32: bit-exact; fp64: for finite
-    differences).  clamp: the max_res-grid coordinate clipped to [0, max_res-1] (positions slightly outside [0, 1]).
-    Returns [n, L*F] with column j*L + level."""
-    f32 = np.float32
-    x = np.asarray(xyz, f32)
-    n, L, F, mr = x.shape[0], lay.levels, lay.feat_dim, lay.max_res
-    tab = np.asarray(table).astype(acc, copy=False)
-    out = np.zeros((n, L * F), acc)
-    for level in range(L):
-        res = lay.resolutions[level]
-        pos = x * f32(res - 1) + f32(0.5)                      # :56
-        g = np.floor(pos).astype(np.uint32)                     # :57
-        frac = pos - g.astype(f32)                              # :58
-        lf = np.zeros((3, n, F), acc)
-        for fd, (d0, d1) in enumerate(((0, 1), (1, 2), (2, 0))):   # xyz6 = [x,y, y,z, z,x], [d::2] (:46-50)
-            for idx in range(4):
-                w = np.ones(n, f32)
-                gl = []
-                for d, ax in enumerate((d0, d1)):
-                    if idx & (1 << d):
-                        gl.append(g[:, ax] + 1)
-                        w = w * frac[:, ax]
-                    else:
-                        gl.append(g[:, ax])
-                        w = w * (f32(1) - frac[:, ax])
-                ori = [(gi.astype(f32) / f32(res) * f32(mr - 1)).astype(np.uint32) for gi in gl]   # :73-76
-                if clamp:
-                    ori = [np.minimum(o, mr - 1) for o in ori]
-                index = ori[0].astype(np.int64) + ori[1].astype(np.int64) * mr                       # :78-82
-                base = fd * mr * mr * F + index * F                                                  # :84-87
-                for j in range(F):
-                    lf[fd, :, j] = lf[fd, :, j] + w.astype(acc) * tab[base + j]                      # :90-92
-        for j in range(F):
-            cp = np.ones(n, acc)
-            for fd in range(3):
-                cp = cp * lf[fd, :, j]                                                               # :94-96
-            out[:, j * L + level] = cp
-    return out
 
 
 def _positions(rng, n, lay):
