@@ -336,27 +336,15 @@ int ngp_frame_round_begin(int32_t* state, void* stream);
 /* One round of marching (modules/ray_march.py:197-268 semantics: resume at t_cur[ray], strict 0 < t, no jitter):
  * persistent warps walk alive[0 .. state[2]); every live ray emits at most min(limit, capacity / state[2]) samples
  * (so the rows always fit), reserves them with one atomicAdd on state[0], writes rays_a[slot] = (ray, start, n) and
- * leaves its resume point in t_cur[ray] (+inf once it has left the box).  No cap over the frame. */
+ * leaves its resume point in t_cur[ray] (+inf once it has left the box).  The cap over the frame: a live ray emits at
+ * most max_samples - n_marched[ray] samples, adds what it emitted to n_marched[ray] (zeroed by ngp_frame_begin; must
+ * not be NULL) and gets t_cur[ray] = +inf once it has max_samples, so that no ray gets more samples over the frame
+ * than the one-shot march gives it. */
 int ngp_raymarching_round(const float* rays_o, const float* rays_d, const float* hits_t,
                           const uint8_t* density_bitfield, int cascades, int grid_size, float scale,
-                          float exp_step_factor, int limit, const int32_t* alive, int32_t* state, float* t_cur,
-                          int32_t* rays_a, float* xyzs, float* dirs, float* deltas, float* ts, int64_t n_rays,
-                          int64_t capacity, const uint32_t* coarse_or_null, void* stream);
-/* As ngp_raymarching_round, with a per-ray cap over the frame: a live ray emits at most max_samples - n_marched[ray]
- * samples, adds what it emitted to n_marched[ray] (zeroed by ngp_frame_begin) and gets t_cur[ray] = +inf once it has
- * max_samples, so that no ray gets more samples over the frame than the one-shot march gives it.  n_marched == NULL
- * is ngp_raymarching_round. */
-int ngp_raymarching_round_capped(const float* rays_o, const float* rays_d, const float* hits_t,
-                                 const uint8_t* density_bitfield, int cascades, int grid_size, float scale,
-                                 float exp_step_factor, int limit, int max_samples, const int32_t* alive,
-                                 int32_t* state, float* t_cur, int32_t* n_marched, int32_t* rays_a, float* xyzs,
-                                 float* dirs, float* deltas, float* ts, int64_t n_rays, int64_t capacity,
-                                 const uint32_t* coarse_or_null, void* stream);
-/* Optional accelerator of the round march for one-cascade, constant-step scenes: coarse[(G/8)^3 / 32 words], bit s =
- * the 8^3-cell super-cell with Morton index s holds an occupied cell.  With it the march leaps over up to 256
- * candidate positions at a time where the ray crosses empty space; the emitted samples are unchanged (bit-exact: the
- * leap is taken only where the reference loop would visit every position and emit nothing). */
-int ngp_build_coarse_occupancy(const uint8_t* density_bitfield, int grid_size, uint32_t* coarse, void* stream);
+                          float exp_step_factor, int limit, int max_samples, const int32_t* alive, int32_t* state,
+                          float* t_cur, int32_t* n_marched, int32_t* rays_a, float* xyzs, float* dirs, float* deltas,
+                          float* ts, int64_t n_rays, int64_t capacity, void* stream);
 /* composite_test (modules/volume_render_test.py:4-54) for the round's samples, accumulating into opacity/depth/rgb
  * [n_rays], + block-level compaction of the rays that stay alive (T > T_threshold and still inside the box) into
  * next_alive[0 .. state[3]).  `limit` = the round's sample budget per ray (picks how many lanes share a ray). */

@@ -10,9 +10,6 @@ from .volume_render_test import composite_test
 
 MAX_SAMPLES = 1024
 NEAR_DISTANCE = 0.01
-_FORCE_LOOP = False  # set True to use the reference-shaped incremental loop for test-time rendering
-import os as _os
-_NO_COMPACTION = _os.environ.get('NGP_FRAME_COMPACT', '1') == '0'  # (or set True) to render frames by evaluating every marched sample (render_frame) instead of rounds
 
 
 def render(model, rays_o, rays_d, test_time=False, exp_step_factor=0, T_threshold=1e-4,
@@ -24,10 +21,10 @@ def render(model, rays_o, rays_d, test_time=False, exp_step_factor=0, T_threshol
     rays_d = rays_d.contiguous()
     hits_t = ray_aabb_intersection(rays_o, rays_d, model.scale)
     if test_time:
-        if getattr(model, '_fusable', None) is not None and rays_o.is_cuda and not _FORCE_LOOP:
+        if getattr(model, '_fusable', None) is not None and rays_o.is_cuda:
             # same result as the incremental loop below, without its per-iteration host syncs
             from taichi_nerfs_b200.render_frame import render_frame, render_frame_compact
-            if model._fusable(rays_o) and not _NO_COMPACTION:
+            if model._fusable(rays_o):
                 # stock model: one CUDA graph per frame, live rays compacted between rounds (early termination)
                 return render_frame_compact(model, rays_o, rays_d, exp_step_factor, T_threshold, max_samples)
             return render_frame(model, rays_o, rays_d, exp_step_factor, T_threshold, max_samples)

@@ -10,8 +10,9 @@ import torch
 import bench
 from datasets.ray_utils import get_ray_directions, get_rays
 from datasets.synthetic import SyntheticLego, hemisphere_poses
+from modules.intersection import ray_aabb_intersection
 from modules.networks import NGP
-from modules.rendering import render
+from modules.rendering import _render_rays_test, render
 
 dev = torch.device("cuda", 0)
 lay, table, ws = bench.init_weights_numpy(bench.SEED)
@@ -30,8 +31,9 @@ def frame():
     with torch.autocast("cuda", dtype=torch.float16):
         directions = get_ray_directions(800, 800, K, device=dev)
         rays_o, rays_d = get_rays(directions, pose)
-        import modules.rendering as R
-        R._FORCE_LOOP = impl == "loop"
+        if impl == "loop":   # the reference-shaped incremental loop
+            rays_o, rays_d = rays_o.contiguous(), rays_d.contiguous()
+            return _render_rays_test(model, rays_o, rays_d, ray_aabb_intersection(rays_o, rays_d, model.scale))
         return render(model, rays_o, rays_d, test_time=True)
 
 

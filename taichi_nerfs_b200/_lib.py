@@ -91,10 +91,8 @@ def _declare(lib):
         "ngp_adam_step_p2p": (ci, [vp, vp, vp, vp, vp, ci, ci, vp, vp, f32, f32, f32, i64, i64, i64, i64, vp]),
         "ngp_frame_begin": (ci, [vp, vp, vp, vp, vp, vp, vp, vp, i64, vp]),
         "ngp_frame_round_begin": (ci, [vp, vp]),
-        "ngp_raymarching_round": (ci, [vp, vp, vp, vp, ci, ci, f32, f32, ci, vp, vp, vp, vp, vp, vp, vp, vp, i64, i64, vp, vp]),
-        "ngp_raymarching_round_capped": (ci, [vp, vp, vp, vp, ci, ci, f32, f32, ci, ci, vp, vp, vp, vp, vp, vp, vp, vp, vp,
-                                              i64, i64, vp, vp]),
-        "ngp_build_coarse_occupancy": (ci, [vp, ci, vp, vp]),
+        "ngp_raymarching_round": (ci, [vp, vp, vp, vp, ci, ci, f32, f32, ci, ci, vp, vp, vp, vp, vp, vp, vp, vp, vp,
+                                       i64, i64, vp]),
         "ngp_composite_round": (ci, [vp, vp, ci, vp, vp, vp, vp, vp, vp, f32, vp, vp, vp, vp, i64, ci, vp]),
         "ngp_grid_workspace_bytes": (i64, [ci, ci]),
         "ngp_grid_sample_cells": (ci, [vp, ci, ci, f32, f32, ci, i64, C.c_uint64, C.c_uint32, vp, vp, vp, vp]),

@@ -59,7 +59,6 @@ struct MarchParams {
     float scale;
     float esf;
     float dt_max;    // SQRT3_2*scale/grid_size
-    const uint32_t* __restrict__ coarse;  // optional: dilated 8^3-cell occupancy (ngp_build_coarse_occupancy), 1 cascade
 };
 
 __device__ __forceinline__ void load_ray(const float* __restrict__ rays_o, const float* __restrict__ rays_d,
@@ -222,8 +221,7 @@ struct RoundArgs {
     const int32_t* __restrict__ alive;      // live ray ids of this round
     const int32_t* __restrict__ n_alive;    // their number (device)
     float* __restrict__ t_cur;              // per ray: where the march resumes (in/out); +inf = left the box
-    int32_t* __restrict__ n_marched;        // per ray: samples emitted in earlier rounds of the frame (in/out), or
-                                            // null: no cap over the frame
+    int32_t* __restrict__ n_marched;        // per ray: samples emitted in earlier rounds of the frame (in/out)
     int max_samples;                        // per-ray cap over the whole frame (the one-shot march's max_samples)
     int limit;                              // samples per ray this round (reduced so that all live rays fit `capacity`)
 };
@@ -263,10 +261,8 @@ __device__ __forceinline__ void march_one_ray(const float* __restrict__ rays_o, 
     if (kMode == 3) {
         t = round.t_cur[r];
         if (!(0.0f < t)) t = -1.0f;
-        if (round.n_marched != nullptr) {
-            marched_before = round.n_marched[r];
-            limit = max(0, min(limit, round.max_samples - marched_before));   // the frame's per-ray cap
-        }
+        marched_before = round.n_marched[r];
+        limit = max(0, min(limit, round.max_samples - marched_before));   // the frame's per-ray cap
     } else if (kMode == 2 && noise == nullptr) {  // test time: no jitter, strict 0 < t (ray_march.py:226)
         t = hits_t[r * 2 + 0];
         if (!(0.0f < t)) t = -1.0f;
@@ -278,69 +274,7 @@ __device__ __forceinline__ void march_one_ray(const float* __restrict__ rays_o, 
     const bool const_dt = p.esf == 0.0f;
     const float dt0 = calc_dt(t, p.esf, p.dt_max);
 
-    // Empty-space leap (constant step, one cascade, coarse occupancy available): up to 256 candidate positions at once.
-    // Lane j looks at positions 8j and 8j+7; if every 8^3-cell super-cell in the box spanned by their two super-cells
-    // is empty, positions 8j .. 8j+7 (collinear) lie in empty cells.  If the first position is "regular" (an axis
-    // with d < -1e-3 and an unclamped coordinate, which only decreases along the ray) the reference loop visits every
-    // position, emits nothing in empty cells and advances by exactly one step each (tests/test_oracle.py, exit quirk),
-    // so with f leading lanes vouching t jumps to position 8f by the closed form of the fp32 recurrence.
-    bool leap_ok = false;
-    float mb0 = 0.0f, mb0_inv = 0.0f;
-    if (kMode >= 2 && p.coarse != nullptr && const_dt && p.cascades == 1) {
-        mb0 = fminf(__uint_as_float((uint32_t)(127 - 1) << 23), p.scale);
-        mb0_inv = f_div(1.0f, mb0);
-        const float dmax = fmaxf(fmaxf(fabsf(ray.d[0]), fabsf(ray.d[1])), fabsf(ray.d[2]));
-        leap_ok = dt0 * dmax * p.gsf * 0.5f * mb0_inv <= 1.0f;   // at most one cell per step and axis
-    }
-    bool try_leap = leap_ok;
-
     while (0.0f <= t && t < t2 && emitted < limit) {  // ray_march.py:43 / :86 (warp-uniform)
-        if (try_leap && skip_until == -INFINITY) {
-            const uint32_t b = __float_as_uint(t), e = b >> 23, m = (b & 0x7fffffu) | 0x800000u;
-            const uint32_t b1 = __float_as_uint(f_add(t, dt0));
-            const uint32_t cs = ((b1 & 0x7fffffu) | 0x800000u) - m;
-            int f = 0;
-            if ((b1 >> 23) == e) {
-                // lane j vouches for positions 8j .. 8j+7 (and the landing position 8j+8): same binade as t (closed
-                // form valid), all inside the box and within 7 steps of position 8j, whose dilated super-cell is empty
-                const bool in_binade = m + (uint32_t)(8 * lane + 8) * cs <= 0xffffffu;
-                const float tq = __uint_as_float((e << 23) | ((m + (uint32_t)(8 * lane) * cs) & 0x7fffffu));
-                const float tl = __uint_as_float((e << 23) | ((m + (uint32_t)(8 * lane + 7) * cs) & 0x7fffffu));
-                // cells of the first (p) and last (q) position of this lane's range; the six positions in between lie
-                // on the segment p-q, so their cells are inside the box spanned by the two cells, i.e. inside the (at
-                // most 2x2x2) super-cells spanned by the two super-cells
-                bool reg = false;
-                uint32_t sa[3], sb[3];
-#pragma unroll
-                for (int k = 0; k < 3; ++k) {
-                    const float xp = f_add(ray.o[k], f_mul(tq, ray.d[k]));
-                    const float xq = f_add(ray.o[k], f_mul(tl, ray.d[k]));
-                    const float rp = f_mul(f_mul(0.5f, f_add(f_mul(xp, mb0_inv), 1.0f)), p.gsf);
-                    const float rq = f_mul(f_mul(0.5f, f_add(f_mul(xq, mb0_inv), 1.0f)), p.gsf);
-                    reg = reg || (ray.d[k] < -1e-3f && rp < f_sub(p.gsf, 1.0f));
-                    const uint32_t up = __float2uint_rz(fminf(fmaxf(rp, 0.0f), f_sub(p.gsf, 1.0f))) >> 3;
-                    const uint32_t uq = __float2uint_rz(fminf(fmaxf(rq, 0.0f), f_sub(p.gsf, 1.0f))) >> 3;
-                    sa[k] = min(up, uq);
-                    sb[k] = max(up, uq);
-                }
-                bool empty = true;
-                for (uint32_t z = sa[2]; z <= sb[2]; ++z)
-                    for (uint32_t y = sa[1]; y <= sb[1]; ++y)
-                        for (uint32_t x = sa[0]; x <= sb[0]; ++x) {
-                            const uint32_t sc = morton3d(x, y, z);   // Morton index of the 8^3 super-cell
-                            empty = empty && ((__ldg(p.coarse + (sc >> 5)) >> (sc & 31u)) & 1u) == 0u;
-                        }
-                const bool ok = in_binade && tl < t2 && empty;
-                const unsigned okm = __ballot_sync(full, ok);
-                const bool reg0 = __shfl_sync(full, reg, 0);
-                f = reg0 ? (okm == full ? 32 : __ffs(~okm) - 1) : 0;    // leading lanes that vouch
-            }
-            if (f >= 4) {   // >= 32 positions: cheaper than testing them one by one
-                t = __uint_as_float((e << 23) | ((m + (uint32_t)(8 * f) * cs) & 0x7fffffu));
-                continue;
-            }
-            try_leap = false;   // close to geometry: test positions one by one until a whole chunk comes out empty
-        }
         // t chain: position k of this chunk, identical on every lane
         float tk = t, my_t = t, my_dt = dt0;
         if (const_dt) {
@@ -375,7 +309,6 @@ __device__ __forceinline__ void march_one_ray(const float* __restrict__ rays_o, 
         const CellTest c = test_cell(p, ray, my_t, my_dt);
         const unsigned valid_mask = __ballot_sync(full, valid);
         const unsigned occ_mask = __ballot_sync(full, valid && c.occ);
-        if (leap_ok) try_leap = occ_mask == 0u;   // a chunk without any occupied position: back in empty space
 
         // Independent-positions fast path: if every in-box lane is occupied or "regular" (and no jump is pending from
         // the previous chunk) each visited position's successor is simply the next one, so the visited set is the
@@ -471,8 +404,8 @@ __device__ __forceinline__ void march_one_ray(const float* __restrict__ rays_o, 
             rays_a[slot * 3 + 1] = s0;
             rays_a[slot * 3 + 2] = emitted;
             // a ray that has reached max_samples is done, like the one-shot march: +inf takes it off the live list
-            const bool capped = round.n_marched != nullptr && marched_before + emitted >= round.max_samples;
-            if (round.n_marched != nullptr) round.n_marched[r] = marched_before + emitted;
+            const bool capped = marched_before + emitted >= round.max_samples;
+            round.n_marched[r] = marched_before + emitted;
             round.t_cur[r] = capped ? INFINITY : t_resume;
         }
         __syncwarp();
@@ -524,8 +457,10 @@ __device__ __forceinline__ void march_one_ray(const float* __restrict__ rays_o, 
     }
 }
 
+// The single-pass march (kMode 2: the graph-captured training step, render_frame) is held to 12 CTAs per SM, i.e. at
+// most 40 registers; left to itself ptxas gives it 47 and 10 CTAs.  0 leaves the other modes unconstrained.
 template <int kMode>
-__global__ void __launch_bounds__(kRaysPerBlock * 32)
+__global__ void __launch_bounds__(kRaysPerBlock * 32, kMode == 2 ? 12 : 0)
 march_train_warp_kernel(const float* __restrict__ rays_o, const float* __restrict__ rays_d,
                         const float* __restrict__ hits_t, const float* __restrict__ noise, MarchParams p,
                         int max_samples, int32_t* __restrict__ rays_a, int32_t* __restrict__ counter,
@@ -629,30 +564,6 @@ __global__ void __launch_bounds__(128) march_test_kernel(const float* __restrict
     samples_counter[n] = s;
 }
 
-// coarse occupancy of cascade 0: bit s (Morton index of an 8^3-cell super-cell) is set when the super-cell holds an
-// occupied cell.  The bitfield is Morton ordered, so a super-cell is 512 consecutive bits = 64 bytes.  One CTA,
-// (G/8)^3 <= 4096 super-cells.
-__global__ void __launch_bounds__(1024) coarse_occupancy_kernel(const uint8_t* __restrict__ bits, int G,
-                                                                uint32_t* __restrict__ coarse) {
-    const int S = G >> 3, n_sc = S * S * S;
-    for (int base = 0; base < n_sc; base += blockDim.x) {
-        const int sc = base + threadIdx.x;
-        bool occ = false;
-        if (sc < n_sc) {
-            const uint4* p = reinterpret_cast<const uint4*>(bits + (size_t)sc * 64);
-            uint32_t any = 0;
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-                const uint4 v = __ldg(p + k);
-                any |= v.x | v.y | v.z | v.w;
-            }
-            occ = any != 0;
-        }
-        const unsigned word = __ballot_sync(0xffffffffu, occ);
-        if ((threadIdx.x & 31) == 0 && sc < n_sc) coarse[sc >> 5] = word;
-    }
-}
-
 MarchParams make_params(const uint8_t* bits, int cascades, int grid_size, float scale, float esf) {
     MarchParams p;
     p.bits = bits;
@@ -666,7 +577,6 @@ MarchParams make_params(const uint8_t* bits, int cascades, int grid_size, float 
     // SQRT3_2 * scale / grid_size in fp32, mul then div (utils.py:56-57); host IEEE fp32
     volatile float m = kSqrt3x2 * scale;
     p.dt_max = m / p.gsf;
-    p.coarse = nullptr;
     return p;
 }
 
@@ -744,30 +654,18 @@ int ngp_raymarching_frame(const float* rays_o, const float* rays_d, const float*
 }
 
 
-int ngp_build_coarse_occupancy(const uint8_t* density_bitfield, int grid_size, uint32_t* coarse, void* stream) {
-    NGP_REQUIRE(density_bitfield && coarse, "null pointer");
-    NGP_REQUIRE(grid_size >= 32 && grid_size <= 128 && (grid_size & (grid_size - 1)) == 0,
-                "grid_size must be 32, 64 or 128");
-    NGP_REQUIRE((reinterpret_cast<uintptr_t>(density_bitfield) & 15) == 0, "bitfield must be 16-byte aligned");
-    coarse_occupancy_kernel<<<1, 1024, 0, ngp::as_stream(stream)>>>(density_bitfield, grid_size, coarse);
-    NGP_LAUNCHED("coarse_occupancy_kernel");
-    return 0;
-}
-
-int ngp_raymarching_round_capped(const float* rays_o, const float* rays_d, const float* hits_t,
-                                 const uint8_t* density_bitfield, int cascades, int grid_size, float scale,
-                                 float exp_step_factor, int limit, int max_samples, const int32_t* alive,
-                                 int32_t* state, float* t_cur, int32_t* n_marched, int32_t* rays_a, float* xyzs,
-                                 float* dirs, float* deltas, float* ts, int64_t n_rays, int64_t capacity,
-                                 const uint32_t* coarse_or_null, void* stream) {
+int ngp_raymarching_round(const float* rays_o, const float* rays_d, const float* hits_t,
+                          const uint8_t* density_bitfield, int cascades, int grid_size, float scale,
+                          float exp_step_factor, int limit, int max_samples, const int32_t* alive, int32_t* state,
+                          float* t_cur, int32_t* n_marched, int32_t* rays_a, float* xyzs, float* dirs, float* deltas,
+                          float* ts, int64_t n_rays, int64_t capacity, void* stream) {
     NGP_REQUIRE(n_rays >= 0 && capacity >= 1, "bad size");
     if (n_rays == 0) return 0;
-    NGP_REQUIRE(rays_o && rays_d && hits_t && density_bitfield && alive && state && t_cur && rays_a && xyzs && dirs &&
-                    deltas && ts, "null pointer");
+    NGP_REQUIRE(rays_o && rays_d && hits_t && density_bitfield && alive && state && t_cur && n_marched && rays_a &&
+                    xyzs && dirs && deltas && ts, "null pointer");
     NGP_REQUIRE(limit >= 1 && limit <= kMaxFrameSamples, "limit must be in [1, 1024]");
-    NGP_REQUIRE(n_marched == nullptr || max_samples >= 1, "max_samples must be >= 1");
-    MarchParams p = make_params(density_bitfield, cascades, grid_size, scale, exp_step_factor);
-    if (cascades == 1 && grid_size <= 128 && grid_size >= 32) p.coarse = coarse_or_null;
+    NGP_REQUIRE(max_samples >= 1, "max_samples must be >= 1");
+    const MarchParams p = make_params(density_bitfield, cascades, grid_size, scale, exp_step_factor);
     RoundArgs ra;
     ra.alive = alive;
     ra.n_alive = state + 2;
@@ -783,16 +681,6 @@ int ngp_raymarching_round_capped(const float* rays_o, const float* rays_d, const
         rays_o, rays_d, hits_t, nullptr, p, limit, rays_a, state, xyzs, dirs, deltas, ts, n_rays, capacity, ra);
     NGP_LAUNCHED("march_train_warp_kernel<round>");
     return 0;
-}
-
-int ngp_raymarching_round(const float* rays_o, const float* rays_d, const float* hits_t,
-                          const uint8_t* density_bitfield, int cascades, int grid_size, float scale,
-                          float exp_step_factor, int limit, const int32_t* alive, int32_t* state, float* t_cur,
-                          int32_t* rays_a, float* xyzs, float* dirs, float* deltas, float* ts, int64_t n_rays,
-                          int64_t capacity, const uint32_t* coarse_or_null, void* stream) {
-    return ngp_raymarching_round_capped(rays_o, rays_d, hits_t, density_bitfield, cascades, grid_size, scale,
-                                        exp_step_factor, limit, 0, alive, state, t_cur, nullptr, rays_a, xyzs, dirs,
-                                        deltas, ts, n_rays, capacity, coarse_or_null, stream);
 }
 
 int ngp_raymarching_test(const float* rays_o, const float* rays_d, float* hits_t, const int64_t* alive_indices,

@@ -113,9 +113,9 @@ class FrameRenderer:
     """
     SCHEDULE = (4, 8, 16, 32, 64, 128, 256, 512, 4)     # samples per live ray and round; sums to max_samples = 1024
     MAX_SAMPLES = 1024     # per ray over the whole frame, extra rounds included (the one-shot march's max_samples)
+    coarse = None          # no empty-space occupancy: bench.py reads this attribute of a cached renderer
 
-    def __init__(self, model, n_rays, exp_step_factor=0.0, T_threshold=1e-4, rows_per_ray=6, use_graph=True,
-                 use_leap=True):
+    def __init__(self, model, n_rays, exp_step_factor=0.0, T_threshold=1e-4, rows_per_ray=6, use_graph=True):
         import ctypes as C
         from ._lib import F16, F32, MlpWeights, check, load
         self._C, self._check, self._load = C, check, load
@@ -138,13 +138,6 @@ class FrameRenderer:
         self.xyzs, self.dirs, self.deltas, self.ts = z(cap, 3), z(cap, 3), z(cap), z(cap)
         self.emb, self.sig, self.rgbs = z(cap, 32, dtype=edt), z(cap), z(cap, 3, dtype=torch.float16)
         self.opacity, self.depth, self.rgb = z(n), z(n), z(n, 3)
-        self.coarse = None
-        import os
-        # The empty-space leap of the round march is opt-in (NGP_FRAME_LEAP=1): bit-exact (tests), but its exact
-        # super-cell box test cost more than the steps it skips on the Lego-sized box when it was measured.
-        use_leap = use_leap and os.environ.get("NGP_FRAME_LEAP", "0") == "1"
-        if use_leap and model.cascades == 1 and model.grid_size in (32, 64, 128) and self.esf == 0.0:
-            self.coarse = z(max((model.grid_size // 8) ** 3 // 32, 1), dtype=i32)
         self.aabb6 = (C.c_float * 6)(*[float(v) for v in model.xyz_min.flatten().tolist()],
                                      *[float(v) for v in (model.xyz_max - model.xyz_min).flatten().tolist()])
         self._w_keep = [w.detach().float().contiguous() for w in mlp_weights(model)]
@@ -167,11 +160,10 @@ class FrameRenderer:
         L, m, st, p, check = self._load(), self.model, self._C.c_void_p(torch.cuda.current_stream().cuda_stream), self._p, self._check
         cur, nxt = self.alive[j & 1], self.alive[(j + 1) & 1]
         check(L.ngp_frame_round_begin(p(self.state), st))
-        check(L.ngp_raymarching_round_capped(p(self.rays_o), p(self.rays_d), p(self.hits), p(m.density_bitfield),
-                                             m.cascades, m.grid_size, float(m.scale), self.esf, int(limit),
-                                             self.MAX_SAMPLES, p(cur), p(self.state), p(self.t_cur), p(self.n_marched),
-                                             p(self.rays_a), p(self.xyzs), p(self.dirs), p(self.deltas), p(self.ts),
-                                             self.n, self.cap, p(self.coarse), st))
+        check(L.ngp_raymarching_round(p(self.rays_o), p(self.rays_d), p(self.hits), p(m.density_bitfield),
+                                      m.cascades, m.grid_size, float(m.scale), self.esf, int(limit), self.MAX_SAMPLES,
+                                      p(cur), p(self.state), p(self.t_cur), p(self.n_marched), p(self.rays_a),
+                                      p(self.xyzs), p(self.dirs), p(self.deltas), p(self.ts), self.n, self.cap, st))
         check(m.pos_encoder.enqueue_encode_dyn(L, p(self.xyzs), p(self._table_t), p(self.emb), self.cap, p(self.state),
                                                self.aabb6, st))
         check(L.ngp_mlp_fwd_dyn(p(self.emb), self.tag, p(self.dirs), self._C.byref(self._wst), p(self.sig), p(self.rgbs),
@@ -185,8 +177,6 @@ class FrameRenderer:
         check(L.ngp_ray_aabb_intersect(p(self.rays_o), p(self.rays_d), float(m.scale), p(self.hits), self.n, st))
         check(L.ngp_frame_begin(p(self.hits), p(self.t_cur), p(self.n_marched), p(self.alive[0]), p(self.state),
                                 p(self.opacity), p(self.depth), p(self.rgb), self.n, st))
-        if self.coarse is not None:   # 8^3-cell dilated occupancy: lets the march leap over empty space
-            check(L.ngp_build_coarse_occupancy(p(m.density_bitfield), m.grid_size, p(self.coarse), st))
         for j, limit in enumerate(self.SCHEDULE):
             self._enqueue_round(j, limit)
 

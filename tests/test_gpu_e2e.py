@@ -76,12 +76,14 @@ def test_gui_render_cam():
     assert img.shape == (64, 64, 3) and torch.isfinite(img).all()
 
 
-def test_render_frame_equals_incremental_loop(lego_bitfield):
+def test_frame_paths_equal_incremental_loop(lego_bitfield):
     """Batched test-time rendering == the reference-shaped while-loop (chunking must not matter)."""
     import modules.rendering as R
     from datasets.ray_utils import get_ray_directions, get_rays
     from datasets.synthetic import SyntheticLego, hemisphere_poses
+    from modules.intersection import ray_aabb_intersection
     from modules.networks import NGP
+    from taichi_nerfs_b200.render_frame import render_frame
     torch.manual_seed(1)
     m = NGP(scale=0.5, max_res=1024, half_opt=True).cuda()
     with torch.no_grad():
@@ -91,12 +93,9 @@ def test_render_frame_equals_incremental_loop(lego_bitfield):
     o, d = get_rays(get_ray_directions(160, 160, K, device='cuda'), hemisphere_poses(3)[2].cuda())
     with torch.autocast('cuda', dtype=torch.float16):
         thr = 0.25    # a high termination threshold so that most rays that hit the medium terminate early
-        R._FORCE_LOOP = True
-        ref = R.render(m, o, d, test_time=True, T_threshold=thr)
-        R._FORCE_LOOP = False
-        R._NO_COMPACTION = True
-        allsamples = R.render(m, o, d, test_time=True, T_threshold=thr)   # march everything, shade everything, composite
-        R._NO_COMPACTION = False
+        o, d = o.contiguous(), d.contiguous()
+        ref = R._render_rays_test(m, o, d, ray_aabb_intersection(o, d, m.scale), T_threshold=thr)   # reference loop
+        allsamples = render_frame(m, o, d, T_threshold=thr)                # march everything, shade everything, composite
         got = R.render(m, o, d, test_time=True, T_threshold=thr)          # compacting rounds (one CUDA graph per frame)
         got2 = R.render(m, o, d, test_time=True, T_threshold=thr)         # replay of the cached graph
     assert float(ref['opacity'].max()) > 0.5

@@ -241,16 +241,15 @@ def _render(m, o, d, esf, thr):
         return R.render(m, T(o), T(d), test_time=True, exp_step_factor=esf, T_threshold=thr)
 
 
-def _frame_vs_oracle(name, half, thr, use_leap=False):
+def _frame_vs_oracle(name, half, thr):
     from oracle import oracle as O
     from taichi_nerfs_b200.render_frame import FrameRenderer
     cfg, m, om, o, d = _case(name, half)
     ref = render_test(om, o, d, cfg["esf"], thr)
     hits = O.ray_aabb_intersect(o, d, cfg["scale"])
     out = _render(m, o, d, cfg["esf"], thr)
-    fr = m._frame_renderers[(o.shape[0], float(cfg["esf"]), float(thr), T(o).device)]
-    assert (fr.coarse is not None) == use_leap
-    _check_frame(out, ref, hits, thr, f"{name} half={half} thr={thr} leap={use_leap}")
+    assert (o.shape[0], float(cfg["esf"]), float(thr), T(o).device) in m._frame_renderers   # the compacting renderer
+    _check_frame(out, ref, hits, thr, f"{name} half={half} thr={thr}")
     # graph replay == eager enqueue, bit for bit (per-ray results do not depend on row order)
     again = _render(m, o, d, cfg["esf"], thr)
     eager = FrameRenderer(m, o.shape[0], cfg["esf"], thr, use_graph=False).render(T(o), T(d))
@@ -276,12 +275,6 @@ def test_frame_garden(oracle):
     _frame_vs_oracle("garden", True, 1e-4)
 
 
-def test_frame_lego_leap(oracle, monkeypatch):
-    """The empty-space leap of the round march (NGP_FRAME_LEAP=1) renders the same frame."""
-    monkeypatch.setenv("NGP_FRAME_LEAP", "1")
-    _frame_vs_oracle("lego", True, 1e-4, use_leap=True)
-
-
 def test_frame_fog_stops_at_max_samples(oracle):
     """sigma = 1 everywhere, every cell occupied, no ray terminates: the rays outlast the scheduled rounds and take the
     host-driven extra rounds, which must stop every ray at max_samples samples like the one-shot march."""
@@ -303,14 +296,12 @@ def test_frame_fog_stops_at_max_samples(oracle):
 
 # ---- the non-compacting render_frame ----------------------------------------------------------------------------
 @pytest.mark.parametrize("name", ["lego", "garden"])
-def test_render_frame_matches_oracle(oracle, monkeypatch, name):
-    """render_frame (NGP_FRAME_COMPACT=0): the first frame marches in two passes and learns the row capacity, the
-    second takes the single-pass march; then a frame that needs more rows than were learned overflows the single-pass
-    buffers (dropped > 0) and is rendered again by the two-pass march."""
-    import modules.rendering as R
+def test_render_frame_passes_match_oracle(oracle, monkeypatch, name):
+    """render_frame (the path of models the compacting renderer does not take): the first frame marches in two passes
+    and learns the row capacity, the second takes the single-pass march; then a frame that needs more rows than were
+    learned overflows the single-pass buffers (dropped > 0) and is rendered again by the two-pass march."""
     from oracle import oracle as O
     from taichi_nerfs_b200 import render_frame as RF
-    monkeypatch.setattr(R, "_NO_COMPACTION", True)
     calls = dict(count=0, frame=0)
     real_count, real_frame = RF.ops.raymarching_train_count, RF.ops.raymarching_frame
 
@@ -327,11 +318,15 @@ def test_render_frame_matches_oracle(oracle, monkeypatch, name):
     monkeypatch.setattr(RF.ops, "raymarching_frame", frame)
     cfg, m, om, o, d = _case(name)
     thr = 1e-4
+
+    def render_frame(o, d):
+        with torch.autocast("cuda", dtype=torch.float16):
+            return RF.render_frame(m, T(o), T(d), cfg["esf"], thr)
     ref = render_test(om, o, d, cfg["esf"], thr)
     hits = O.ray_aabb_intersect(o, d, cfg["scale"])
-    first = _render(m, o, d, cfg["esf"], thr)
+    first = render_frame(o, d)
     assert calls == dict(count=1, frame=0)
-    second = _render(m, o, d, cfg["esf"], thr)
+    second = render_frame(o, d)
     assert calls["count"] == 1 and calls["frame"] == 1 and calls["dropped"] == 0
     for out, what in ((first, "two-pass"), (second, "single-pass")):
         _check_frame(out, ref, hits, thr, f"render_frame {name} {what}")
@@ -342,11 +337,11 @@ def test_render_frame_matches_oracle(oracle, monkeypatch, name):
     # learned capacity from a frame that misses the scene, then a frame that needs more rows
     m.__dict__.pop("_frame_capacity", None)
     away = o * 40.0                                         # far outside the box, looking away from it
-    empty = _render(m, away, -d, cfg["esf"], thr)
+    empty = render_frame(away, -d)
     assert int(empty["total_samples"]) == 0
     assert ref["S"] > 1 << 16
     calls.update(count=0, frame=0)
-    third = _render(m, o, d, cfg["esf"], thr)
+    third = render_frame(o, d)
     assert calls["frame"] == 1 and calls["dropped"] > 0 and calls["count"] == 1      # overflow -> two-pass march
     for k in ("opacity", "depth", "rgb", "total_samples"):
         assert torch.equal(third[k], first[k]), k

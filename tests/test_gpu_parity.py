@@ -667,30 +667,17 @@ def test_fused_grid_update_no_occupied_cells_and_erode(ops, oracle):
     np.testing.assert_array_equal(N(bits), bits_ref)
 
 
-# ---- compacting renderer: round march (resume points, empty-space leap) --------------------------------------------
+# ---- compacting renderer: round march (resume points, per-ray cap over the frame) ----------------------------------
 # garden scale, every cell occupied, rays from inside the box: every ray has more than max_samples candidate positions
 GARDEN_FULL = dict(scale=16.0, cascades=6, esf=1 / 256, occ="full")
 
 
-@pytest.mark.parametrize("leap", [False, True])
-def test_round_march_equals_full_march(ops, oracle, lego_bitfield, rays_factory, leap):
-    """The per-round march of the compacting frame renderer (persistent warps over a live list, <= limit samples per
-    ray and round, resume at t_cur, optional 256-position leap over empty space guided by the dilated coarse occupancy)
-    must emit, ray by ray, exactly the samples of the oracle's one-shot march with zero noise (bit-exact t, delta, xyz and
-    count), whatever the rounds.  Lego rays stay below max_samples, so the entry point without the cap gives them all."""
-    _check_round_march(ops, oracle, lego_bitfield, rays_factory, MARCH_CFGS[0], leap, capped=False)
-
-
-@pytest.mark.parametrize("leap", [False, True])
 @pytest.mark.parametrize("cfg", MARCH_CFGS + [GARDEN_FULL], ids=MARCH_IDS + ["6casc_full_capped"])
-def test_round_march_capped_equals_full_march(ops, oracle, lego_bitfield, rays_factory, cfg, leap):
-    """The round march as the frame renderer runs it, with the per-ray count that caps a ray at max_samples over all
-    rounds, at every march configuration.  The leap applies to one cascade with a constant step only: elsewhere the
-    kernel must ignore the coarse occupancy it is given."""
-    _check_round_march(ops, oracle, lego_bitfield, rays_factory, cfg, leap, capped=True)
-
-
-def _check_round_march(ops, oracle, lego_bitfield, rays_factory, cfg, leap, capped):
+def test_round_march_equals_full_march(ops, oracle, lego_bitfield, rays_factory, cfg):
+    """The per-round march of the compacting frame renderer (persistent warps over a live list, <= limit samples per
+    ray and round, resume at t_cur, a per-ray count that caps a ray at max_samples over all rounds) must emit, ray by
+    ray, exactly the samples of the oracle's one-shot march with zero noise (bit-exact t, delta, xyz and count),
+    whatever the rounds, at every march configuration."""
     import ctypes as C
     from taichi_nerfs_b200 import _lib
     L = _lib.load()
@@ -711,17 +698,6 @@ def _check_round_march(ops, oracle, lego_bitfield, rays_factory, cfg, leap, capp
     r_a = torch.zeros(n, 3, device="cuda", dtype=torch.int32)
     xyz, dirs = torch.empty(cap, 3, device="cuda"), torch.empty(cap, 3, device="cuda")
     dl, ts = torch.empty(cap, device="cuda"), torch.empty(cap, device="cuda")
-    coarse = None
-    if leap:
-        coarse = torch.zeros(128, device="cuda", dtype=torch.int32)
-        _lib.check(L.ngp_build_coarse_occupancy(p(bits), 128, p(coarse), st))    # from cascade 0
-        c = N(coarse).view(np.uint32)
-        # bit s = any occupied cell among the 512 Morton-consecutive cells (64 bytes) of super-cell s
-        want = np.packbits(bits_np[:128 ** 3 // 8].reshape(4096, 64).any(1), bitorder="little").view(np.uint32)
-        np.testing.assert_array_equal(c, want)
-        if cfg["occ"] == "lego":
-            occupied_sc = sum(bin(int(w)).count("1") for w in c)
-            assert 0 < occupied_sc < 4096 * 0.4, occupied_sc            # the Lego grid leaves most super-cells empty
     rows_ray, rows_t, rows_dl, rows_xyz = [], [], [], []
     schedule = [4, 8, 16, 3, 64, 128, 256, 512]
     rounds = 0
@@ -730,14 +706,9 @@ def _check_round_march(ops, oracle, lego_bitfield, rays_factory, cfg, leap, capp
         rounds += 1
         state.zero_()
         state[2] = n                                                  # every ray stays on the live list
-        pc = None if coarse is None else p(coarse)
-        if capped:
-            _lib.check(L.ngp_raymarching_round_capped(p(o), p(d), p(hits), p(bits), casc, 128, sc, esf, limit, 1024,
-                                                      p(alive), p(state), p(t_cur), p(n_marched), p(r_a), p(xyz),
-                                                      p(dirs), p(dl), p(ts), n, cap, pc, st))
-        else:
-            _lib.check(L.ngp_raymarching_round(p(o), p(d), p(hits), p(bits), casc, 128, sc, esf, limit, p(alive),
-                                               p(state), p(t_cur), p(r_a), p(xyz), p(dirs), p(dl), p(ts), n, cap, pc, st))
+        _lib.check(L.ngp_raymarching_round(p(o), p(d), p(hits), p(bits), casc, 128, sc, esf, limit, 1024, p(alive),
+                                           p(state), p(t_cur), p(n_marched), p(r_a), p(xyz), p(dirs), p(dl), p(ts),
+                                           n, cap, st))
         rows = int(state[0])
         eff = max(1, min(limit, cap // n))
         r_np = N(r_a)
@@ -750,8 +721,7 @@ def _check_round_march(ops, oracle, lego_bitfield, rays_factory, cfg, leap, capp
         rows_xyz.append(N(xyz)[idx])
     done = (t_cur == float("inf")) | (t_cur < 0)
     assert bool(done.all()), "every ray must have left the box or reached max_samples"
-    if capped:
-        np.testing.assert_array_equal(N(n_marched), ra[:, 2])          # per-ray sample count == the capped march's
+    np.testing.assert_array_equal(N(n_marched), ra[:, 2])              # per-ray sample count == the capped march's
     # rows of all rounds, stably grouped by ray (rounds in order) == the oracle's rows, which are in ray order
     order = np.argsort(np.concatenate(rows_ray), kind="stable")
     for got, want in ((rows_t, ts_ref), (rows_dl, dl_ref), (rows_xyz, xyz_ref)):
@@ -759,7 +729,5 @@ def _check_round_march(ops, oracle, lego_bitfield, rays_factory, cfg, leap, capp
         assert got.shape == want.shape
         assert np.array_equal(got.view(np.uint32), want.view(np.uint32))
     assert S > 30000
-    if not capped:
-        assert ra[:, 2].max() < 1024
     if cfg["occ"] == "full":
         assert (ra[:, 2] == 1024).mean() > 0.9            # the per-ray cap is what ends these rays
