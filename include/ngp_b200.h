@@ -310,6 +310,16 @@ int ngp_ray_head_fused(const float* sigmas, const void* rgbs, int rgbs_dtype, co
                        const int32_t* rays_a, const float* gt, float bg, float loss_scale,
                        const float* scale_dev, float T_threshold, float* loss_sum, float* opacity_out,
                        float* rgb_out, float* dL_dsigmas, void* dL_drgbs, int64_t n_rays, void* stream);
+/* The same head with the distortion loss (modules/distortion.py, train.py:194-195) in the same launch: the loss is
+ * mse + distortion_w * mean(loss_ray), loss_ray as in ngp_distortion_fwd over the composited weights.  Its dL/dw
+ * (ngp_distortion_bwd with dL_dloss = distortion_w / n_rays, times the loss scale) enters the composite backward as
+ * dL_dws does in ngp_composite_train_bwd.  *loss_sum accumulates sum((out-gt)^2) + 3 distortion_w sum(loss_ray), so
+ * that loss_sum / (3 n_rays) is the total loss.  ts are the sample midpoints; distortion_w >= 0 (0 adds nothing). */
+int ngp_ray_head_fused_distortion(const float* sigmas, const void* rgbs, int rgbs_dtype, const float* deltas,
+                                  const float* ts, const int32_t* rays_a, const float* gt, float bg,
+                                  float loss_scale, const float* scale_dev, float T_threshold,
+                                  float distortion_w, float* loss_sum, float* opacity_out, float* rgb_out,
+                                  float* dL_dsigmas, void* dL_drgbs, int64_t n_rays, void* stream);
 
 /* ---- distortion loss (SURVEY §8f rank 3) -------------------------------------- */
 /* replaces prefix_sums_kernel + _loss_kernel + distortion_loss_fw_kernel

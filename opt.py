@@ -43,7 +43,8 @@ _FLAGS = [
     ('--gui', dict(action='store_true', default=False, help='render an orbit with the GUI camera after training')),
     ('--graph_step', dict(action='store_true', default=False,
                           help='run the training step as one CUDA-graph replay (StaticTrainStep; stock NGP '
-                               'architecture, no distortion loss); same update as the default module path')),
+                               'architecture with the hash encoder, --distortion_loss_w included); same update as '
+                               'the default module path')),
     ('--deployment', dict(action='store_true', default=False)),
     ('--deployment_model_path', dict(type=str, default='./')),
 ]

@@ -69,6 +69,8 @@ def _declare(lib):
         "ngp_composite_train_bwd": (ci, [vp, vp, vp, vp, vp, vp, ci, vp, vp, vp, vp, vp, vp, f32, vp, vp, i64, i64, vp]),
         "ngp_composite_test": (ci, [vp, vp, ci, vp, vp, vp, vp, f32, vp, vp, vp, i64, vp]),
         "ngp_ray_head_fused": (ci, [vp, vp, ci, vp, vp, vp, f32, f32, vp, f32, vp, vp, vp, vp, vp, i64, vp]),
+        "ngp_ray_head_fused_distortion": (ci, [vp, vp, ci, vp, vp, vp, vp, f32, f32, vp, f32, f32, vp, vp, vp, vp, vp,
+                                               i64, vp]),
         "ngp_distortion_fwd": (ci, [vp, vp, vp, vp, vp, i64, i64, vp]),
         "ngp_distortion_bwd": (ci, [vp, vp, vp, vp, vp, vp, i64, i64, vp]),
         "ngp_packbits": (ci, [vp, f32, vp, i64, vp]),

@@ -297,35 +297,57 @@ __global__ void __launch_bounds__(256) mse_loss_grad_kernel(const float* __restr
 // One warp per ray does what composite_train_fwd_kernel, mse_loss_grad_kernel and composite_train_bwd_kernel do
 // in three launches: the ray's samples are read from HBM once (the reverse pass hits L1/L2), and the
 // per-sample ws / per-ray depth that the loss does not need are never written.
-template <typename T>
+//
+// kDist adds the distortion loss w_d * mean(distortion) (distortion_fwd_kernel / distortion_bwd_kernel) to the same
+// launch.  With W_<k, WT_<k the exclusive prefix sums of w and w t along the ray and W_>k, WT_>k the suffix sums:
+//   loss_ray = sum_k w_k (2 (t_k W_<k - WT_<k) + w_k delta_k / 3)
+//   dL/dw_k  = coef_d (2 (t_k W_<k - WT_<k) + 2 (WT_>k - t_k W_>k) + 2/3 w_k delta_k),  coef_d = scale w_d / n_rays
+// and dL/dw_k joins G_k, as dL_dws does in composite_train_bwd_kernel.  The prefix carries at every chunk start sit in
+// shared memory beside Tstart (the reverse pass rescans each chunk); the suffixes are accumulated by the reverse walk.
+template <typename T, bool kDist>
 __global__ void __launch_bounds__(kWarpsPerBlock * 32)
 ray_head_fused_kernel(const float* __restrict__ sigmas, const T* __restrict__ rgbs, const float* __restrict__ deltas,
-                      const int32_t* __restrict__ rays_a, const float* __restrict__ gt, float bg, float coef,
-                      const float* __restrict__ scale_dev, float thr, float* __restrict__ loss_sum,
-                      float* __restrict__ opacity_out, float* __restrict__ rgb_out, float* __restrict__ dsigmas,
-                      T* __restrict__ drgbs, int64_t n_rays) {
+                      const float* __restrict__ ts, const int32_t* __restrict__ rays_a, const float* __restrict__ gt,
+                      float bg, float coef, float coef_d, float w_d, const float* __restrict__ scale_dev, float thr,
+                      float* __restrict__ loss_sum, float* __restrict__ opacity_out, float* __restrict__ rgb_out,
+                      float* __restrict__ dsigmas, T* __restrict__ drgbs, int64_t n_rays) {
     __shared__ float Tstart_s[kWarpsPerBlock][kChunkCap];
+    __shared__ float Wstart_s[kDist ? kWarpsPerBlock : 1][kDist ? kChunkCap : 1];   // W_<k at every chunk start
+    __shared__ float WTstart_s[kDist ? kWarpsPerBlock : 1][kDist ? kChunkCap : 1];  // WT_<k at every chunk start
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
     const int64_t n = (int64_t)blockIdx.x * kWarpsPerBlock + wid;
     if (n >= n_rays) return;
-    if (scale_dev != nullptr) coef *= *scale_dev;
+    if (scale_dev != nullptr) {
+        coef *= *scale_dev;
+        if constexpr (kDist) coef_d *= *scale_dev;
+    }
     const int64_t ray = rays_a[n * 3 + 0], start = rays_a[n * 3 + 1];
     const int N = rays_a[n * 3 + 2];
     float* Tstart = Tstart_s[wid];
+    float* Wstart = Wstart_s[kDist ? wid : 0];
+    float* WTstart = WTstart_s[kDist ? wid : 0];
 
     // forward: colour / opacity sums, transmittance at every chunk start, last active chunk
     const int n_chunks = (N + 31) >> 5;
     int last_chunk = -1;
     float r = 0.f, g = 0.f, b = 0.f, op = 0.f;
+    float dist = 0.f;  // kDist: this lane's share of loss_ray
     {
         float Tc = 1.0f;
+        float Wc = 0.f, WTc = 0.f;  // kDist: W_<k, WT_<k at the chunk start
         for (int c = 0; c < n_chunks; ++c) {
             const int k = c * 32 + lane;
             const bool valid = k < N;
             const int64_t s = start + k;
-            float a = 0.f, c0 = 0.f, c1 = 0.f, c2 = 0.f;
+            float a = 0.f, c0 = 0.f, c1 = 0.f, c2 = 0.f, dl = 0.f, tm = 0.f;
             if (valid) {
-                a = 1.0f - expf(-sigmas[s] * deltas[s]);
+                if constexpr (kDist) {
+                    dl = deltas[s];
+                    tm = ts[s];
+                    a = 1.0f - expf(-sigmas[s] * dl);
+                } else {
+                    a = 1.0f - expf(-sigmas[s] * deltas[s]);
+                }
                 c0 = load_as_float(rgbs, s * 3 + 0);
                 c1 = load_as_float(rgbs, s * 3 + 1);
                 c2 = load_as_float(rgbs, s * 3 + 2);
@@ -340,6 +362,19 @@ ray_head_fused_kernel(const float* __restrict__ sigmas, const T* __restrict__ rg
             g += w * c1;
             b += w * c2;
             op += w;
+            if constexpr (kDist) {
+                const float wt = w * tm;
+                const float wi = warp_scan_add(w, lane), wti = warp_scan_add(wt, lane);
+                float we = __shfl_up_sync(0xffffffffu, wi, 1), wte = __shfl_up_sync(0xffffffffu, wti, 1);
+                if (lane == 0) we = wte = 0.0f;
+                dist += w * (2.0f * (tm * (Wc + we) - (WTc + wte)) + (1.0f / 3.0f) * w * dl);
+                if (lane == 0 && c < kChunkCap) {
+                    Wstart[c] = Wc;
+                    WTstart[c] = WTc;
+                }
+                Wc += __shfl_sync(0xffffffffu, wi, 31);
+                WTc += __shfl_sync(0xffffffffu, wti, 31);
+            }
             const unsigned act = __ballot_sync(0xffffffffu, active);
             const unsigned val = __ballot_sync(0xffffffffu, valid);
             if (lane == 0 && c < kChunkCap) Tstart[c] = Tc;
@@ -369,8 +404,11 @@ ray_head_fused_kernel(const float* __restrict__ sigmas, const T* __restrict__ rg
     const float d0 = r + keep - gt[ray * 3 + 0], d1 = g + keep - gt[ray * 3 + 1], d2 = b + keep - gt[ray * 3 + 2];
     const float gr = coef * d0, gg = coef * d1, gb = coef * d2;
     const float go = -bg * (gr + gg + gb);
+    if constexpr (kDist) dist = warp_sum(dist);
     if (lane == 0) {
-        atomicAdd(loss_sum, d0 * d0 + d1 * d1 + d2 * d2);
+        // kDist: loss_sum / (3 n_rays) = mse + w_d mean(loss_ray)
+        if constexpr (kDist) atomicAdd(loss_sum, d0 * d0 + d1 * d1 + d2 * d2 + 3.0f * w_d * dist);
+        else atomicAdd(loss_sum, d0 * d0 + d1 * d1 + d2 * d2);
         if (opacity_out) opacity_out[ray] = op;
         if (rgb_out) {
             rgb_out[ray * 3 + 0] = r + keep;
@@ -380,12 +418,37 @@ ray_head_fused_kernel(const float* __restrict__ sigmas, const T* __restrict__ rg
     }
     __syncwarp();
 
-    // backward: exact reverse suffix accumulation (same as composite_train_bwd_kernel with g_depth = g_ws = 0)
+    // backward: exact reverse suffix accumulation (same as composite_train_bwd_kernel with g_depth = 0, and g_ws = 0
+    // or the distortion term)
     float suffix = 0.0f;
+    float sW = 0.f, sWT = 0.f;  // kDist: sums of w and w t over the later chunks
     for (int c = last_chunk; c >= 0; --c) {
-        float Tc;
+        float Tc, Wc = 0.f, WTc = 0.f;
         if (c < kChunkCap) {
             Tc = Tstart[c];
+            if constexpr (kDist) {
+                Wc = Wstart[c];
+                WTc = WTstart[c];
+            }
+        } else if constexpr (kDist) {  // rare: > 4096 samples on one ray — redo the forward carries from the last kept
+            Tc = Tstart[kChunkCap - 1];
+            Wc = Wstart[kChunkCap - 1];
+            WTc = WTstart[kChunkCap - 1];
+            for (int c2i = kChunkCap - 1; c2i < c; ++c2i) {
+                const int k2 = c2i * 32 + lane;
+                const bool v2 = k2 < N;
+                const float dl2 = v2 ? deltas[start + k2] : 0.0f;
+                const float a2 = v2 ? 1.0f - expf(-sigmas[start + k2] * dl2) : 0.0f;
+                const float in2 = warp_scan_mul(1.0f - a2, lane);
+                float ex2 = __shfl_up_sync(0xffffffffu, in2, 1);
+                if (lane == 0) ex2 = 1.0f;
+                const float Tb2 = Tc * ex2;
+                const float w2 = v2 && Tb2 > thr ? a2 * Tb2 : 0.0f;
+                const float wt2 = w2 * (v2 ? ts[start + k2] : 0.0f);
+                Wc += __shfl_sync(0xffffffffu, warp_scan_add(w2, lane), 31);
+                WTc += __shfl_sync(0xffffffffu, warp_scan_add(wt2, lane), 31);
+                Tc = Tc * __shfl_sync(0xffffffffu, in2, 31);
+            }
         } else {
             Tc = Tstart[kChunkCap - 1];
             for (int c2i = kChunkCap - 1; c2i < c; ++c2i) {
@@ -398,13 +461,14 @@ ray_head_fused_kernel(const float* __restrict__ sigmas, const T* __restrict__ rg
         const int k = c * 32 + lane;
         const bool valid = k < N;
         const int64_t s = start + k;
-        float a = 0.f, dl = 0.f, c0 = 0.f, c1 = 0.f, c2v = 0.f;
+        float a = 0.f, dl = 0.f, c0 = 0.f, c1 = 0.f, c2v = 0.f, tm = 0.f;
         if (valid) {
             dl = deltas[s];
             a = 1.0f - expf(-sigmas[s] * dl);
             c0 = load_as_float(rgbs, s * 3 + 0);
             c1 = load_as_float(rgbs, s * 3 + 1);
             c2v = load_as_float(rgbs, s * 3 + 2);
+            if constexpr (kDist) tm = ts[s];
         }
         const float incl = warp_scan_mul(1.0f - a, lane);
         float excl = __shfl_up_sync(0xffffffffu, incl, 1);
@@ -412,7 +476,31 @@ ray_head_fused_kernel(const float* __restrict__ sigmas, const T* __restrict__ rg
         const float Tb = Tc * excl;
         const bool active = valid && Tb > thr;
         const float w = active ? a * Tb : 0.0f;
-        const float G = gr * c0 + gg * c1 + gb * c2v + go;
+        float G = gr * c0 + gg * c1 + gb * c2v + go;
+        if constexpr (kDist) {
+            const float wt = w * tm;
+            // prefix W_<k, WT_<k: the forward's own scan, from the same carries
+            const float wi = warp_scan_add(w, lane), wti = warp_scan_add(wt, lane);
+            float we = __shfl_up_sync(0xffffffffu, wi, 1), wte = __shfl_up_sync(0xffffffffu, wti, 1);
+            if (lane == 0) we = wte = 0.0f;
+            // suffix W_>k, WT_>k: reverse inclusive scan inside the chunk, shifted down one lane, plus the later chunks
+            float rw = w, rwt = wt;
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) {
+                const float nw = __shfl_down_sync(0xffffffffu, rw, o), nwt = __shfl_down_sync(0xffffffffu, rwt, o);
+                if (lane + o < 32) {
+                    rw += nw;
+                    rwt += nwt;
+                }
+            }
+            float lw = __shfl_down_sync(0xffffffffu, rw, 1), lwt = __shfl_down_sync(0xffffffffu, rwt, 1);
+            if (lane == 31) lw = lwt = 0.0f;
+            const float sel = tm * (Wc + we) - (WTc + wte);       // distortion.py:110; 0 at k = 0
+            const float later_d = (sWT + lwt) - tm * (sW + lw);
+            G += coef_d * (2.0f * (sel + later_d) + (2.0f / 3.0f) * w * dl);
+            sW += __shfl_sync(0xffffffffu, rw, 0);
+            sWT += __shfl_sync(0xffffffffu, rwt, 0);
+        }
         const float wG = w * G;
         float rs = wG;
 #pragma unroll
@@ -682,13 +770,40 @@ int ngp_ray_head_fused(const float* sigmas, const void* rgbs, int rgbs_dtype, co
     const unsigned grid = (unsigned)((n_rays + kWarpsPerBlock - 1) / kWarpsPerBlock);
     cudaStream_t st = ngp::as_stream(stream);
     if (rgbs_dtype == NGP_F16)
-        ray_head_fused_kernel<__half><<<grid, kWarpsPerBlock * 32, 0, st>>>(
-            sigmas, (const __half*)rgbs, deltas, rays_a, gt, bg, coef, scale_dev, T_threshold, loss_sum, opacity_out,
-            rgb_out, dL_dsigmas, (__half*)dL_drgbs, n_rays);
+        ray_head_fused_kernel<__half, false><<<grid, kWarpsPerBlock * 32, 0, st>>>(
+            sigmas, (const __half*)rgbs, deltas, nullptr, rays_a, gt, bg, coef, 0.0f, 0.0f, scale_dev, T_threshold,
+            loss_sum, opacity_out, rgb_out, dL_dsigmas, (__half*)dL_drgbs, n_rays);
     else
-        ray_head_fused_kernel<float><<<grid, kWarpsPerBlock * 32, 0, st>>>(
-            sigmas, (const float*)rgbs, deltas, rays_a, gt, bg, coef, scale_dev, T_threshold, loss_sum, opacity_out,
-            rgb_out, dL_dsigmas, (float*)dL_drgbs, n_rays);
+        ray_head_fused_kernel<float, false><<<grid, kWarpsPerBlock * 32, 0, st>>>(
+            sigmas, (const float*)rgbs, deltas, nullptr, rays_a, gt, bg, coef, 0.0f, 0.0f, scale_dev, T_threshold,
+            loss_sum, opacity_out, rgb_out, dL_dsigmas, (float*)dL_drgbs, n_rays);
+    NGP_LAUNCHED("ray_head_fused_kernel");
+    return 0;
+}
+
+int ngp_ray_head_fused_distortion(const float* sigmas, const void* rgbs, int rgbs_dtype, const float* deltas,
+                                  const float* ts, const int32_t* rays_a, const float* gt, float bg, float loss_scale,
+                                  const float* scale_dev, float T_threshold, float distortion_w, float* loss_sum,
+                                  float* opacity_out, float* rgb_out, float* dL_dsigmas, void* dL_drgbs, int64_t n_rays,
+                                  void* stream) {
+    NGP_REQUIRE(n_rays >= 0, "negative n_rays");
+    NGP_REQUIRE(rgbs_dtype == NGP_F32 || rgbs_dtype == NGP_F16, "bad dtype");
+    NGP_REQUIRE(distortion_w >= 0.0f && distortion_w < INFINITY, "distortion_w must be finite and >= 0");
+    if (n_rays == 0) return 0;
+    NGP_REQUIRE(sigmas && rgbs && deltas && ts && rays_a && gt && loss_sum && dL_dsigmas && dL_drgbs, "null pointer");
+    const float scale = scale_dev ? 1.0f : loss_scale;
+    const float coef = scale * 2.0f / (3.0f * (float)n_rays);
+    const float coef_d = scale * distortion_w / (float)n_rays;   // d(w_d mean(loss_ray)) / d loss_ray, scaled
+    const unsigned grid = (unsigned)((n_rays + kWarpsPerBlock - 1) / kWarpsPerBlock);
+    cudaStream_t st = ngp::as_stream(stream);
+    if (rgbs_dtype == NGP_F16)
+        ray_head_fused_kernel<__half, true><<<grid, kWarpsPerBlock * 32, 0, st>>>(
+            sigmas, (const __half*)rgbs, deltas, ts, rays_a, gt, bg, coef, coef_d, distortion_w, scale_dev,
+            T_threshold, loss_sum, opacity_out, rgb_out, dL_dsigmas, (__half*)dL_drgbs, n_rays);
+    else
+        ray_head_fused_kernel<float, true><<<grid, kWarpsPerBlock * 32, 0, st>>>(
+            sigmas, (const float*)rgbs, deltas, ts, rays_a, gt, bg, coef, coef_d, distortion_w, scale_dev,
+            T_threshold, loss_sum, opacity_out, rgb_out, dL_dsigmas, (float*)dL_drgbs, n_rays);
     NGP_LAUNCHED("ray_head_fused_kernel");
     return 0;
 }

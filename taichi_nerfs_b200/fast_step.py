@@ -4,8 +4,8 @@ Same math as NGPTrainer.step / the reference's loop body (train.py:184-201) — 
 the C-ABI kernels, enqueued in a fixed order on fixed buffers:
 
   [ray-batch sampler] -> ray_aabb -> single-pass march (capacity buffers, one atomic row reservation per ray) ->
-  hash fwd (+AABB normalisation) -> fused MLP fwd -> fused per-ray head (composite fwd + background + MSE +
-  composite bwd) -> MLP bwd -> hash bwd -> [gradient exchange] -> check_finite -> device-side LR/bias-correction update
+  hash fwd (+AABB normalisation) -> fused MLP fwd -> fused per-ray head (composite fwd + background + MSE
+  [+ distortion loss] + composite bwd) -> MLP bwd -> hash bwd -> [gradient exchange] -> check_finite -> device-side LR/bias-correction update
   -> fused Adam (+fp16 shadow, grad zero) -> device-side GradScaler update
 
 What makes it graph-capturable: the number of samples S stays on the device (kernels read it from the
@@ -31,7 +31,7 @@ def _p(t):
 class StaticTrainStep:
     def __init__(self, trainer, n_rays: int, samples_per_ray_capacity: int = 384, exp_step_factor: float = 0.0,
                  T_threshold: float = 1e-4, max_samples: int = 1024, use_graph: bool = True,
-                 dynamic_loss_scale: bool = True, overlap_optimizer: bool = False):
+                 dynamic_loss_scale: bool = True, overlap_optimizer: bool = False, distortion_loss_w: float = 0.0):
         self.tr = trainer
         m = self.model = trainer.model
         enc = m.pos_encoder
@@ -44,6 +44,10 @@ class StaticTrainStep:
         self.dev, self.n = dev, int(n_rays)
         self.cap = C_ = int(n_rays) * int(samples_per_ray_capacity)
         self.esf, self.T_thr, self.max_samples = float(exp_step_factor), float(T_threshold), int(max_samples)
+        # weight of the distortion loss (train.py --distortion_loss_w): loss = mse + w * mean(distortion per ray)
+        self.distortion_w = float(distortion_loss_w)
+        if not self.distortion_w >= 0.0 or self.distortion_w == float("inf"):
+            raise ValueError(f"distortion_loss_w must be finite and >= 0, got {distortion_loss_w}")
         self.half = hasattr(enc, "table_f16")
         edt = torch.float16 if self.half else torch.float32
         f32, i32 = torch.float32, torch.int32
@@ -164,8 +168,15 @@ class StaticTrainStep:
                                 _p(self.mlp_save), self.cap, _p(self.counter), st))
 
     def _k_head(self):
-        # composite forward + background + MSE + composite backward in one launch (per-ray work)
+        # composite forward + background + MSE [+ distortion loss] + composite backward in one launch (per-ray work)
         bg = 1.0 if self.esf == 0 else 0.0
+        if self.distortion_w > 0:
+            check(load().ngp_ray_head_fused_distortion(
+                _p(self.sig), _p(self.rgbs), F16, _p(self.deltas), _p(self.ts), _p(self.rays_a), _p(self.gt), bg,
+                float(self.tr.loss_scale), _p(self.scale_state) if self.dynamic_loss_scale else None, self.T_thr,
+                self.distortion_w, _p(self.loss_sum), _p(self.opacity), _p(self.rgb), _p(self.dsig), _p(self.drgbs),
+                self.n, self._st()))
+            return
         check(load().ngp_ray_head_fused(_p(self.sig), _p(self.rgbs), F16, _p(self.deltas), _p(self.rays_a), _p(self.gt),
                                         bg, float(self.tr.loss_scale),
                                         _p(self.scale_state) if self.dynamic_loss_scale else None, self.T_thr,
