@@ -187,6 +187,15 @@ int ngp_triplane_encode_fwd_dyn(const float* xyz, const float* table, const ngp_
  * buffer.  xyz in [0,1] (no aabb).  There is no dL/dxyz (the reference returns None, :197). */
 int ngp_triplane_encode_bwd(const float* xyz, const float* table, const float* dout,
                             const ngp_triplane_layout* layout, float* grad_table, int64_t n, void* stream);
+/* the same with the row count read on the device, for the graph-captured training step: rows
+ * [0, min(n_max, max(*n_dev, 0))) (n_dev == NULL: n_max rows); rows at or beyond the count are never read.
+ * `aabb6` as in the forward (world positions, normalised by the same arithmetic, so the geometry is the forward's bit
+ * for bit).  found_inf_or_null: set to 1 when a non-finite value is handed to a reduction - GradScaler's inf check
+ * raised at the source (see ngp_hash_encode_bwd_levels); a row whose dout is zero in all F columns of a level issues
+ * no reduction and raises nothing.  ngp_triplane_encode_bwd is this call with n_dev = aabb6 = found_inf = NULL. */
+int ngp_triplane_encode_bwd_dyn(const float* xyz, const float* table, const float* dout,
+                                const ngp_triplane_layout* layout, float* grad_table, int64_t n_max,
+                                const int32_t* n_dev, const float* aabb6, int32_t* found_inf_or_null, void* stream);
 
 /* ---- sync-free ("_dyn") variants used by the graph-captured training step -------------------
  * Same kernels as above, but the number of valid rows is read ON THE DEVICE: rows [0, min(n_max,*n_dev))

@@ -85,3 +85,9 @@ class TriPlaneEncoder(torch.nn.Module):
         """Raw launch of the device-counted encode (FrameRenderer's rounds): pointers in, rc out."""
         return lib.ngp_triplane_encode_fwd_dyn(xyzs, table, ctypes.byref(self._clayout), emb, n_max, n_dev, aabb6,
                                                stream)
+
+    def enqueue_encode_bwd_dyn(self, lib, xyzs, table, demb, grad_table, n_max, n_dev, aabb6, found_inf, stream):
+        """Raw launch of the device-counted table backward (the graph-captured training step): grad_table += dL/dtable
+        of the first min(n_max, *n_dev) rows; found_inf (may be None) is raised on a non-finite contribution."""
+        return lib.ngp_triplane_encode_bwd_dyn(xyzs, table, demb, ctypes.byref(self._clayout), grad_table, n_max,
+                                               n_dev, aabb6, found_inf, stream)

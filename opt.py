@@ -20,7 +20,8 @@ _FLAGS = [
     ('--half_opt', dict(action='store_true', default=False, help='whether to use half optimization')),
     ('--encoder_type', dict(type=str, default='hash', choices=['hash', 'triplane'],
                         help='which encoder to use: the multiresolution hash grid or the tri-plane encoder (fp32 '
-                             'planes; not with --half_opt, --graph_step or --deployment)')),
+                             'planes; not with --half_opt or --deployment; --graph_step is not wired to it yet, '
+                             'StaticTrainStep runs it)')),
     ('--sh_degree', dict(type=int, default=2, help='degree of spherical harmonics (svox only; unused)')),
     ('--grid_size', dict(type=int, default=256, help='size of voxel grid in each dimension (svox only; unused)')),
     ('--grid_radius', dict(type=float, default=0.0125, help='radius of voxel grid points (svox only; unused)')),
@@ -43,7 +44,8 @@ _FLAGS = [
     ('--gui', dict(action='store_true', default=False, help='render an orbit with the GUI camera after training')),
     ('--graph_step', dict(action='store_true', default=False,
                           help='run the training step as one CUDA-graph replay (StaticTrainStep; stock NGP '
-                               'architecture with the hash encoder, --distortion_loss_w included); same update as '
+                               'architecture, --distortion_loss_w included; this switch takes the hash encoder only); '
+                               'same update as '
                                'the default module path')),
     ('--deployment', dict(action='store_true', default=False)),
     ('--deployment_model_path', dict(type=str, default='./')),
@@ -57,7 +59,8 @@ def get_opts(prefix_args=None):
     hparams = parser.parse_args(prefix_args)
     if hparams.encoder_type == 'triplane':
         for flag, why in (('half_opt', 'the tri-plane table is fp32 (an fp16 plane table is not supported)'),
-                          ('graph_step', 'the graph-captured step runs the hash encoder only'),
+                          ('graph_step', 'this switch is not wired to the tri-plane encoder yet (the graph-captured step '
+                                         'itself runs it: taichi_nerfs_b200.fast_step.StaticTrainStep)'),
                           ('deployment', 'the deployment export (mobile demo format) is hash-only')):
             if getattr(hparams, flag):
                 parser.error(f"--encoder_type triplane does not combine with --{flag}: {why}")

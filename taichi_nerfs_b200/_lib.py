@@ -53,6 +53,7 @@ def _declare(lib):
         "ngp_triplane_encode_fwd": (ci, [vp, vp, tri, vp, i64, vp, vp]),
         "ngp_triplane_encode_fwd_dyn": (ci, [vp, vp, tri, vp, i64, vp, vp, vp]),
         "ngp_triplane_encode_bwd": (ci, [vp, vp, vp, tri, vp, i64, vp]),
+        "ngp_triplane_encode_bwd_dyn": (ci, [vp, vp, vp, tri, vp, i64, vp, vp, vp, vp]),
         "ngp_mlp_fwd_dyn": (ci, [vp, ci, vp, mw, vp, vp, vp, i64, vp, vp]),
         "ngp_mlp_bwd_dyn": (ci, [vp, ci, vp, mw, vp, vp, vp, vp, vp, i64, vp, vp, vp]),
         "ngp_adam_step_dyn": (ci, [vp, vp, vp, vp, vp, vp, vp, f32, f32, f32, ci, i64, vp]),

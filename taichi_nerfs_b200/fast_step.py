@@ -4,8 +4,8 @@ Same math as NGPTrainer.step / the reference's loop body (train.py:184-201) — 
 the C-ABI kernels, enqueued in a fixed order on fixed buffers:
 
   [ray-batch sampler] -> ray_aabb -> single-pass march (capacity buffers, one atomic row reservation per ray) ->
-  hash fwd (+AABB normalisation) -> fused MLP fwd -> fused per-ray head (composite fwd + background + MSE
-  [+ distortion loss] + composite bwd) -> MLP bwd -> hash bwd -> [gradient exchange] -> check_finite -> device-side LR/bias-correction update
+  hash (or tri-plane) fwd (+AABB normalisation) -> fused MLP fwd -> fused per-ray head (composite fwd + background + MSE
+  [+ distortion loss] + composite bwd) -> MLP bwd -> hash (or tri-plane) bwd -> [gradient exchange] -> check_finite -> device-side LR/bias-correction update
   -> fused Adam (+fp16 shadow, grad zero) -> device-side GradScaler update
 
 What makes it graph-capturable: the number of samples S stays on the device (kernels read it from the
@@ -37,9 +37,10 @@ class StaticTrainStep:
         enc = m.pos_encoder
         if not m._fusable(next(m.parameters())):
             raise _lib.NgpError("StaticTrainStep needs the stock NGP architecture (fused MLP)")
-        if not hasattr(enc, "hash_table"):
-            raise _lib.NgpError("StaticTrainStep runs the hash encoder's kernels; the graph-captured step does not "
-                                "support the tri-plane encoder (train it without --graph_step)")
+        # the tri-plane model: fp32 planes and embedding, no fp16 shadow; the encode launches go through the encoder
+        self.tri = hasattr(enc, "plane_embedding")
+        if not self.tri and not hasattr(enc, "hash_table"):
+            raise _lib.NgpError("StaticTrainStep runs the hash or the tri-plane encoder's kernels")
         dev = next(m.parameters()).device
         self.dev, self.n = dev, int(n_rays)
         self.cap = C_ = int(n_rays) * int(samples_per_ray_capacity)
@@ -78,7 +79,7 @@ class StaticTrainStep:
         self._w_keep = [w.detach() for w in mlp_weights(m)]
         self._wst = _lib.MlpWeights(*[w.data_ptr() for w in self._w_keep])
         self.P = enc.total_param_size
-        assert trainer.slices[0] == (0, self.P), "hash table must be the first parameter"
+        assert trainer.slices[0] == (0, self.P), "the encoder's table must be the first parameter"
         offs = [o for o, _ in trainer.slices[1:]]
         assert offs == [self.P, self.P + 2048, self.P + 3072, self.P + 5120, self.P + 9216], offs
         # valid placeholder rays (an all-zero direction would march forever, in the reference too)
@@ -100,8 +101,9 @@ class StaticTrainStep:
         # one rank or the peer-memory step + dynamic loss scale: the backward kernels raise GradScaler's inf flag
         # themselves (a non-finite contribution is seen where it is scattered), the optimizer consumes and clears it -
         # no 45 MB check pass (the NCCL fallback checks the reduced fp16 sum instead)
+        # (the hash backward raises it in its F = 2 instantiation only, the tri-plane backward in both)
         self.inf_at_source = bool((trainer.world_size == 1 or trainer.p2p is not None) and self.dynamic_loss_scale
-                                  and enc._clayout.feat_dim == 2)
+                                  and (self.tri or enc._clayout.feat_dim == 2))
         if self.inf_at_source:
             trainer.found_inf.zero_()
         self.use_graph = bool(use_graph)
@@ -143,6 +145,8 @@ class StaticTrainStep:
         return C.c_void_p(torch.cuda.current_stream().cuda_stream)
 
     def _table(self):
+        if self.tri:
+            return self.model.pos_encoder.kernel_table()   # a view of the trainer's flat_param: stable across steps
         return self.tr._shadow if self.half else self.model.pos_encoder.hash_table.data
 
     def _enqueue_march(self):
@@ -157,8 +161,13 @@ class StaticTrainStep:
                                       _p(self.deltas), _p(self.ts), n, cap, st))
 
     # the five network kernels, one method each (bench.py times them one by one on the buffers of a real step)
+    # (the two _k_hash_* are "the position encoder": for a tri-plane model they run its launches)
     def _k_hash_fwd(self):
         L, st, tag = load(), self._st(), (F16 if self.half else F32)
+        if self.tri:
+            check(self.model.pos_encoder.enqueue_encode_dyn(L, _p(self.xyzs), _p(self._table()), _p(self.emb),
+                                                            self.cap, _p(self.counter), self.aabb6, st))
+            return
         check(L.ngp_hash_encode_fwd_dyn(_p(self.xyzs), _p(self._table()), C.byref(self._clayout), _p(self.emb), tag,
                                         self.cap, _p(self.counter), self.aabb6, st))
 
@@ -192,6 +201,14 @@ class StaticTrainStep:
 
     def _k_hash_bwd(self, level_begin=0, level_end=None):
         L, st, tag = load(), self._st(), (F16 if self.half else F32)
+        if self.tri:
+            if level_begin != 0 or level_end is not None:
+                raise _lib.NgpError("level_begin / level_end select hash levels; all tri-plane levels scatter into "
+                                    "the same three planes")
+            check(self.model.pos_encoder.enqueue_encode_bwd_dyn(
+                L, _p(self.xyzs), _p(self._table()), _p(self.demb), _p(self.tr.flat_grad), self.cap, _p(self.counter),
+                self.aabb6, _p(self.tr.found_inf) if self.inf_at_source else None, st))
+            return
         level_end = self._clayout.n_levels if level_end is None else level_end
         check(L.ngp_hash_encode_bwd_levels(_p(self.xyzs), _p(self.demb), tag, C.byref(self._clayout),
                                            _p(self.tr.flat_grad), self.cap, _p(self.counter), self.aabb6,

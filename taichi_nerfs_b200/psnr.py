@@ -21,8 +21,9 @@ def train_vs_teacher(device, steps: int = 3000, batch: int = 8192, train_views: 
                      downsample: float = 0.5, seed: int = 23, half_opt: bool = True, graph: bool = True,
                      teacher=None, log=None, pos_encoder_type: str = 'hash'):
     """pos_encoder_type='triplane' trains the reference's tri-plane model instead (fp32 planes: half_opt does not
-    apply and the loss scale is 2**19, as train.py without --half_opt; the graph-captured step is hash-only, so pass
-    graph=False).  Returns {"psnr": mean dB over the held-out views, "psnr_views": [...], "steps": ..., "steps_per_s": ...,
+    apply and the loss scale is 2**19, as train.py without --half_opt).  graph=True trains through the graph-captured
+    step (StaticTrainStep, either encoder), graph=False through NGPTrainer.step; "path" in the result says which.
+    Returns {"psnr": mean dB over the held-out views, "psnr_views": [...], "steps": ..., "steps_per_s": ...,
     "rays_per_s": ..., "model": the trained NGP} or None when the teacher fixture is not staged."""
     from datasets.ray_utils import get_rays
     from datasets.teacher import TeacherLego, load_teacher
