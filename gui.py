@@ -10,7 +10,7 @@ import numpy as np
 import torch
 
 from datasets.ray_utils import get_ray_directions, get_rays
-from modules.networks import NGP
+from modules.networks import MODEL_DICT
 from modules.rendering import render
 from modules.utils import depth2img
 
@@ -88,7 +88,7 @@ class OrbitCamera:
 class NGPGUI:
     def __init__(self, hparams, model_config, K, img_wh, poses, radius=4.5):
         self.hparams = hparams
-        self.model = NGP(**model_config).cuda()
+        self.model = MODEL_DICT[getattr(hparams, 'model_name', 'ngp')](**model_config).cuda()
         if getattr(hparams, 'ckpt_path', None):
             print(f"loading ckpt from: {hparams.ckpt_path}")
             self.model.load_state_dict(torch.load(hparams.ckpt_path, map_location='cuda'))

@@ -69,6 +69,20 @@ typedef struct ngp_triplane_layout {
     uint32_t resolutions[NGP_MAX_LEVELS]; /* ceil(scale)+1                         */
 } ngp_triplane_layout;
 
+/*
+ * Voxel-grid layout (`--model_name svox`, the reference's VoxelGrid, modules/networks.py:382-575): a G^3 lattice of
+ * nodes ((i,j,k) - ceil(G/2) + 1) * radius (networks.py:450-466), i.e. node 0 at c_min = (1 - ceil(G/2)) * radius
+ * on every axis (rounded to fp32 on the host).  sh field [G,G,G,3*(deg+1)^2] and density field [G,G,G], node
+ * (i,j,k) at ((i*G + j)*G + k).
+ */
+#define NGP_VOXEL_MAX_GRID 2048
+typedef struct ngp_voxel_layout {
+    int32_t grid;        /* G, 1..NGP_VOXEL_MAX_GRID                        */
+    int32_t sh_degree;   /* 0, 1 or 2                                       */
+    float   radius;      /* node spacing                                    */
+    float   c_min;       /* world coordinate of node 0 on every axis        */
+} ngp_voxel_layout;
+
 /* Weights of the tiny NGP MLP (modules/networks.py:111-132): no biases.
  * Row-major [out, in] exactly like torch.nn.Linear.weight, fp32 master copy. */
 typedef struct ngp_mlp_weights {
@@ -196,6 +210,32 @@ int ngp_triplane_encode_bwd(const float* xyz, const float* table, const float* d
 int ngp_triplane_encode_bwd_dyn(const float* xyz, const float* table, const float* dout,
                                 const ngp_triplane_layout* layout, float* grad_table, int64_t n_max,
                                 const int32_t* n_dev, const float* aabb6, int32_t* found_inf_or_null, void* stream);
+
+/* ---- voxel grid (`--model_name svox`) ---------------------------------------------------------- */
+/* forward: the reference's VoxelGrid.forward / query_grids (modules/networks.py:521-575) with the semantics it leaves
+ * undefined decided in DESIGN.md §6d.  xyz [n,3] world positions, dirs [n,3] (normalised in the kernel, as in
+ * NGP.forward, networks.py:152-166) -> sigma [n] = ReLU(trilinear density), rgb [n,3] =
+ * sigmoid(sum_k Y_k(d) * sh[c*D + k]) (real SH basis of modules/sh_utils.py:58-113, degree <= 2), all fp32.  Corners
+ * outside [0, G) contribute zero (the out-of-grid mask, networks.py:489-508, :552).  rgb == NULL: density-only mode
+ * (sh and dirs are not read); its sigma is bit-identical to the full forward's. */
+int ngp_voxel_fwd(const float* xyz, const float* dirs, const float* sh, const float* density,
+                  const ngp_voxel_layout* layout, float* sigma, float* rgb, int64_t n, void* stream);
+/* the same with the row count read on the device: rows [0, min(n_max, max(*n_dev, 0))); rows beyond are not
+ * written. */
+int ngp_voxel_fwd_dyn(const float* xyz, const float* dirs, const float* sh, const float* density,
+                      const ngp_voxel_layout* layout, float* sigma, float* rgb, int64_t n_max, const int32_t* n_dev,
+                      void* stream);
+/* backward wrt the fields: dsh += dL/dsh, ddensity += dL/ddensity, ACCUMULATED into the caller's fp32 buffers.
+ * sigma and rgb are the forward's outputs (they give the ReLU mask sigma > 0 and the sigmoid derivative
+ * rgb*(1-rgb)); dsigma [n], drgb [n,3] fp32.  No dL/dxyz, no dL/ddirs.  found_inf_or_null: set to 1 when a
+ * non-finite value is handed to a reduction (GradScaler's inf check at the source).  mapping: NGP_VOXEL_BWD_WARP
+ * (lanes walk one corner's channels: one coalesced scatter instruction per corner) or NGP_VOXEL_BWD_THREAD (one thread
+ * per sample issues all 8 * (3D+1) reductions; kept for comparison). */
+#define NGP_VOXEL_BWD_WARP 0
+#define NGP_VOXEL_BWD_THREAD 1
+int ngp_voxel_bwd(const float* xyz, const float* dirs, const float* sigma, const float* rgb, const float* dsigma,
+                  const float* drgb, const ngp_voxel_layout* layout, float* dsh, float* ddensity, int64_t n,
+                  int32_t* found_inf_or_null, int mapping, void* stream);
 
 /* ---- sync-free ("_dyn") variants used by the graph-captured training step -------------------
  * Same kernels as above, but the number of valid rows is read ON THE DEVICE: rows [0, min(n_max,*n_dev))

@@ -44,6 +44,25 @@ def _grid_coords(n: int) -> torch.Tensor:
     return torch.stack([d, w, h], dim=-1).reshape(-1, 3).contiguous()
 
 
+def init_occupancy_grid(model: nn.Module, scale: float) -> None:
+    """The scene box and the cascaded 128^3 occupancy grid (networks.py:55-86): the buffers center, xyz_min, xyz_max,
+    half_size, density_bitfield, density_grid, grid_coords (registered in this order) and the attributes scale,
+    cascades, grid_size that the marches and the grid update read."""
+    model.scale = scale
+    model.register_buffer('center', torch.zeros(1, 3))
+    model.register_buffer('xyz_min', -torch.ones(1, 3) * scale)
+    model.register_buffer('xyz_max', torch.ones(1, 3) * scale)
+    model.register_buffer('half_size', (model.xyz_max - model.xyz_min) / 2)
+
+    # cascade k covers [-2^(k-1), 2^(k-1)]^3 (networks.py:62-63)
+    model.cascades = max(1 + int(math.ceil(math.log2(2 * scale))), 1)
+    model.grid_size = 128
+    g3 = model.grid_size ** 3
+    model.register_buffer('density_bitfield', torch.zeros(model.cascades * g3 // 8, dtype=torch.uint8))
+    model.register_buffer('density_grid', torch.zeros(model.cascades, g3))
+    model.register_buffer('grid_coords', _grid_coords(model.grid_size))
+
+
 class NGP(nn.Module):
 
     def __init__(
@@ -65,20 +84,8 @@ class NGP(nn.Module):
             rgb_net_width: int = 64,
     ):
         super().__init__()
-        self.scale = scale
         self.half_opt = half_opt
-        self.register_buffer('center', torch.zeros(1, 3))
-        self.register_buffer('xyz_min', -torch.ones(1, 3) * scale)
-        self.register_buffer('xyz_max', torch.ones(1, 3) * scale)
-        self.register_buffer('half_size', (self.xyz_max - self.xyz_min) / 2)
-
-        # cascade k covers [-2^(k-1), 2^(k-1)]^3 (networks.py:62-63)
-        self.cascades = max(1 + int(math.ceil(math.log2(2 * scale))), 1)
-        self.grid_size = 128
-        g3 = self.grid_size ** 3
-        self.register_buffer('density_bitfield', torch.zeros(self.cascades * g3 // 8, dtype=torch.uint8))
-        self.register_buffer('density_grid', torch.zeros(self.cascades, g3))
-        self.register_buffer('grid_coords', _grid_coords(self.grid_size))
+        init_occupancy_grid(self, scale)
 
         if pos_encoder_type == 'hash':
             if half_opt:
@@ -349,3 +356,7 @@ class MLP(nn.Module):
 
 
 MODEL_DICT = {'ngp': NGP}
+
+# modules/voxel_grid.py shares NGP's occupancy-grid methods and adds MODEL_DICT['svox'] when it is loaded; importing the
+# module object (not a name from it) keeps either import order working
+from . import voxel_grid  # noqa: E402,F401

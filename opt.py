@@ -15,18 +15,24 @@ _FLAGS = [
                      help='use which split to train')),
     ('--downsample', dict(type=float, default=1.0, help='downsample factor (<=1.0) for the images')),
     # model parameters
-    ('--model_name', dict(type=str, default='ngp', choices=['ngp'], help='which model to train/test')),
+    ('--model_name', dict(type=str, default='ngp', choices=['ngp', 'svox'],
+                          help='which model to train/test: ngp (hash or tri-plane encoder + MLPs) or svox (voxel grid '
+                               'of spherical-harmonics coefficients and densities; not with --encoder_type triplane, '
+                               '--graph_step or --deployment)')),
     ('--scale', dict(type=float, default=0.5, help='scene scale (whole scene must lie in [-scale, scale]^3')),
     ('--half_opt', dict(action='store_true', default=False, help='whether to use half optimization')),
     ('--encoder_type', dict(type=str, default='hash', choices=['hash', 'triplane'],
                         help='which encoder to use: the multiresolution hash grid or the tri-plane encoder (fp32 '
                              'planes; not with --half_opt or --deployment; --graph_step is not wired to it yet, '
                              'StaticTrainStep runs it)')),
-    ('--sh_degree', dict(type=int, default=2, help='degree of spherical harmonics (svox only; unused)')),
-    ('--grid_size', dict(type=int, default=256, help='size of voxel grid in each dimension (svox only; unused)')),
-    ('--grid_radius', dict(type=float, default=0.0125, help='radius of voxel grid points (svox only; unused)')),
-    ('--origin_sh', dict(type=float, default=0., help='origin value of sh coeffs in voxel grid (unused)')),
-    ('--origin_sigma', dict(type=float, default=0.1, help='origin value of sigma in voxel grid (unused)')),
+    ('--sh_degree', dict(type=int, default=2, help='degree of spherical harmonics: 0, 1 or 2 (svox only)')),
+    ('--grid_size', dict(type=int, default=256, help='nodes of the voxel grid in each dimension (svox only; the '
+                                                     'occupancy grid stays 128^3)')),
+    ('--grid_radius', dict(type=float, default=0.0125, help='spacing of the voxel grid nodes (svox only)')),
+    ('--origin_sh', dict(type=float, default=0., help='initial value of the sh coefficients in the voxel grid '
+                                                      '(svox only)')),
+    ('--origin_sigma', dict(type=float, default=0.1, help='initial value of the density in the voxel grid '
+                                                          '(svox only)')),
     # loss parameters
     ('--distortion_loss_w', dict(type=float, default=0, help='weight of distortion loss, 0 to disable (default)')),
     # training options
@@ -57,6 +63,16 @@ def get_opts(prefix_args=None):
     for flag, kw in _FLAGS:
         parser.add_argument(flag, **kw)
     hparams = parser.parse_args(prefix_args)
+    if hparams.model_name == 'svox':
+        for flag, bad, why in (
+                ('encoder_type', hparams.encoder_type == 'triplane',
+                 'the voxel grid has no position encoder (--encoder_type applies to ngp)'),
+                ('graph_step', hparams.graph_step,
+                 'the graph-captured step runs the NGP encoder + MLP kernels; train the voxel grid without it'),
+                ('deployment', hparams.deployment, 'the deployment export (mobile demo format) is hash-only')):
+            if bad:
+                parser.error(f"--model_name svox does not combine with --{flag}"
+                             f"{' triplane' if flag == 'encoder_type' else ''}: {why}")
     if hparams.encoder_type == 'triplane':
         for flag, why in (('half_opt', 'the tri-plane table is fp32 (an fp16 plane table is not supported)'),
                           ('graph_step', 'this switch is not wired to the tri-plane encoder yet (the graph-captured step '

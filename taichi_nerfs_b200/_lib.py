@@ -10,7 +10,7 @@ import ctypes as C
 import os
 import threading
 
-from .layout import CHashLayout, CTriplaneLayout
+from .layout import CHashLayout, CTriplaneLayout, CVoxelLayout
 
 _PKG = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_PKG, "lib", "libngp_b200.so")
@@ -33,6 +33,7 @@ def _declare(lib):
     i64, i32, f32, vp, ci = C.c_int64, C.c_int32, C.c_float, C.c_void_p, C.c_int
     lay = C.POINTER(CHashLayout)
     tri = C.POINTER(CTriplaneLayout)
+    vox = C.POINTER(CVoxelLayout)
     mw = C.POINTER(MlpWeights)
     sigs = {
         "ngp_version": (ci, []),
@@ -54,6 +55,9 @@ def _declare(lib):
         "ngp_triplane_encode_fwd_dyn": (ci, [vp, vp, tri, vp, i64, vp, vp, vp]),
         "ngp_triplane_encode_bwd": (ci, [vp, vp, vp, tri, vp, i64, vp]),
         "ngp_triplane_encode_bwd_dyn": (ci, [vp, vp, vp, tri, vp, i64, vp, vp, vp, vp]),
+        "ngp_voxel_fwd": (ci, [vp, vp, vp, vp, vox, vp, vp, i64, vp]),
+        "ngp_voxel_fwd_dyn": (ci, [vp, vp, vp, vp, vox, vp, vp, i64, vp, vp]),
+        "ngp_voxel_bwd": (ci, [vp, vp, vp, vp, vp, vp, vox, vp, vp, i64, vp, ci, vp]),
         "ngp_mlp_fwd_dyn": (ci, [vp, ci, vp, mw, vp, vp, vp, i64, vp, vp]),
         "ngp_mlp_bwd_dyn": (ci, [vp, ci, vp, mw, vp, vp, vp, vp, vp, i64, vp, vp, vp]),
         "ngp_adam_step_dyn": (ci, [vp, vp, vp, vp, vp, vp, vp, f32, f32, f32, ci, i64, vp]),

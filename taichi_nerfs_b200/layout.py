@@ -195,3 +195,58 @@ def make_triplane_layout(levels: int = 16, base_res: float = 16.0, max_res: int 
         lay.scales.append(scale)
         lay.resolutions.append(res)
     return lay
+
+
+# ---- voxel grid (VoxelGrid of the reference, modules/networks.py:382-575) -------------------------------
+NGP_VOXEL_MAX_GRID = 2048
+VOXEL_SH_DEGREES = (0, 1, 2)
+
+
+class CVoxelLayout(ctypes.Structure):
+    """ctypes mirror of ``ngp_voxel_layout`` (include/ngp_b200.h)."""
+
+    _fields_ = [
+        ("grid", ctypes.c_int32),
+        ("sh_degree", ctypes.c_int32),
+        ("radius", ctypes.c_float),
+        ("c_min", ctypes.c_float),
+    ]
+
+
+@dataclass
+class VoxelLayout:
+    grid: int
+    sh_degree: int
+    radius: float   # fp32 node spacing
+    c_min: float    # fp32 world coordinate of node 0 on every axis
+
+    @property
+    def sh_dim(self) -> int:
+        return (1 + self.sh_degree) ** 2
+
+    @property
+    def channels(self) -> int:
+        """sh channels per node (3 colours x sh_dim); the density is a field of its own."""
+        return 3 * self.sh_dim
+
+    def as_ctypes(self) -> CVoxelLayout:
+        return CVoxelLayout(self.grid, self.sh_degree, self.radius, self.c_min)
+
+
+def voxel_node_offset(grid: int) -> int:
+    """Lattice index of the node at the origin: node i sits at (i - ceil(G/2) + 1) * radius (networks.py:458-463)."""
+    return int(math.ceil(grid / 2)) - 1
+
+
+def make_voxel_layout(grid_size: int = 256, grid_radius: float = 0.0125, sh_degree: int = 2) -> VoxelLayout:
+    """Kernel constants of a VoxelGrid: c_min = (1 - ceil(G/2)) * radius (the minimum node coordinate,
+    networks.py:521-522), computed in f64 and rounded once to f32.  Supported: G in [1, 2048], sh_degree 0..2."""
+    G, deg = int(grid_size), int(sh_degree)
+    if G != grid_size or not 1 <= G <= NGP_VOXEL_MAX_GRID:
+        raise ValueError(f"grid_size must be an integer in [1, {NGP_VOXEL_MAX_GRID}], got {grid_size}")
+    if deg != sh_degree or deg not in VOXEL_SH_DEGREES:
+        raise ValueError(f"sh_degree must be 0, 1 or 2, got {sh_degree}")
+    if not (math.isfinite(grid_radius) and grid_radius > 0):
+        raise ValueError(f"grid_radius must be positive and finite, got {grid_radius}")
+    return VoxelLayout(grid=G, sh_degree=deg, radius=_f32(grid_radius),
+                       c_min=_f32(-voxel_node_offset(G) * float(grid_radius)))

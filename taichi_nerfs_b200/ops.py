@@ -159,6 +159,38 @@ def triplane_encode_bwd(xyz, table, dout, clayout, grad_table):
     return grad_table
 
 
+# ---- voxel grid (--model_name svox) ------------------------------------------------------------------
+VOXEL_BWD_WARP, VOXEL_BWD_THREAD = 0, 1     # NGP_VOXEL_BWD_* of include/ngp_b200.h
+
+
+def _voxel_inputs(xyz, *fields):
+    _need_cuda(xyz, *fields)
+    for t in (xyz,) + fields:
+        if t is not None and (t.dtype != torch.float32 or not t.is_contiguous()):
+            raise TypeError("voxel ops take contiguous fp32 tensors")
+
+
+def voxel_fwd(xyz, dirs, sh, density, clayout):
+    """World positions xyz [n,3], directions dirs [n,3] (normalised in the kernel), fields sh [G,G,G,3D] and density
+    [G,G,G,1] -> sigma [n], rgb [n,3], fp32.  dirs = None: density-only mode, returns sigma alone."""
+    _voxel_inputs(xyz, dirs, sh, density)
+    n = xyz.shape[0]
+    sigma = torch.empty(n, device=xyz.device, dtype=torch.float32)
+    rgb = None if dirs is None else torch.empty(n, 3, device=xyz.device, dtype=torch.float32)
+    check(load().ngp_voxel_fwd(_ptr(xyz), _ptr(dirs), _ptr(sh), _ptr(density), C.byref(clayout), _ptr(sigma),
+                               _ptr(rgb), n, _stream()), "voxel_fwd")
+    return sigma if dirs is None else (sigma, rgb)
+
+
+def voxel_bwd(xyz, dirs, sigma, rgb, dsigma, drgb, clayout, dsh, ddensity, found_inf=None, mapping=VOXEL_BWD_WARP):
+    """dsh (fp32, sh-field sized) += dL/dsh and ddensity (fp32, density-field sized) += dL/ddensity, from the forward's
+    outputs sigma / rgb and their gradients.  found_inf (int32 [1], optional) is raised on a non-finite gradient."""
+    _voxel_inputs(xyz, dirs, sigma, rgb, dsigma, drgb, dsh, ddensity)
+    check(load().ngp_voxel_bwd(_ptr(xyz), _ptr(dirs), _ptr(sigma), _ptr(rgb), _ptr(dsigma), _ptr(drgb),
+                               C.byref(clayout), _ptr(dsh), _ptr(ddensity), xyz.shape[0], _ptr(found_inf),
+                               int(mapping), _stream()), "voxel_bwd")
+
+
 # ---- a6 ------------------------------------------------------------------------------------------
 def dir_encode(dirs):
     _need_cuda(dirs)

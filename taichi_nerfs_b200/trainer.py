@@ -56,10 +56,11 @@ class NGPTrainer:
         # kernel that sums the owned 1/N of the gradient with peer loads, runs Adam on it and stores the new fp16 table
         # slice into every rank's shadow with peer stores (csrc/p2p.cu).  None when unavailable (NCCL fallback below).
         self.p2p = None
-        P_, enc_ = sizes[0], model.pos_encoder
-        if p2p_optimizer and hasattr(enc_, 'plane_embedding'):
-            raise ValueError("NGPTrainer: the peer-memory optimizer shards the fp16 hash table; a tri-plane model uses "
-                             "the all-reduce of the flat gradient (p2p_optimizer off)")
+        # a model without a position encoder (VoxelGrid) scatters into the .grad views of its own parameters
+        P_, enc_ = sizes[0], getattr(model, 'pos_encoder', None)
+        if p2p_optimizer and (enc_ is None or hasattr(enc_, 'plane_embedding')):
+            raise ValueError("NGPTrainer: the peer-memory optimizer shards the fp16 hash table; a tri-plane or "
+                             "voxel-grid model uses the all-reduce of the flat gradient (p2p_optimizer off)")
         if (p2p_optimizer is not False and self.world_size > 1 and dev.type == "cuda" and hasattr(enc_, "adopt_shadow")
                 and self.params[0] is enc_.hash_table and P_ % (4 * self.world_size) == 0):
             from .p2p import PeerRegion
@@ -79,9 +80,11 @@ class NGPTrainer:
                 self.flat_param[off:off + s].copy_(p.data.reshape(-1))
             p.data = self.flat_param[off:off + s].view_as(p)
             off += s + q
-            if (p is getattr(model.pos_encoder, 'hash_table', None)
-                    or p is getattr(model.pos_encoder, 'plane_embedding', None)):
-                model.pos_encoder.grad_sink = self.flat_grad[off - s - q:off - q]
+            if enc_ is not None and (p is getattr(enc_, 'hash_table', None)
+                                     or p is getattr(enc_, 'plane_embedding', None)):
+                enc_.grad_sink = self.flat_grad[off - s - q:off - q]
+        if enc_ is None:
+            model.grad_sink = (model.sh_fields.grad, model.density_fields.grad)
         self.found_inf = torch.zeros(1, device=dev, dtype=torch.int32)
         # device-side optimizer scalars (shared with StaticTrainStep): iteration counter, [lr/bc1, sqrt(bc2), 1/(scale*world),
         # Adam step count], GradScaler state [scale, growth tracker]
@@ -92,7 +95,7 @@ class NGPTrainer:
         self.scale_state = torch.tensor([self.loss_scale, 0.0], device=dev, dtype=torch.float32)
         self._views = [(p, p.data_ptr(), p.grad.data_ptr()) for p in self.params]
         self._shadow = self._shadow_full = None
-        enc = model.pos_encoder
+        enc = enc_
         if hasattr(enc, "adopt_shadow"):
             assert self.params[0] is enc.hash_table, "the hash table must be the first parameter"
             # fp16 copy of the whole flat buffer, rewritten by the Adam pass; the encoder reads its first slice
@@ -136,7 +139,7 @@ class NGPTrainer:
         for p in self.params:
             p.data = p.data.clone()
             p.grad = None
-        enc = self.model.pos_encoder
+        enc = getattr(self.model, 'pos_encoder', self.model)   # a VoxelGrid holds its grad_sink itself
         if hasattr(enc, 'grad_sink'):
             enc.grad_sink = None
         if self._shadow is not None and hasattr(enc, 'adopt_shadow'):

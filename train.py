@@ -29,6 +29,10 @@ warnings.filterwarnings("ignore")
 
 
 def build_model_config(hparams):
+    if getattr(hparams, 'model_name', 'ngp') == 'svox':   # VoxelGrid's keyword arguments (networks.py:383-393)
+        return {'scale': hparams.scale, 'half_opt': hparams.half_opt, 'sh_degree': hparams.sh_degree,
+                'grid_size': hparams.grid_size, 'grid_radius': hparams.grid_radius, 'origin_sh': hparams.origin_sh,
+                'origin_sigma': hparams.origin_sigma}
     if hparams.deployment:  # train.py:88-99
         return {'scale': hparams.scale, 'pos_encoder_type': 'hash', 'levels': 4, 'feature_per_level': 4,
                 'base_res': 32, 'max_res': 128, 'log2_T': 21, 'xyz_net_width': 16, 'rgb_net_width': 16,
