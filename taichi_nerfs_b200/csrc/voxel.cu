@@ -56,8 +56,19 @@ __device__ __forceinline__ float sh_basis(int k, const float d[3]) {
     }
 }
 
+// d / |d|.  A direction whose largest component lies outside [2^-40, 2^40] is first scaled by 2^90 or 2^-90, so that
+// its squares neither underflow (subnormal components: 0/0) nor overflow (components ~1e30: x/inf = 0).  The scaling is
+// exact unless a component more than 2^-50 times smaller than the largest underflows, which is below the fp32
+// resolution of d / |d|.  Every other direction takes the unscaled formula, bit for bit.  A zero direction stays 0/0 = NaN, as in the fp64 model.
 __device__ __forceinline__ void unit_dir(const float* dirs, int64_t i, float d[3]) {
-    const float a = dirs[i * 3], b = dirs[i * 3 + 1], c = dirs[i * 3 + 2];
+    float a = dirs[i * 3], b = dirs[i * 3 + 1], c = dirs[i * 3 + 2];
+    const float m = fmaxf(fabsf(a), fmaxf(fabsf(b), fabsf(c)));
+    if (m > 0x1p40f || (m < 0x1p-40f && m > 0.0f)) {
+        const float s = m > 0x1p40f ? 0x1p-90f : 0x1p90f;
+        a = f_mul(a, s);
+        b = f_mul(b, s);
+        c = f_mul(c, s);
+    }
     const float norm = sqrtf(f_add(f_add(f_mul(a, a), f_mul(b, b)), f_mul(c, c)));
     d[0] = f_div(a, norm);
     d[1] = f_div(b, norm);

@@ -71,13 +71,15 @@ def interpolate(xyz, field, radius, c_min):
     return (w[..., None] * gather(field, node)).sum(1)
 
 
-def _model(w, vals, dirs, deg):
+def _model(w, vals, dirs, deg, relu_mask=None):
     D = (deg + 1) ** 2
     feats = (w[..., None] * vals).sum(1)
     d = dirs.double()
     d = d / torch.norm(d, dim=1, keepdim=True)
     z = (feats[:, :3 * D].reshape(-1, 3, D) * sh_basis(deg, d)[:, None, :]).sum(-1)
-    return torch.relu(feats[:, -1]), torch.sigmoid(z)
+    if relu_mask is None:
+        return torch.relu(feats[:, -1]), torch.sigmoid(z)
+    return torch.where(relu_mask, feats[:, -1], torch.zeros_like(feats[:, -1])), torch.sigmoid(z)
 
 
 def default_c_min(G, radius):
@@ -110,14 +112,16 @@ def touched_nodes(node):
     return uniq, inv
 
 
-def grads(xyz, dirs, sh, density, radius, deg, dsigma, drgb, c_min=None):
+def grads(xyz, dirs, sh, density, radius, deg, dsigma, drgb, c_min=None, relu_mask=None):
     """dL/dsh and dL/ddensity in fp64 for L = sum(dsigma * sigma) + sum(drgb * rgb), on the nodes the batch touches:
-    -> (nodes [U], dsh [U, 3D], ddensity [U, 1]).  Every other node's gradient is zero."""
+    -> (nodes [U], dsh [U, 3D], ddensity [U, 1]).  Every other node's gradient is zero.  relu_mask (bool [N]), when
+    given, replaces the ReLU's own mask (interpolated density > 0): where the fp64 density is within the fp32 error of
+    zero, a kernel's backward is judged with the mask its own forward chose."""
     G = sh.shape[0]
     c_min = default_c_min(G, radius) if c_min is None else c_min
     node, w = corners(xyz, G, radius, c_min)
     vals = torch.cat([gather(sh, node), gather(density, node)], dim=-1).requires_grad_(True)
-    sigma, rgb = _model(w, vals, dirs, deg)
+    sigma, rgb = _model(w, vals, dirs, deg, relu_mask)
     ((sigma * dsigma.double()).sum() + (rgb * drgb.double()).sum()).backward()
     g = torch.where((node >= 0)[..., None], vals.grad, torch.zeros_like(vals.grad))
     idx = touched_nodes(node)
