@@ -236,6 +236,19 @@ int ngp_voxel_fwd_dyn(const float* xyz, const float* dirs, const float* sh, cons
 int ngp_voxel_bwd(const float* xyz, const float* dirs, const float* sigma, const float* rgb, const float* dsigma,
                   const float* drgb, const ngp_voxel_layout* layout, float* dsh, float* ddensity, int64_t n,
                   int32_t* found_inf_or_null, int mapping, void* stream);
+/* Regularisers of the voxel grid (DESIGN.md §6d) over the node block B = [lo, hi) per axis, block6 (HOST pointer) =
+ * {lo_x, lo_y, lo_z, hi_x, hi_y, hi_z}, 0 <= lo < hi <= G.  For a channel of node v in B, with forward differences
+ * Delta_a = V(v + e_a) - V(v) (0 when v + e_a lies outside B), s(v) = sqrt(Dx^2 + Dy^2 + Dz^2 + 1e-8):
+ *   L_tv_sigma = mean over B of s (density), L_tv_sh = mean over B x the 3D sh channels of s,
+ *   L_sparsity = mean over B of log(1 + 2 ReLU(density)^2).
+ * dsh / ddensity += scale * (w_tv_sigma dL_tv_sigma + w_tv_sh dL_tv_sh + w_sparsity dL_sparsity), scale =
+ * scale_dev[0] if scale_dev != NULL else loss_scale.  Each gradient float is computed and written by one thread (no
+ * atomics): the result is bit-reproducible.  A weight of 0 skips its term (its channels are not written); all three 0:
+ * no launch.  Weights must be finite and >= 0.  loss_or_null accumulates the unscaled weighted loss
+ * w_tv_sigma L_tv_sigma + w_tv_sh L_tv_sh + w_sparsity L_sparsity (caller zeroes it; fp32 atomic sum). */
+int ngp_voxel_reg(const float* sh, const float* density, const ngp_voxel_layout* layout, const int32_t* block6,
+                  float w_tv_sigma, float w_tv_sh, float w_sparsity, float loss_scale, const float* scale_dev,
+                  float* dsh, float* ddensity, float* loss_or_null, void* stream);
 
 /* ---- sync-free ("_dyn") variants used by the graph-captured training step -------------------
  * Same kernels as above, but the number of valid rows is read ON THE DEVICE: rows [0, min(n_max,*n_dev))

@@ -12,7 +12,7 @@ import torch
 from torch import nn
 
 from taichi_nerfs_b200 import ops
-from taichi_nerfs_b200.layout import make_voxel_layout, voxel_node_offset
+from taichi_nerfs_b200.layout import make_voxel_layout, voxel_node_offset, voxel_reg_block
 
 from .networks import MODEL_DICT, NGP, init_occupancy_grid
 from .volume_train import VolumeRenderer
@@ -65,6 +65,7 @@ class VoxelGrid(nn.Module):
         lay = make_voxel_layout(grid_size, grid_radius, sh_degree)   # ValueError on an unsupported degree / size
         self._layout = lay
         self._clayout = lay.as_ctypes()
+        self._reg_block = voxel_reg_block(lay, scale)   # the nodes the regularisers act on (NGPTrainer voxel_reg)
         self.half_opt = half_opt
         init_occupancy_grid(self, scale)
         self.sh_degree = lay.sh_degree

@@ -2,6 +2,7 @@
 flag table is restated here as data; `--dataset_name synthetic` and the torchrun-related behaviour are
 the only additions)."""
 import argparse
+import math
 
 # (flag, kwargs)
 _FLAGS = [
@@ -35,6 +36,12 @@ _FLAGS = [
                                                           '(svox only)')),
     # loss parameters
     ('--distortion_loss_w', dict(type=float, default=0, help='weight of distortion loss, 0 to disable (default)')),
+    ('--tv_sigma_loss_w', dict(type=float, default=0., help='weight of the total-variation loss on the voxel grid\'s '
+                                                           'density, 0 to disable (default; svox only)')),
+    ('--tv_sh_loss_w', dict(type=float, default=0., help='weight of the total-variation loss on the voxel grid\'s sh '
+                                                        'coefficients, 0 to disable (default; svox only)')),
+    ('--sparsity_loss_w', dict(type=float, default=0., help='weight of the Cauchy sparsity loss on the voxel grid\'s '
+                                                           'densities, 0 to disable (default; svox only)')),
     # training options
     ('--batch_size', dict(type=int, default=8192, help='number of rays in a batch')),
     ('--ray_sampling_strategy', dict(type=str, default='all_images', choices=['all_images', 'same_image'],
@@ -57,12 +64,20 @@ _FLAGS = [
     ('--deployment_model_path', dict(type=str, default='./')),
 ]
 
+_VOXEL_REG_FLAGS = ('tv_sigma_loss_w', 'tv_sh_loss_w', 'sparsity_loss_w')
+
 
 def get_opts(prefix_args=None):
     parser = argparse.ArgumentParser()
     for flag, kw in _FLAGS:
         parser.add_argument(flag, **kw)
     hparams = parser.parse_args(prefix_args)
+    for flag in _VOXEL_REG_FLAGS:
+        w = getattr(hparams, flag)
+        if not (math.isfinite(w) and w >= 0):
+            parser.error(f"--{flag} must be finite and >= 0, got {w}")
+        if w != 0 and hparams.model_name != 'svox':
+            parser.error(f"--{flag} regularises the voxel grid: it needs --model_name svox")
     if hparams.model_name == 'svox':
         for flag, bad, why in (
                 ('encoder_type', hparams.encoder_type == 'triplane',

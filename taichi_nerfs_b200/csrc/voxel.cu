@@ -1,5 +1,6 @@
 // voxel.cu — the voxel-grid model (`--model_name svox`): trilinear spherical-harmonics field, forward (full and
-// density-only, static and device-counted rows) and field backward.
+// density-only, static and device-counted rows), field backward and the gradient of the total-variation and sparsity
+// regularisers.
 //
 // Semantics (DESIGN.md §6d): the reference's VoxelGrid (modules/networks.py:382-575) with its missing parts decided
 // here.  Node (i,j,k) of the G^3 lattice sits at ((i,j,k) - ceil(G/2) + 1) * radius (networks.py:450-466); a world
@@ -267,6 +268,133 @@ __global__ void __launch_bounds__(kThreads) voxel_bwd_thread_kernel(
     if (bad && found_inf != nullptr) *found_inf = 1;
 }
 
+// ---- regularisers: total variation and density sparsity over the node block B (DESIGN.md §6d) ----------------------
+// Gather, not scatter: the thread of (node v, channel ch) computes the whole gradient of that element from v's own
+// term and the terms of its three backward neighbours v - e_a, so every gradient float is written by one thread with
+// a plain read-modify-write: no atomics, bit-reproducible.  Mapping: blockIdx.y = the x-slice of B; the (y, z) plane
+// of B times the C active channels is flattened, channel fastest, so C consecutive lanes own one node and a node's
+// neighbour read is one coalesced row (the lane-per-channel mapping of the kernels above).
+struct RegArgs {
+    const float* sh;
+    const float* density;
+    float* dsh;
+    float* ddensity;
+    const float* scale_dev;
+    float* loss;
+    float loss_scale;
+    float c_tv_sh;       // w_tv_sh / (|B| * 3D)
+    float c_tv_sigma;    // w_tv_sigma / |B|
+    float c_sparsity;    // w_sparsity / |B|
+    int32_t grid;
+    int32_t lo[3], hi[3];
+    int32_t ny, nz;      // B's extent along y and z
+};
+
+constexpr float kRegEps = 1e-8f;
+
+// sqrt(dx^2 + dy^2 + dz^2 + eps), in this order
+__device__ __forceinline__ float tv_norm(float dx, float dy, float dz) {
+    return sqrtf(f_add(f_add(f_add(f_mul(dx, dx), f_mul(dy, dy)), f_mul(dz, dz)), kRegEps));
+}
+
+template <int NSH, bool DEN>
+__global__ void __launch_bounds__(kThreads) voxel_reg_kernel(const RegArgs a) {
+    constexpr int C = NSH + (DEN ? 1 : 0);
+    __shared__ float part[kWarps];
+    const int e = blockIdx.x * kThreads + threadIdx.x;   // < ny * nz * C <= 2048^2 * 28
+    float loss = 0.0f;
+    if (e < a.ny * a.nz * C) {
+        const int yz = e / C, ch = e - yz * C;
+        const int i = a.lo[0] + (int)blockIdx.y, j = a.lo[1] + yz / a.nz, k = a.lo[2] + yz % a.nz;
+        const bool den = DEN && ch == NSH;
+        const float* f = den ? a.density : a.sh + ch;
+        float* dst = den ? a.ddensity : a.dsh + ch;
+        const int64_t stride = den ? 1 : NSH;   // floats per node
+        const int64_t G = a.grid, sx = G * G, sy = G;
+        const int64_t n0 = ((int64_t)i * G + j) * G + k;
+        const bool px = i + 1 < a.hi[0], py = j + 1 < a.hi[1], pz = k + 1 < a.hi[2];
+        const float v0 = __ldg(f + n0 * stride);
+        const float c_tv = den ? a.c_tv_sigma : a.c_tv_sh;
+        float g = 0.0f;
+        if (c_tv != 0.0f) {
+            // v's own term: d s(v) / d V(v) = -(dx + dy + dz) / s(v)
+            const float dx = px ? f_sub(__ldg(f + (n0 + sx) * stride), v0) : 0.0f;
+            const float dy = py ? f_sub(__ldg(f + (n0 + sy) * stride), v0) : 0.0f;
+            const float dz = pz ? f_sub(__ldg(f + (n0 + 1) * stride), v0) : 0.0f;
+            const float s = tv_norm(dx, dy, dz);
+            float t = -f_div(f_add(f_add(dx, dy), dz), s);
+            // backward neighbour w = v - e_a: d s(w) / d V(v) = Delta_a(w) / s(w); w's other two differences reach
+            // w + e_b, which lies in B exactly when v + e_b does
+            if (i > a.lo[0]) {
+                const int64_t w = n0 - sx;
+                const float b = __ldg(f + w * stride);
+                const float ex = f_sub(v0, b);
+                const float ey = py ? f_sub(__ldg(f + (w + sy) * stride), b) : 0.0f;
+                const float ez = pz ? f_sub(__ldg(f + (w + 1) * stride), b) : 0.0f;
+                t = f_add(t, f_div(ex, tv_norm(ex, ey, ez)));
+            }
+            if (j > a.lo[1]) {
+                const int64_t w = n0 - sy;
+                const float b = __ldg(f + w * stride);
+                const float ex = px ? f_sub(__ldg(f + (w + sx) * stride), b) : 0.0f;
+                const float ey = f_sub(v0, b);
+                const float ez = pz ? f_sub(__ldg(f + (w + 1) * stride), b) : 0.0f;
+                t = f_add(t, f_div(ey, tv_norm(ex, ey, ez)));
+            }
+            if (k > a.lo[2]) {
+                const int64_t w = n0 - 1;
+                const float b = __ldg(f + w * stride);
+                const float ex = px ? f_sub(__ldg(f + (w + sx) * stride), b) : 0.0f;
+                const float ey = py ? f_sub(__ldg(f + (w + sy) * stride), b) : 0.0f;
+                const float ez = f_sub(v0, b);
+                t = f_add(t, f_div(ez, tv_norm(ex, ey, ez)));
+            }
+            g = f_mul(c_tv, t);
+            loss = f_mul(c_tv, s);
+        }
+        if (den && a.c_sparsity != 0.0f) {
+            // log(1 + 2 r^2), r = ReLU(density); d/d density = 4 r / (1 + 2 r^2).  NaN stays NaN (not 0) so that the
+            // finite check downstream sees it.
+            const float r = v0 < 0.0f ? 0.0f : v0;
+            const float q = f_add(1.0f, f_mul(2.0f, f_mul(r, r)));
+            g = f_add(g, f_mul(a.c_sparsity, f_div(f_mul(4.0f, r), q)));
+            loss = f_add(loss, f_mul(a.c_sparsity, logf(q)));
+        }
+        const float scale = a.scale_dev != nullptr ? *a.scale_dev : a.loss_scale;
+        // a channel whose terms are all off is not written (DEN is false when both density weights are 0)
+        if (den ? (c_tv != 0.0f || a.c_sparsity != 0.0f) : c_tv != 0.0f)
+            dst[n0 * stride] = f_add(dst[n0 * stride], f_mul(scale, g));
+    }
+    if (a.loss == nullptr) return;   // uniform over the launch
+    loss = warp_sum(loss);
+    if ((threadIdx.x & 31) == 0) part[threadIdx.x >> 5] = loss;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        float sum = 0.0f;
+#pragma unroll
+        for (int w = 0; w < kWarps; ++w) sum += part[w];
+        atomicAdd(a.loss, sum);
+    }
+}
+
+template <int NSH, bool DEN>
+void launch_reg(const RegArgs& a, int nx, cudaStream_t st) {
+    constexpr int C = NSH + (DEN ? 1 : 0);
+    const int plane = a.ny * a.nz * C;
+    voxel_reg_kernel<NSH, DEN><<<dim3((unsigned)((plane + kThreads - 1) / kThreads), (unsigned)nx), kThreads, 0, st>>>(a);
+}
+
+template <int DEG>
+void launch_reg_deg(const RegArgs& a, int nx, bool sh, bool den, cudaStream_t st) {
+    constexpr int NSH = 3 * Lanes<DEG>::D;
+    if (sh && den)
+        launch_reg<NSH, true>(a, nx, st);
+    else if (sh)
+        launch_reg<NSH, false>(a, nx, st);
+    else
+        launch_reg<0, true>(a, nx, st);
+}
+
 int check_layout(const ngp_voxel_layout* lay) {
     NGP_REQUIRE(lay != nullptr, "null layout");
     NGP_REQUIRE(lay->grid >= 1 && lay->grid <= NGP_VOXEL_MAX_GRID, "grid must be in [1, 2048]");
@@ -359,6 +487,50 @@ int ngp_voxel_bwd(const float* xyz, const float* dirs, const float* sigma, const
             break;
     }
     NGP_LAUNCHED("voxel_bwd_kernel");
+    return 0;
+}
+
+int ngp_voxel_reg(const float* sh, const float* density, const ngp_voxel_layout* layout, const int32_t* block6,
+                  float w_tv_sigma, float w_tv_sh, float w_sparsity, float loss_scale, const float* scale_dev,
+                  float* dsh, float* ddensity, float* loss_or_null, void* stream) {
+    if (int rc = check_layout(layout)) return rc;
+    NGP_REQUIRE(block6 != nullptr, "null block");
+    for (int a = 0; a < 3; ++a)
+        NGP_REQUIRE(block6[a] >= 0 && block6[a] < block6[a + 3] && block6[a + 3] <= layout->grid,
+                    "block bounds must satisfy 0 <= lo < hi <= grid on every axis");
+    for (float w : {w_tv_sigma, w_tv_sh, w_sparsity})
+        NGP_REQUIRE(w >= 0.0f && w < INFINITY, "weights must be finite and >= 0");
+    NGP_REQUIRE(scale_dev != nullptr || fabsf(loss_scale) < INFINITY, "loss_scale must be finite");
+    const bool sh_on = w_tv_sh != 0.0f, den_on = w_tv_sigma != 0.0f || w_sparsity != 0.0f;
+    if (!sh_on && !den_on) return 0;
+    NGP_REQUIRE(sh && density && dsh && ddensity, "null pointer");
+    RegArgs a;
+    a.sh = sh;
+    a.density = density;
+    a.dsh = dsh;
+    a.ddensity = ddensity;
+    a.scale_dev = scale_dev;
+    a.loss = loss_or_null;
+    a.loss_scale = loss_scale;
+    a.grid = layout->grid;
+    for (int k = 0; k < 3; ++k) {
+        a.lo[k] = block6[k];
+        a.hi[k] = block6[k + 3];
+    }
+    const int nx = a.hi[0] - a.lo[0];
+    a.ny = a.hi[1] - a.lo[1];
+    a.nz = a.hi[2] - a.lo[2];
+    const double nodes = (double)nx * a.ny * a.nz, nsh = 3.0 * (layout->sh_degree + 1) * (layout->sh_degree + 1);
+    a.c_tv_sh = (float)(w_tv_sh / (nodes * nsh));
+    a.c_tv_sigma = (float)(w_tv_sigma / nodes);
+    a.c_sparsity = (float)(w_sparsity / nodes);
+    cudaStream_t st = ngp::as_stream(stream);
+    switch (layout->sh_degree) {
+        case 0: launch_reg_deg<0>(a, nx, sh_on, den_on, st); break;
+        case 1: launch_reg_deg<1>(a, nx, sh_on, den_on, st); break;
+        default: launch_reg_deg<2>(a, nx, sh_on, den_on, st); break;
+    }
+    NGP_LAUNCHED("voxel_reg_kernel");
     return 0;
 }
 

@@ -250,3 +250,16 @@ def make_voxel_layout(grid_size: int = 256, grid_radius: float = 0.0125, sh_degr
         raise ValueError(f"grid_radius must be positive and finite, got {grid_radius}")
     return VoxelLayout(grid=G, sh_degree=deg, radius=_f32(grid_radius),
                        c_min=_f32(-voxel_node_offset(G) * float(grid_radius)))
+
+
+def voxel_reg_block(lay: VoxelLayout, scale: float):
+    """The node block B the voxel regularisers act on (DESIGN.md §6d), as (lo_x, lo_y, lo_z, hi_x, hi_y, hi_z),
+    half-open: on every axis the nodes floor(u(-scale)) - 1 .. floor(u(scale)) + 2 clamped to [0, G-1], with
+    u(x) = (x - c_min) / radius in the kernels' fp32 arithmetic (sample_cell in csrc/voxel.cu).  The margin of one node
+    covers march positions an ulp outside the scene box; nodes outside B never feed a rendered sample."""
+    def u(x):
+        return float(np.float32(np.float32(np.float32(x) - np.float32(lay.c_min)) / np.float32(lay.radius)))
+
+    lo = min(max(math.floor(u(-scale)) - 1, 0), lay.grid - 1)
+    hi = min(max(math.floor(u(scale)) + 2, 0), lay.grid - 1)
+    return (lo,) * 3 + (hi + 1,) * 3

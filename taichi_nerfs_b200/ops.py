@@ -191,6 +191,20 @@ def voxel_bwd(xyz, dirs, sigma, rgb, dsigma, drgb, clayout, dsh, ddensity, found
                                int(mapping), _stream()), "voxel_bwd")
 
 
+def voxel_reg(sh, density, clayout, block, weights, dsh, ddensity, loss_scale=1.0, scale_dev=None, loss=None):
+    """Total-variation and sparsity regularisers over the node block ``block`` = (lo_x, lo_y, lo_z, hi_x, hi_y, hi_z)
+    (``layout.voxel_reg_block``): dsh += scale * dL/dsh and ddensity += scale * dL/ddensity for
+    L = w_tv_sigma L_tv_sigma + w_tv_sh L_tv_sh + w_sparsity L_sparsity, ``weights`` = (w_tv_sigma, w_tv_sh,
+    w_sparsity).  scale = scale_dev[0] (fp32 device tensor) when given, else loss_scale.  loss (fp32 [1], optional)
+    accumulates the unscaled L.  All three weights 0: nothing is launched."""
+    _voxel_inputs(sh, density, dsh, ddensity, scale_dev, loss)
+    w_tv_sigma, w_tv_sh, w_sparsity = (float(w) for w in weights)
+    b6 = (C.c_int32 * 6)(*[int(v) for v in block])
+    check(load().ngp_voxel_reg(_ptr(sh), _ptr(density), C.byref(clayout), b6, w_tv_sigma, w_tv_sh, w_sparsity,
+                               float(loss_scale), _ptr(scale_dev), _ptr(dsh), _ptr(ddensity), _ptr(loss), _stream()),
+          "voxel_reg")
+
+
 # ---- a6 ------------------------------------------------------------------------------------------
 def dir_encode(dirs):
     _need_cuda(dirs)

@@ -31,7 +31,19 @@ def _p(t):
 class NGPTrainer:
     def __init__(self, model, lr: float = 1e-2, max_steps: int = 20000, loss_scale: float | None = None,
                  betas=(0.9, 0.999), eps: float = 1e-15, process_group=None, dynamic_loss_scale: bool = True,
-                 p2p_optimizer: bool | None = None):
+                 p2p_optimizer: bool | None = None, voxel_reg=None):
+        # voxel_reg = (w_tv_sigma, w_tv_sh, w_sparsity): the voxel grid's regularisers (DESIGN.md §6d), enqueued after
+        # the render backward.  None or all zero: nothing is enqueued.
+        self.voxel_reg = None
+        if voxel_reg is not None:
+            if not (hasattr(model, 'sh_fields') and hasattr(model, 'density_fields')):
+                raise ValueError("NGPTrainer: voxel_reg (total variation / sparsity) applies to a model with voxel "
+                                 "fields (--model_name svox); this model has none")
+            w = tuple(float(v) for v in voxel_reg)
+            if len(w) != 3 or not all(math.isfinite(v) and v >= 0 for v in w):
+                raise ValueError(f"NGPTrainer: voxel_reg must be three finite weights >= 0 "
+                                 f"(w_tv_sigma, w_tv_sh, w_sparsity), got {voxel_reg}")
+            self.voxel_reg = w if any(w) else None
         self.model = model
         self.lr0 = lr
         self.max_steps = max_steps
@@ -156,7 +168,19 @@ class NGPTrainer:
         # GradScaler.scale(loss): the current scale is a device scalar, no host read
         scale = self.scale_state[0] if self.dynamic_loss_scale else self.loss_scale
         (loss * scale).backward()
+        if self.voxel_reg is not None:
+            self.add_voxel_reg()
         return loss, results
+
+    def add_voxel_reg(self, loss=None):
+        """Add loss_scale * the gradient of the voxel regularisers into the flat gradient (the model's grad_sink), from
+        the parameters the forward read; the scale is the device value when it is dynamic.  loss (fp32 [1], optional)
+        accumulates the unscaled weighted regulariser loss."""
+        m = self.model
+        dsh, dden = m.grad_sink
+        dyn = self.scale_state if self.dynamic_loss_scale else None
+        ops.voxel_reg(m.sh_fields.detach(), m.density_fields.detach(), m._clayout, m._reg_block, self.voxel_reg, dsh,
+                      dden, loss_scale=self.loss_scale, scale_dev=dyn, loss=loss)
 
     def enqueue_update(self, check_finite: bool = True):
         """Gradient exchange -> inf check -> LR / bias-correction scalars -> fused Adam (+fp16 shadow, grad zero) ->

@@ -87,7 +87,10 @@ def main(prefix_args=None):
     model.mark_invisible_cells(train_dataset.K, train_dataset.poses, train_dataset.img_wh)
 
     torch.manual_seed(seed + rank)  # data / marching noise differ per rank from here on
-    trainer = NGPTrainer(model, lr=hparams.lr, max_steps=hparams.max_steps)
+    voxel_reg = None
+    if hparams.model_name == 'svox':   # total variation / sparsity weights; all 0 (the default) enqueue nothing
+        voxel_reg = (hparams.tv_sigma_loss_w, hparams.tv_sh_loss_w, hparams.sparsity_loss_w)
+    trainer = NGPTrainer(model, lr=hparams.lr, max_steps=hparams.max_steps, voxel_reg=voxel_reg)
 
     fast = None
     if hparams.graph_step:
