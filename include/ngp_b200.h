@@ -236,6 +236,12 @@ int ngp_voxel_fwd_dyn(const float* xyz, const float* dirs, const float* sh, cons
 int ngp_voxel_bwd(const float* xyz, const float* dirs, const float* sigma, const float* rgb, const float* dsigma,
                   const float* drgb, const ngp_voxel_layout* layout, float* dsh, float* ddensity, int64_t n,
                   int32_t* found_inf_or_null, int mapping, void* stream);
+/* the warp-mapped backward with the row count read on the device: rows [0, min(n_max, max(*n_dev, 0))); rows beyond
+ * are not read.  n_dev == NULL: n_max rows, which is what ngp_voxel_bwd(..., NGP_VOXEL_BWD_WARP, ...) calls.
+ * found_inf_or_null as in ngp_voxel_bwd (graph-capturable: the launch arguments do not depend on the count). */
+int ngp_voxel_bwd_dyn(const float* xyz, const float* dirs, const float* sigma, const float* rgb, const float* dsigma,
+                      const float* drgb, const ngp_voxel_layout* layout, float* dsh, float* ddensity, int64_t n_max,
+                      const int32_t* n_dev, int32_t* found_inf_or_null, void* stream);
 /* Regularisers of the voxel grid (DESIGN.md §6d) over the node block B = [lo, hi) per axis, block6 (HOST pointer) =
  * {lo_x, lo_y, lo_z, hi_x, hi_y, hi_z}, 0 <= lo < hi <= G.  For a channel of node v in B, with forward differences
  * Delta_a = V(v + e_a) - V(v) (0 when v + e_a lies outside B), s(v) = sqrt(Dx^2 + Dy^2 + Dz^2 + 1e-8):
@@ -493,6 +499,17 @@ int ngp_adam_step(float* param, float* grad, float* exp_avg, float* exp_avg_sq,
                   int32_t step, int zero_grad, int64_t n, void* stream);
 /* sets *found_inf = 1 if any element of grad is non-finite (GradScaler check) */
 int ngp_check_finite(const float* grad, int64_t n, int32_t* found_inf, void* stream);
+/* The finite check and the Adam pass of ngp_check_finite / ngp_adam_step_dyn restricted to the node block B of one
+ * voxel field (DESIGN.md §6b): the field is [G, G, G, C] fp32 (sh: C = 3 * sh_dim, density: C = 1), block6 (HOST
+ * pointer) = {lo_x, lo_y, lo_z, hi_x, hi_y, hi_z} as in ngp_voxel_reg, 0 <= lo < hi <= G.  Every (x, y) of B is one
+ * contiguous run of (hi_z - lo_z) * C floats; no alignment is required.  Elements outside B are neither read nor
+ * written.  The Adam entry: hyper_dev as ngp_adam_step_dyn, nothing but the gradient changes when *found_inf != 0,
+ * the gradient inside B is zeroed on every call, no fp16 shadow.  Inside B the arithmetic is ngp_adam_step_dyn's. */
+int ngp_check_finite_voxel_block(const float* grad, int32_t grid, int32_t channels, const int32_t* block6,
+                                 int32_t* found_inf, void* stream);
+int ngp_adam_step_voxel_block_dyn(float* param, float* grad, float* exp_avg, float* exp_avg_sq, int32_t grid,
+                                  int32_t channels, const int32_t* block6, const int32_t* found_inf_or_null,
+                                  const float* hyper_dev, float beta1, float beta2, float eps, void* stream);
 /* Multi-GPU gradient transport in fp16 (what the reference's autocast backward produces for its parameters; the
  * loss scale keeps the values in range and a value that does not fit becomes inf, i.e. a skipped step + scale backoff
  * exactly as with GradScaler): pack the fp32 accumulation buffer, all-reduce the fp16 buffer (half the bytes), check

@@ -58,6 +58,7 @@ def _declare(lib):
         "ngp_voxel_fwd": (ci, [vp, vp, vp, vp, vox, vp, vp, i64, vp]),
         "ngp_voxel_fwd_dyn": (ci, [vp, vp, vp, vp, vox, vp, vp, i64, vp, vp]),
         "ngp_voxel_bwd": (ci, [vp, vp, vp, vp, vp, vp, vox, vp, vp, i64, vp, ci, vp]),
+        "ngp_voxel_bwd_dyn": (ci, [vp, vp, vp, vp, vp, vp, vox, vp, vp, i64, vp, vp, vp]),
         "ngp_voxel_reg": (ci, [vp, vp, vox, vp, f32, f32, f32, f32, vp, vp, vp, vp, vp]),
         "ngp_mlp_fwd_dyn": (ci, [vp, ci, vp, mw, vp, vp, vp, i64, vp, vp]),
         "ngp_mlp_bwd_dyn": (ci, [vp, ci, vp, mw, vp, vp, vp, vp, vp, i64, vp, vp, vp]),
@@ -87,6 +88,8 @@ def _declare(lib):
         "ngp_morton3d_invert": (ci, [vp, vp, i64, vp]),
         "ngp_adam_step": (ci, [vp, vp, vp, vp, vp, vp, f32, f32, f32, f32, f32, i32, ci, i64, vp]),
         "ngp_check_finite": (ci, [vp, i64, vp, vp]),
+        "ngp_check_finite_voxel_block": (ci, [vp, i32, i32, vp, vp, vp]),
+        "ngp_adam_step_voxel_block_dyn": (ci, [vp, vp, vp, vp, i32, i32, vp, vp, vp, f32, f32, f32, vp]),
         "ngp_grad_pack_f16": (ci, [vp, vp, i64, vp]),
         "ngp_check_finite_f16": (ci, [vp, i64, vp, vp]),
         "ngp_adam_step_dyn_g16": (ci, [vp, vp, vp, vp, vp, vp, vp, vp, f32, f32, f32, i64, vp]),

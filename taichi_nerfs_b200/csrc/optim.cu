@@ -196,6 +196,78 @@ __global__ void __launch_bounds__(256) check_finite_kernel(const float* __restri
     if (__any_sync(0xffffffffu, bad) && (threadIdx.x & 31) == 0) atomicExch(found_inf, 1);
 }
 
+// ---- the node block B of a voxel field (DESIGN.md §6b) ------------------------------------------------------------
+// A field [G, G, G, C] restricted to B = [lo, hi) per axis is nx * ny runs, one per (x, y), of nz * C contiguous
+// floats.  One CTA walks one run at a time with scalar, coalesced accesses (a run starts at any float); the CTAs
+// stride over the runs.  Offsets are int64: a degree-2 field passes 2^31 floats at G >= 431.
+struct BlockRuns {
+    int64_t G, C;
+    int32_t lo_x, lo_y, lo_z, ny;
+    int64_t runs, run_len;
+};
+
+__device__ __forceinline__ int64_t run_base(const BlockRuns& b, int64_t r) {
+    const int64_t i = b.lo_x + r / b.ny, j = b.lo_y + r % b.ny;
+    return ((i * b.G + j) * b.G + b.lo_z) * b.C;
+}
+
+__global__ void __launch_bounds__(256) adam_block_kernel(float* __restrict__ param, float* __restrict__ grad,
+                                                         float* __restrict__ exp_avg, float* __restrict__ exp_avg_sq,
+                                                         const int32_t* __restrict__ found_inf,
+                                                         const float* __restrict__ hyper_dev, AdamArgs a,
+                                                         const BlockRuns b) {
+    const bool skip = found_inf != nullptr && *found_inf != 0;
+    a.lr_over_bc1 = hyper_dev[0];
+    a.bc2_sqrt = hyper_dev[1];
+    a.inv_scale = hyper_dev[2];
+    for (int64_t r = blockIdx.x; r < b.runs; r += gridDim.x) {
+        const int64_t base = run_base(b, r);
+        for (int64_t e = threadIdx.x; e < b.run_len; e += blockDim.x) {
+            const int64_t k = base + e;
+            if (!skip) {
+                float p = param[k], g = grad[k], m = exp_avg[k], v = exp_avg_sq[k];
+                adam1(p, g, m, v, a);
+                param[k] = p;
+                exp_avg[k] = m;
+                exp_avg_sq[k] = v;
+            }
+            grad[k] = 0.0f;
+        }
+    }
+}
+
+__global__ void __launch_bounds__(256) check_finite_block_kernel(const float* __restrict__ grad, const BlockRuns b,
+                                                                 int32_t* __restrict__ found_inf) {
+    bool bad = false;
+    for (int64_t r = blockIdx.x; r < b.runs; r += gridDim.x) {
+        const int64_t base = run_base(b, r);
+        for (int64_t e = threadIdx.x; e < b.run_len; e += blockDim.x) bad |= !(fabsf(grad[base + e]) < INFINITY);
+    }
+    if (__any_sync(0xffffffffu, bad) && (threadIdx.x & 31) == 0) atomicExch(found_inf, 1);
+}
+
+int block_runs(int32_t grid, int32_t channels, const int32_t* block6, BlockRuns& b) {
+    NGP_REQUIRE(grid >= 1, "grid must be >= 1");
+    NGP_REQUIRE(channels >= 1, "channels must be >= 1");
+    NGP_REQUIRE(block6 != nullptr, "null block");
+    for (int k = 0; k < 3; ++k)
+        NGP_REQUIRE(block6[k] >= 0 && block6[k] < block6[k + 3] && block6[k + 3] <= grid,
+                    "block bounds must satisfy 0 <= lo < hi <= grid on every axis");
+    b.G = grid;
+    b.C = channels;
+    b.lo_x = block6[0];
+    b.lo_y = block6[1];
+    b.lo_z = block6[2];
+    b.ny = block6[4] - block6[1];
+    b.runs = (int64_t)(block6[3] - block6[0]) * b.ny;
+    b.run_len = (int64_t)(block6[5] - block6[2]) * channels;
+    return 0;
+}
+
+unsigned block_grid(const BlockRuns& b) {   // one run per CTA (B has at most 2048^2 runs)
+    return (unsigned)min(b.runs, (int64_t)INT32_MAX);
+}
+
 }  // namespace
 
 extern "C" {
@@ -347,6 +419,36 @@ int ngp_check_finite(const float* grad, int64_t n, int32_t* found_inf, void* str
     const unsigned grid = (unsigned)min((work + 255) / 256, max_blocks);
     check_finite_kernel<<<grid, 256, 0, ngp::as_stream(stream)>>>(grad, n, found_inf);
     NGP_LAUNCHED("check_finite_kernel");
+    return 0;
+}
+
+int ngp_check_finite_voxel_block(const float* grad, int32_t grid, int32_t channels, const int32_t* block6,
+                                 int32_t* found_inf, void* stream) {
+    BlockRuns b;
+    if (int rc = block_runs(grid, channels, block6, b)) return rc;
+    NGP_REQUIRE(grad && found_inf, "null pointer");
+    check_finite_block_kernel<<<block_grid(b), 256, 0, ngp::as_stream(stream)>>>(grad, b, found_inf);
+    NGP_LAUNCHED("check_finite_block_kernel");
+    return 0;
+}
+
+int ngp_adam_step_voxel_block_dyn(float* param, float* grad, float* exp_avg, float* exp_avg_sq, int32_t grid,
+                                  int32_t channels, const int32_t* block6, const int32_t* found_inf_or_null,
+                                  const float* hyper_dev, float beta1, float beta2, float eps, void* stream) {
+    BlockRuns b;
+    if (int rc = block_runs(grid, channels, block6, b)) return rc;
+    NGP_REQUIRE(param && grad && exp_avg && exp_avg_sq && hyper_dev, "null pointer");
+    AdamArgs a;
+    a.lr_over_bc1 = 0.f;
+    a.bc2_sqrt = 1.f;
+    a.inv_scale = 1.f;
+    a.beta1 = beta1;
+    a.beta2 = beta2;
+    a.eps = eps;
+    a.zero_grad = 1;
+    adam_block_kernel<<<block_grid(b), 256, 0, ngp::as_stream(stream)>>>(param, grad, exp_avg, exp_avg_sq,
+                                                                         found_inf_or_null, hyper_dev, a, b);
+    NGP_LAUNCHED("adam_block_kernel");
     return 0;
 }
 

@@ -466,9 +466,12 @@ int ngp_voxel_fwd_dyn(const float* xyz, const float* dirs, const float* sh, cons
 int ngp_voxel_bwd(const float* xyz, const float* dirs, const float* sigma, const float* rgb, const float* dsigma,
                   const float* drgb, const ngp_voxel_layout* layout, float* dsh, float* ddensity, int64_t n,
                   int32_t* found_inf_or_null, int mapping, void* stream) {
+    NGP_REQUIRE(mapping == NGP_VOXEL_BWD_WARP || mapping == NGP_VOXEL_BWD_THREAD, "unknown mapping");
+    if (mapping == NGP_VOXEL_BWD_WARP)   // the NULL call of the device-counted entry: one warp-mapped backward
+        return ngp_voxel_bwd_dyn(xyz, dirs, sigma, rgb, dsigma, drgb, layout, dsh, ddensity, n, nullptr,
+                                 found_inf_or_null, stream);
     if (int rc = check_layout(layout)) return rc;
     NGP_REQUIRE(n >= 0, "negative n");
-    NGP_REQUIRE(mapping == NGP_VOXEL_BWD_WARP || mapping == NGP_VOXEL_BWD_THREAD, "unknown mapping");
     if (n == 0) return 0;
     NGP_REQUIRE(xyz && dirs && sigma && rgb && dsigma && drgb && dsh && ddensity, "null pointer");
     cudaStream_t st = ngp::as_stream(stream);
@@ -483,6 +486,33 @@ int ngp_voxel_bwd(const float* xyz, const float* dirs, const float* sigma, const
             break;
         default:
             launch_bwd<2>(mapping, xyz, dirs, sigma, rgb, dsigma, drgb, *layout, dsh, ddensity, n, nullptr,
+                          found_inf_or_null, st);
+            break;
+    }
+    NGP_LAUNCHED("voxel_bwd_kernel");
+    return 0;
+}
+
+int ngp_voxel_bwd_dyn(const float* xyz, const float* dirs, const float* sigma, const float* rgb, const float* dsigma,
+                      const float* drgb, const ngp_voxel_layout* layout, float* dsh, float* ddensity, int64_t n_max,
+                      const int32_t* n_dev, int32_t* found_inf_or_null, void* stream) {
+    if (int rc = check_layout(layout)) return rc;
+    NGP_REQUIRE(n_max >= 0, "negative n");
+    if (n_max == 0) return 0;
+    NGP_REQUIRE(xyz && dirs && sigma && rgb && dsigma && drgb && dsh && ddensity, "null pointer");
+    cudaStream_t st = ngp::as_stream(stream);
+    const int w = NGP_VOXEL_BWD_WARP;
+    switch (layout->sh_degree) {
+        case 0:
+            launch_bwd<0>(w, xyz, dirs, sigma, rgb, dsigma, drgb, *layout, dsh, ddensity, n_max, n_dev,
+                          found_inf_or_null, st);
+            break;
+        case 1:
+            launch_bwd<1>(w, xyz, dirs, sigma, rgb, dsigma, drgb, *layout, dsh, ddensity, n_max, n_dev,
+                          found_inf_or_null, st);
+            break;
+        default:
+            launch_bwd<2>(w, xyz, dirs, sigma, rgb, dsigma, drgb, *layout, dsh, ddensity, n_max, n_dev,
                           found_inf_or_null, st);
             break;
     }

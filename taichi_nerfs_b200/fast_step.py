@@ -8,6 +8,9 @@ the C-ABI kernels, enqueued in a fixed order on fixed buffers:
   [+ distortion loss] + composite bwd) -> MLP bwd -> hash (or tri-plane) bwd -> [gradient exchange] -> check_finite -> device-side LR/bias-correction update
   -> fused Adam (+fp16 shadow, grad zero) -> device-side GradScaler update
 
+A voxel-grid model (--model_name svox) has no network: the march feeds the voxel forward (fp32 sigma / rgb) -> head ->
+voxel backward -> [regularisers] -> finite check and Adam over the fields' node block B only (DESIGN.md §6b).
+
 What makes it graph-capturable: the number of samples S stays on the device (kernels read it from the
 march counter; buffers are sized for `capacity` rows and rays that would overflow are dropped and
 counted), and the per-step optimizer scalars live in device memory.  The reference synchronises the
@@ -34,12 +37,18 @@ class StaticTrainStep:
                  dynamic_loss_scale: bool = True, overlap_optimizer: bool = False, distortion_loss_w: float = 0.0):
         self.tr = trainer
         m = self.model = trainer.model
-        enc = m.pos_encoder
-        if not m._fusable(next(m.parameters())):
+        # the voxel-grid model: fp32 fields and outputs, no encoder and no MLP; its optimizer pass covers the node
+        # block B only (DESIGN.md §6b)
+        self.vox = hasattr(m, "sh_fields") and hasattr(m, "density_fields")
+        enc = getattr(m, "pos_encoder", None)
+        self.tri = hasattr(enc, "plane_embedding")
+        if self.vox:
+            if trainer.world_size > 1:
+                raise _lib.NgpError("StaticTrainStep runs a voxel-grid model on one rank only")
+        elif not m._fusable(next(m.parameters())):
             raise _lib.NgpError("StaticTrainStep needs the stock NGP architecture (fused MLP)")
         # the tri-plane model: fp32 planes and embedding, no fp16 shadow; the encode launches go through the encoder
-        self.tri = hasattr(enc, "plane_embedding")
-        if not self.tri and not hasattr(enc, "hash_table"):
+        elif not self.tri and not hasattr(enc, "hash_table"):
             raise _lib.NgpError("StaticTrainStep runs the hash or the tri-plane encoder's kernels")
         dev = next(m.parameters()).device
         self.dev, self.n = dev, int(n_rays)
@@ -58,11 +67,15 @@ class StaticTrainStep:
         # marching
         self.hits, self.counter, self.rays_a = z(self.n, 2), z(2, dtype=i32), z(self.n, 3, dtype=i32)
         self.xyzs, self.dirs, self.deltas, self.ts = z(C_, 3), z(C_, 3), z(C_), z(C_)
-        # network
-        self.emb, self.demb = z(C_, 32, dtype=edt), z(C_, 32, dtype=edt)
+        # network (the voxel grid: sigma and fp32 rgb straight from the fields, no embedding)
         self.sig, self.dsig = z(C_), z(C_)
-        self.rgbs, self.drgbs = z(C_, 3, dtype=torch.float16), z(C_, 3, dtype=torch.float16)
-        self.mlp_save = z(int(load().ngp_mlp_save_bytes(C_)), dtype=torch.uint8)   # h + fp16 rgb kept for the backward
+        if self.vox:
+            self.emb = self.demb = self.mlp_save = None
+            self.rgbs, self.drgbs = z(C_, 3), z(C_, 3)
+        else:
+            self.emb, self.demb = z(C_, 32, dtype=edt), z(C_, 32, dtype=edt)
+            self.rgbs, self.drgbs = z(C_, 3, dtype=torch.float16), z(C_, 3, dtype=torch.float16)
+            self.mlp_save = z(int(load().ngp_mlp_save_bytes(C_)), dtype=torch.uint8)   # h + fp16 rgb for the backward
         # compositing / loss
         self.total, self.opacity, self.depth, self.rgb = z(self.n, dtype=i32), z(self.n), z(self.n), z(self.n, 3)
         self.ws = z(C_)
@@ -75,13 +88,22 @@ class StaticTrainStep:
         trainer.dynamic_loss_scale = self.dynamic_loss_scale = bool(dynamic_loss_scale)
         self.aabb6 = (C.c_float * 6)(*[float(v) for v in m.xyz_min.flatten().tolist()],
                                      *[float(v) for v in (m.xyz_max - m.xyz_min).flatten().tolist()])
-        self._clayout = enc._clayout
-        self._w_keep = [w.detach() for w in mlp_weights(m)]
-        self._wst = _lib.MlpWeights(*[w.data_ptr() for w in self._w_keep])
-        self.P = enc.total_param_size
-        assert trainer.slices[0] == (0, self.P), "the encoder's table must be the first parameter"
-        offs = [o for o, _ in trainer.slices[1:]]
-        assert offs == [self.P, self.P + 2048, self.P + 3072, self.P + 5120, self.P + 9216], offs
+        if self.vox:
+            # B: the nodes the step's samples (inside the scene box, with one node of margin) and the regularisers
+            # reach.  The step's optimizer checks and updates B only; see DESIGN.md §6b for mixed use with the module
+            # path.
+            self._clayout = m._clayout
+            self.block = tuple(int(v) for v in m._reg_block)
+            self.P = m.sh_fields.numel()
+            assert trainer.slices[0] == (0, self.P) and trainer.slices[1][1] == m.density_fields.numel()
+        else:
+            self._clayout = enc._clayout
+            self._w_keep = [w.detach() for w in mlp_weights(m)]
+            self._wst = _lib.MlpWeights(*[w.data_ptr() for w in self._w_keep])
+            self.P = enc.total_param_size
+            assert trainer.slices[0] == (0, self.P), "the encoder's table must be the first parameter"
+            offs = [o for o, _ in trainer.slices[1:]]
+            assert offs == [self.P, self.P + 2048, self.P + 3072, self.P + 5120, self.P + 9216], offs
         # valid placeholder rays (an all-zero direction would march forever, in the reference too)
         self.rays_o[:] = torch.tensor([1.2, 0.3, 0.5], device=dev)
         jitter = (torch.arange(self.n, device=dev, dtype=f32)[:, None] % 97) * 1e-3
@@ -101,9 +123,10 @@ class StaticTrainStep:
         # one rank or the peer-memory step + dynamic loss scale: the backward kernels raise GradScaler's inf flag
         # themselves (a non-finite contribution is seen where it is scattered), the optimizer consumes and clears it -
         # no 45 MB check pass (the NCCL fallback checks the reduced fp16 sum instead)
-        # (the hash backward raises it in its F = 2 instantiation only, the tri-plane backward in both)
+        # (the hash backward raises it in its F = 2 instantiation only, the tri-plane backward in both).  The voxel
+        # grid: the regularisers' gradient is not seen by any backward, so the finite check over B covers them all.
         self.inf_at_source = bool((trainer.world_size == 1 or trainer.p2p is not None) and self.dynamic_loss_scale
-                                  and (self.tri or enc._clayout.feat_dim == 2))
+                                  and not self.vox and (self.tri or enc._clayout.feat_dim == 2))
         if self.inf_at_source:
             trainer.found_inf.zero_()
         self.use_graph = bool(use_graph)
@@ -179,14 +202,15 @@ class StaticTrainStep:
     def _k_head(self):
         # composite forward + background + MSE [+ distortion loss] + composite backward in one launch (per-ray work)
         bg = 1.0 if self.esf == 0 else 0.0
+        ctag = F32 if self.vox else F16
         if self.distortion_w > 0:
             check(load().ngp_ray_head_fused_distortion(
-                _p(self.sig), _p(self.rgbs), F16, _p(self.deltas), _p(self.ts), _p(self.rays_a), _p(self.gt), bg,
+                _p(self.sig), _p(self.rgbs), ctag, _p(self.deltas), _p(self.ts), _p(self.rays_a), _p(self.gt), bg,
                 float(self.tr.loss_scale), _p(self.scale_state) if self.dynamic_loss_scale else None, self.T_thr,
                 self.distortion_w, _p(self.loss_sum), _p(self.opacity), _p(self.rgb), _p(self.dsig), _p(self.drgbs),
                 self.n, self._st()))
             return
-        check(load().ngp_ray_head_fused(_p(self.sig), _p(self.rgbs), F16, _p(self.deltas), _p(self.rays_a), _p(self.gt),
+        check(load().ngp_ray_head_fused(_p(self.sig), _p(self.rgbs), ctag, _p(self.deltas), _p(self.rays_a), _p(self.gt),
                                         bg, float(self.tr.loss_scale),
                                         _p(self.scale_state) if self.dynamic_loss_scale else None, self.T_thr,
                                         _p(self.loss_sum), _p(self.opacity), _p(self.rgb), _p(self.dsig),
@@ -215,8 +239,28 @@ class StaticTrainStep:
                                            int(level_begin), int(level_end),
                                            _p(self.tr.found_inf) if self.inf_at_source else None, st))
 
+    # the voxel grid's stages: fields -> fp32 sigma / rgb, and the field gradient into the trainer's flat buffer
+    def _k_voxel_fwd(self):
+        m = self.model
+        check(load().ngp_voxel_fwd_dyn(_p(self.xyzs), _p(self.dirs), _p(m.sh_fields), _p(m.density_fields),
+                                       C.byref(self._clayout), _p(self.sig), _p(self.rgbs), self.cap, _p(self.counter),
+                                       self._st()))
+
+    def _k_voxel_bwd(self):
+        dsh, dden = self.model.grad_sink
+        check(load().ngp_voxel_bwd_dyn(_p(self.xyzs), _p(self.dirs), _p(self.sig), _p(self.rgbs), _p(self.dsig),
+                                       _p(self.drgbs), C.byref(self._clayout), _p(dsh), _p(dden), self.cap,
+                                       _p(self.counter), None, self._st()))
+
     def _enqueue_network(self):
         # counter[0] = number of valid sample rows, read on the device by every kernel
+        if self.vox:
+            self._k_voxel_fwd()
+            self._k_head()
+            self._k_voxel_bwd()
+            if self.tr.voxel_reg is not None:   # TV / sparsity over B, scaled by the device loss scale
+                self.tr.add_voxel_reg()
+            return
         self._k_hash_fwd()
         self._k_mlp_fwd()
         self._k_head()
@@ -233,7 +277,7 @@ class StaticTrainStep:
 
     def _enqueue_update(self):
         # [gradient exchange] -> check_finite -> LR/bias scalars -> fused Adam -> GradScaler.update
-        self.tr.enqueue_update(check_finite=not self.inf_at_source)
+        self.tr.enqueue_update(check_finite=not self.inf_at_source, voxel_block=self.block if self.vox else None)
 
     def _enqueue(self, sampled=False, mode="sync"):
         if sampled:
@@ -326,15 +370,14 @@ class StaticTrainStep:
                 self.tr.found_inf.zero_()
             self._enqueue_update()
             self.pending = False
-            if self.tr._shadow is not None:
+            if self.tr._shadow is not None:   # (a voxel grid has neither a shadow nor a pos_encoder)
                 self.model.pos_encoder.adopt_shadow(self.tr._shadow)
         self.tr.sync_master()   # peer-memory step: the fp32 master table is complete again on every rank
 
     def _finish_step(self):
         self.tr.step_count += 1
-        enc = self.model.pos_encoder
         if self.tr._shadow is not None:
-            enc.adopt_shadow(self.tr._shadow)
+            self.model.pos_encoder.adopt_shadow(self.tr._shadow)
         return self.loss_sum / (3.0 * self.n)
 
     def attach_ray_source(self, image_bank, poses, directions, seed: int = 0, fixed_img: int = -1):

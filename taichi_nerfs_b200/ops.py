@@ -191,6 +191,15 @@ def voxel_bwd(xyz, dirs, sigma, rgb, dsigma, drgb, clayout, dsh, ddensity, found
                                int(mapping), _stream()), "voxel_bwd")
 
 
+def voxel_bwd_dyn(xyz, dirs, sigma, rgb, dsigma, drgb, clayout, dsh, ddensity, n_dev=None, found_inf=None):
+    """voxel_bwd (warp mapping) over rows [0, min(n, max(n_dev[0], 0))) with the count n_dev (int32 [1]) read on the
+    device; n_dev None: all n rows."""
+    _voxel_inputs(xyz, dirs, sigma, rgb, dsigma, drgb, dsh, ddensity)
+    check(load().ngp_voxel_bwd_dyn(_ptr(xyz), _ptr(dirs), _ptr(sigma), _ptr(rgb), _ptr(dsigma), _ptr(drgb),
+                                   C.byref(clayout), _ptr(dsh), _ptr(ddensity), xyz.shape[0], _ptr(n_dev),
+                                   _ptr(found_inf), _stream()), "voxel_bwd_dyn")
+
+
 def voxel_reg(sh, density, clayout, block, weights, dsh, ddensity, loss_scale=1.0, scale_dev=None, loss=None):
     """Total-variation and sparsity regularisers over the node block ``block`` = (lo_x, lo_y, lo_z, hi_x, hi_y, hi_z)
     (``layout.voxel_reg_block``): dsh += scale * dL/dsh and ddensity += scale * dL/ddensity for
@@ -374,6 +383,40 @@ def adam_step(param, grad, exp_avg, exp_avg_sq, lr, step, beta1=0.9, beta2=0.999
 def check_finite(grad, found_inf):
     _need_cuda(grad, found_inf)
     check(load().ngp_check_finite(_ptr(grad), grad.numel(), _ptr(found_inf), _stream()), "check_finite")
+
+
+def _voxel_block(block, field, *others):
+    """(G, C, host block6) of a voxel field [G, G, G, C] and its node block B.  The kernels derive every offset from G
+    and C, so anything but a 4-D cube (and companions of the same shape) is refused."""
+    if field.dim() != 4 or not field.shape[0] == field.shape[1] == field.shape[2]:
+        raise ValueError(f"a voxel field is [G, G, G, C], got {tuple(field.shape)}")
+    for t in others:
+        if t.shape != field.shape:
+            raise ValueError(f"voxel buffers differ in shape: {tuple(t.shape)} vs {tuple(field.shape)}")
+    G, C_ = int(field.shape[0]), int(field.shape[-1])
+    return G, C_, (C.c_int32 * 6)(*[int(v) for v in block])
+
+
+def check_finite_voxel_block(grad, block, found_inf):
+    """found_inf[0] = 1 when an element of the voxel-field gradient grad [G,G,G,C] inside the node block ``block`` =
+    (lo_x, lo_y, lo_z, hi_x, hi_y, hi_z) is not finite (``layout.voxel_reg_block``)."""
+    _voxel_inputs(grad)
+    _need_cuda(found_inf)
+    G, C_, b6 = _voxel_block(block, grad)
+    check(load().ngp_check_finite_voxel_block(_ptr(grad), G, C_, b6, _ptr(found_inf), _stream()),
+          "check_finite_voxel_block")
+
+
+def adam_step_voxel_block(param, grad, exp_avg, exp_avg_sq, block, hyper, found_inf=None, beta1=0.9, beta2=0.999,
+                          eps=1e-15):
+    """ngp_adam_step_dyn (device scalars ``hyper``, zero_grad) over the elements of a voxel field [G,G,G,C] inside the
+    node block ``block``; everything outside it is left alone."""
+    _voxel_inputs(param, grad, exp_avg, exp_avg_sq, hyper)
+    _need_cuda(found_inf)
+    G, C_, b6 = _voxel_block(block, param, grad, exp_avg, exp_avg_sq)
+    check(load().ngp_adam_step_voxel_block_dyn(_ptr(param), _ptr(grad), _ptr(exp_avg), _ptr(exp_avg_sq), G, C_, b6,
+                                               _ptr(found_inf), _ptr(hyper), float(beta1), float(beta2), float(eps),
+                                               _stream()), "adam_step_voxel_block")
 
 
 # ---- a7 ------------------------------------------------------------------------------------------

@@ -182,7 +182,16 @@ class NGPTrainer:
         ops.voxel_reg(m.sh_fields.detach(), m.density_fields.detach(), m._clayout, m._reg_block, self.voxel_reg, dsh,
                       dden, loss_scale=self.loss_scale, scale_dev=dyn, loss=loss)
 
-    def enqueue_update(self, check_finite: bool = True):
+    def voxel_fields(self):
+        """(param, grad, exp_avg, exp_avg_sq) views [G, G, G, C] of the sh field and of the density field in the flat
+        buffers, for the node-block optimizer pass (enqueue_update(voxel_block=...))."""
+        out = []
+        for p, (off, n) in zip(self.params, self.slices):
+            out.append(tuple(t[off:off + n].view(p.shape) for t in (self.flat_param, self.flat_grad, self.exp_avg,
+                                                                    self.exp_avg_sq)))
+        return out
+
+    def enqueue_update(self, check_finite: bool = True, voxel_block=None):
         """Gradient exchange -> inf check -> LR / bias-correction scalars -> fused Adam (+fp16 shadow, grad zero) ->
         GradScaler.update(), all on the current stream with device-side scalars (graph-capturable).
 
@@ -194,10 +203,23 @@ class NGPTrainer:
         (always: identical on every rank, catches local inf/NaN and overflow alike) -> Adam reads the fp16 sum and
         zeroes the fp32 accumulation buffer.
 
-        check_finite=False: the backward kernels already raised the inf flag at the source (fast_step.py)."""
+        check_finite=False: the backward kernels already raised the inf flag at the source (fast_step.py).
+
+        voxel_block = (lo_x, lo_y, lo_z, hi_x, hi_y, hi_z), one rank, a voxel-grid model: the finite check and Adam run
+        over the fields' elements inside that node block only (DESIGN.md §6b).  Elements outside it are neither checked,
+        applied nor cleared, so the caller must know that its gradient is zero there, as StaticTrainStep does: every
+        gradient its own march, backward and regularisers produce lies inside the block."""
         L, st = load(), C.c_void_p(torch.cuda.current_stream().cuda_stream)
         R, fg, g16, P = self.p2p, self.flat_grad, self.grad16, self.slices[0][1]
-        if g16 is not None:
+        if voxel_block is not None:
+            if R is not None or g16 is not None or len(self.params) != 2:
+                raise ValueError("NGPTrainer: the node-block optimizer pass is for a one-rank voxel-grid model")
+            fields = self.voxel_fields()
+            b6 = (C.c_int32 * 6)(*[int(v) for v in voxel_block])
+        if voxel_block is not None and check_finite:
+            for prm, grd, _, _ in fields:
+                check(L.ngp_check_finite_voxel_block(_p(grd), prm.shape[0], prm.shape[-1], b6, _p(self.found_inf), st))
+        elif g16 is not None:
             check(L.ngp_grad_pack_f16(_p(fg), _p(g16), fg.numel(), st))
             parallel.allreduce_gradients(g16, self.pg)
             check(L.ngp_check_finite_f16(_p(g16), g16.numel(), _p(self.found_inf), st))
@@ -210,7 +232,12 @@ class NGPTrainer:
         check(L.ngp_adam_hyper_update(_p(self.step_dev), self.lr0, self.lr0 / 30, self.max_steps, self.betas[0],
                                       self.betas[1], inv, _p(self.found_inf), _p(self.hyper), st))
         # one Adam launch over [hash table | MLP weights]
-        if R is not None:
+        if voxel_block is not None:   # one per field, over its node block
+            for prm, grd, m, v in fields:
+                check(L.ngp_adam_step_voxel_block_dyn(_p(prm), _p(grd), _p(m), _p(v), prm.shape[0], prm.shape[-1], b6,
+                                                      _p(self.found_inf), _p(self.hyper), self.betas[0], self.betas[1],
+                                                      self.eps, st))
+        elif R is not None:
             check(L.ngp_adam_step_p2p(_p(self.flat_param), R.grad_tab, _p(self.exp_avg), _p(self.exp_avg_sq),
                                       R.shadow_tab, R.rank, R.world, _p(self.found_inf), _p(self.hyper), self.betas[0],
                                       self.betas[1], self.eps, self.shard_lo, self.shard_lo + self.shard, P,
