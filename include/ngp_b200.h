@@ -431,6 +431,18 @@ int ngp_composite_round(const float* sigmas, const void* rgbs, int rgbs_dtype, c
                         float T_threshold, float* opacity, float* depth, float* rgb, int32_t* next_alive,
                         int64_t n_rays, int limit, void* stream);
 
+/* ---- test-time evaluation: SSIM ---------------------------------------------------------------------------------
+ * replaces the reference's StructuralSimilarityIndexMeasure(data_range=1) of torchmetrics (train.py:20, :82-84) as
+ * evaluated per held-out view (:269-272) and averaged into the `evaluation: psnr_avg=... | ssim_avg=...` line
+ * (:303-304).  pred / target: n_images fp32 images [height*width, 3], row-major, RGB interleaved, one after another.
+ * Gaussian window sigma 1.5 over 11 taps, C1 = 0.01^2, C2 = 0.03^2; ssim_out[i] = mean of the SSIM map of image i
+ * over its 3 channels x the (height-10) x (width-10) positions where the window lies inside the image (DESIGN.md §6e).
+ * Inputs are not clamped; a NaN or inf in an image makes that image's result NaN.  `partial`: caller scratch of
+ * n_images * (height-10) floats.  No atomics: the result is bit-reproducible.  height, width >= 11; n_images == 0:
+ * no-op. */
+int ngp_ssim(const float* pred, const float* target, int64_t n_images, int height, int width, float* partial,
+             float* ssim_out, void* stream);
+
 /* ---- occupancy-grid helpers (SURVEY §8f rank 1) ---------------------------- */
 /* replaces packbits, modules/utils.py:157-169 */
 int ngp_packbits(const float* density_grid, float density_threshold,

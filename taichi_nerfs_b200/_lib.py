@@ -80,6 +80,7 @@ def _declare(lib):
                                                i64, vp]),
         "ngp_distortion_fwd": (ci, [vp, vp, vp, vp, vp, i64, i64, vp]),
         "ngp_distortion_bwd": (ci, [vp, vp, vp, vp, vp, vp, i64, i64, vp]),
+        "ngp_ssim": (ci, [vp, vp, i64, ci, ci, vp, vp, vp]),
         "ngp_packbits": (ci, [vp, f32, vp, i64, vp]),
         "ngp_packbits_dev": (ci, [vp, vp, f32, vp, i64, vp]),
         "ngp_sample_ray_batch": (ci, [vp, ci, vp, vp, i64, i64, vp, vp, i64, C.c_uint64, vp, i32,

@@ -277,6 +277,26 @@ def distortion_bwd(dL_dloss, ws, deltas, ts, rays_a):
     return out
 
 
+# ---- test-time evaluation --------------------------------------------------------------------------
+def ssim(pred, target, height, width):
+    """SSIM (torchmetrics' StructuralSimilarityIndexMeasure, data_range=1; DESIGN.md §6e) of fp32 images [H*W, 3]
+    (one image) or [B, H*W, 3] -> fp32 [B] on the device.  Nothing is read back to the host."""
+    _need_cuda(pred, target)
+    if pred.dtype != torch.float32 or target.dtype != torch.float32:
+        raise TypeError("ssim takes fp32 images")
+    if pred.shape != target.shape:
+        raise ValueError(f"ssim: pred {tuple(pred.shape)} and target {tuple(target.shape)} differ in shape")
+    h, w = int(height), int(width)
+    if pred.dim() not in (2, 3) or tuple(pred.shape[-2:]) != (h * w, 3):
+        raise ValueError(f"ssim expects [H*W, 3] or [B, H*W, 3] with H*W = {h}*{w}, got {tuple(pred.shape)}")
+    n = 1 if pred.dim() == 2 else pred.shape[0]
+    p, t = pred.contiguous(), target.contiguous()
+    partial = torch.empty(n * max(h - 10, 0), device=p.device, dtype=torch.float32)
+    out = torch.empty(n, device=p.device, dtype=torch.float32)
+    check(load().ngp_ssim(_ptr(p), _ptr(t), n, h, w, _ptr(partial), _ptr(out), _stream()), "ssim")
+    return out
+
+
 # ---- occupancy grid helpers ------------------------------------------------------------------------
 def packbits(density_grid, threshold, bitfield, mean_dev=None):
     """bit i of byte n = grid[8n+i] > thr, thr = threshold or min(*mean_dev, threshold) read on the device."""

@@ -1,6 +1,7 @@
 """"PSNR vs ref" protocol (BASELINE.json metric, SURVEY.md §8c): train the stock model on views of the reference's
 shipped trained Lego model (the teacher, datasets/teacher.py) and evaluate on held-out teacher views exactly like
-the reference's test loop (train.py:237-304: render(test_time=True) per view, PSNR = -10 log10(MSE), averaged).
+the reference's test loop (train.py:237-304: render(test_time=True) per view, PSNR = -10 log10(MSE) and SSIM
+(ops.ssim), each averaged).
 
 The reference publishes 35.0 dB on the real Lego test set after 20 k steps (README.md:33-37); that dataset is not
 available offline, so the number reported here is PSNR against the teacher's own renderings — it measures that the
@@ -23,12 +24,14 @@ def train_vs_teacher(device, steps: int = 3000, batch: int = 8192, train_views: 
     """pos_encoder_type='triplane' trains the reference's tri-plane model instead (fp32 planes: half_opt does not
     apply and the loss scale is 2**19, as train.py without --half_opt).  graph=True trains through the graph-captured
     step (StaticTrainStep, either encoder), graph=False through NGPTrainer.step; "path" in the result says which.
-    Returns {"psnr": mean dB over the held-out views, "psnr_views": [...], "steps": ..., "steps_per_s": ...,
+    Returns {"psnr": mean dB over the held-out views, "psnr_views": [...], "ssim": mean SSIM over the same views (of
+    the same clamped prediction), "ssim_views": [...], "steps": ..., "steps_per_s": ...,
     "rays_per_s": ..., "model": the trained NGP} or None when the teacher fixture is not staged."""
     from datasets.ray_utils import get_rays
     from datasets.teacher import TeacherLego, load_teacher
     from modules.networks import NGP
     from modules.rendering import render
+    from . import ops
     from .fast_step import StaticTrainStep
     from .trainer import NGPTrainer
 
@@ -73,17 +76,21 @@ def train_vs_teacher(device, steps: int = 3000, batch: int = 8192, train_views: 
     dt = time.perf_counter() - t0
 
     model.eval()
-    psnrs = []
+    psnrs, ssims = [], []
+    tw, th = test_ds.img_wh
     with torch.no_grad():
         for i in range(len(test_ds)):
             td = test_ds[i]
             rays_o, rays_d = get_rays(test_ds.directions, td['pose'])
             with torch.autocast('cuda', dtype=torch.float16):
                 res = render(model, rays_o, rays_d, test_time=True)
-            mse = F.mse_loss(res['rgb'].float().clamp(0, 1), td['rgb'])
+            pred = res['rgb'].float().clamp(0, 1)
+            mse = F.mse_loss(pred, td['rgb'])
             psnrs.append(float(-10.0 * torch.log10(mse)))
+            ssims.append(float(ops.ssim(pred, td['rgb'], th, tw)))
     w, h = train_ds.img_wh
-    return {"psnr": sum(psnrs) / len(psnrs), "psnr_views": psnrs, "steps": steps, "batch": batch,
+    return {"psnr": sum(psnrs) / len(psnrs), "psnr_views": psnrs, "ssim": sum(ssims) / len(ssims),
+            "ssim_views": ssims, "steps": steps, "batch": batch,
             "train_views": train_views, "test_views": test_views, "image_wh": [w, h],
             "steps_per_s": steps / dt, "rays_per_s": steps * batch / dt, "train_seconds": dt,
             "path": "graph" if graph else "modules", "model": model, "test_dataset": test_ds}

@@ -2,7 +2,7 @@
 seeds (:39-42), model_config (:86-117), mark_invisible_cells (:129), loss scale 2**16 | 2**19 (:137-141),
 Adam(lr, eps=1e-15) + cosine annealing to lr/30 (:143-163), density-grid update every 16 steps with a
 256-step warm-up (:57-58,178-182), log line every 1000 steps (:203-219), results/model.pth (:232-235),
-test-split PSNR (:237-304).  The step body runs on the sm_90a kernels through NGPTrainer (fused Adam,
+test-split PSNR and SSIM (:237-304).  The step body runs on the sm_90a kernels through NGPTrainer (fused Adam,
 no host sync for the inf check); under torchrun every rank trains on its own rays and the gradients are summed
 once per step: by the peer-memory optimizer kernel when all ranks share one NVLink box, else by an fp16 NCCL
 all-reduce of the flat gradient buffer.
@@ -23,6 +23,7 @@ from modules.networks import MODEL_DICT
 from modules.rendering import MAX_SAMPLES, render
 from modules.utils import depth2img, save_deployment_model
 from opt import get_opts
+from taichi_nerfs_b200 import ops
 from taichi_nerfs_b200.trainer import NGPTrainer
 
 warnings.filterwarnings("ignore")
@@ -137,10 +138,10 @@ def main(prefix_args=None):
     os.makedirs(val_dir, exist_ok=True)
     torch.save(model.state_dict(), os.path.join(val_dir, 'model.pth'))
 
-    # test loop (train.py:237-304): PSNR per held-out view; first view saved as PNG
+    # test loop (train.py:237-304): PSNR and SSIM per held-out view; first view saved as PNG
     model.eval()
     w, h = test_dataset.img_wh
-    psnrs = []
+    psnrs, ssims = [], []
     with torch.no_grad():
         for i in range(len(test_dataset)):
             td = test_dataset[i]
@@ -149,6 +150,7 @@ def main(prefix_args=None):
                 results = render(model, rays_o, rays_d, test_time=True, exp_step_factor=exp_step_factor)
             if 'rgb' in td:
                 psnrs.append(float(psnr_of(F.mse_loss(results['rgb'].float(), td['rgb']))))
+                ssims.append(ops.ssim(results['rgb'].float(), td['rgb'], h, w))
             if i == 0:
                 from PIL import Image
                 img = (results['rgb'].float().clamp(0, 1).reshape(h, w, 3).cpu().numpy() * 255).astype(np.uint8)
@@ -156,7 +158,8 @@ def main(prefix_args=None):
                 Image.fromarray(depth2img(results['depth'].reshape(h, w).cpu().numpy())).save(
                     os.path.join(val_dir, 'depth_000.png'))
     if psnrs:
-        print(f"evaluation: psnr_avg={sum(psnrs) / len(psnrs)}")
+        ssim_avg = float(torch.cat(ssims).double().mean())
+        print(f"evaluation: psnr_avg={sum(psnrs) / len(psnrs)} | ssim_avg={ssim_avg}")
 
     if hparams.gui:
         from gui import NGPGUI
