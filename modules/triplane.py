@@ -69,8 +69,9 @@ class TriPlaneEncoder(torch.nn.Module):
                                       "there); pass positions that do not require grad")
         return _TriplaneEncode.apply(positions.float().contiguous(), self.plane_embedding, self)
 
-    # ---- kernel-level interface (NGP's grid update and the frame renderers) -------------------------------------
+    # ---- kernel-level interface (NGP's grid update, the frame renderers and the graph-captured step) --------------
     emb_dtype = torch.float32
+    bwd_raises_inf = True   # the table backward raises GradScaler's inf flag itself, in both feature widths
 
     def kernel_table(self):
         """The tensor the encode kernel reads (its pointer is tracked by FrameRenderer's graph)."""

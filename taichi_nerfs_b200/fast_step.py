@@ -38,18 +38,15 @@ class StaticTrainStep:
         self.tr = trainer
         m = self.model = trainer.model
         # the voxel-grid model: fp32 fields and outputs, no encoder and no MLP; its optimizer pass covers the node
-        # block B only (DESIGN.md §6b)
-        self.vox = hasattr(m, "sh_fields") and hasattr(m, "density_fields")
-        enc = getattr(m, "pos_encoder", None)
-        self.tri = hasattr(enc, "plane_embedding")
+        # block B only (DESIGN.md §6b).  Otherwise the two encoder stages are the encoder's launches (hash or
+        # tri-plane), with its embedding dtype.
+        enc = self.enc = trainer.encoder
+        self.vox = enc is None
         if self.vox:
             if trainer.world_size > 1:
                 raise _lib.NgpError("StaticTrainStep runs a voxel-grid model on one rank only")
         elif not m._fusable(next(m.parameters())):
             raise _lib.NgpError("StaticTrainStep needs the stock NGP architecture (fused MLP)")
-        # the tri-plane model: fp32 planes and embedding, no fp16 shadow; the encode launches go through the encoder
-        elif not self.tri and not hasattr(enc, "hash_table"):
-            raise _lib.NgpError("StaticTrainStep runs the hash or the tri-plane encoder's kernels")
         dev = next(m.parameters()).device
         self.dev, self.n = dev, int(n_rays)
         self.cap = C_ = int(n_rays) * int(samples_per_ray_capacity)
@@ -58,7 +55,8 @@ class StaticTrainStep:
         self.distortion_w = float(distortion_loss_w)
         if not self.distortion_w >= 0.0 or self.distortion_w == float("inf"):
             raise ValueError(f"distortion_loss_w must be finite and >= 0, got {distortion_loss_w}")
-        self.half = hasattr(enc, "table_f16")
+        # fp16 embeddings (the --half_opt hash encoder): the MLP kernels run their fp16-embedding instantiations
+        self.half = not self.vox and enc.emb_dtype == torch.float16
         edt = torch.float16 if self.half else torch.float32
         f32, i32 = torch.float32, torch.int32
         z = lambda *s, dtype=f32: torch.zeros(*s, device=dev, dtype=dtype)  # noqa: E731
@@ -97,7 +95,6 @@ class StaticTrainStep:
             self.P = m.sh_fields.numel()
             assert trainer.slices[0] == (0, self.P) and trainer.slices[1][1] == m.density_fields.numel()
         else:
-            self._clayout = enc._clayout
             self._w_keep = [w.detach() for w in mlp_weights(m)]
             self._wst = _lib.MlpWeights(*[w.data_ptr() for w in self._w_keep])
             self.P = enc.total_param_size
@@ -123,10 +120,11 @@ class StaticTrainStep:
         # one rank or the peer-memory step + dynamic loss scale: the backward kernels raise GradScaler's inf flag
         # themselves (a non-finite contribution is seen where it is scattered), the optimizer consumes and clears it -
         # no 45 MB check pass (the NCCL fallback checks the reduced fp16 sum instead)
-        # (the hash backward raises it in its F = 2 instantiation only, the tri-plane backward in both).  The voxel
-        # grid: the regularisers' gradient is not seen by any backward, so the finite check over B covers them all.
+        # (enc.bwd_raises_inf: the hash backward raises it in its F = 2 instantiation only, the tri-plane backward in
+        # both).  The voxel grid: the regularisers' gradient is not seen by any backward, so the finite check over B
+        # covers them all.
         self.inf_at_source = bool((trainer.world_size == 1 or trainer.p2p is not None) and self.dynamic_loss_scale
-                                  and not self.vox and (self.tri or enc._clayout.feat_dim == 2))
+                                  and not self.vox and enc.bwd_raises_inf)
         if self.inf_at_source:
             trainer.found_inf.zero_()
         self.use_graph = bool(use_graph)
@@ -168,9 +166,9 @@ class StaticTrainStep:
         return C.c_void_p(torch.cuda.current_stream().cuda_stream)
 
     def _table(self):
-        if self.tri:
-            return self.model.pos_encoder.kernel_table()   # a view of the trainer's flat_param: stable across steps
-        return self.tr._shadow if self.half else self.model.pos_encoder.hash_table.data
+        # the fp16 hash table: the trainer's shadow slice, which the fused Adam rewrites in place (the encoder's own
+        # kernel_table() re-casts into a new tensor whenever the master moved); else a view of the trainer's flat_param
+        return self.tr._shadow if self.tr._shadow is not None else self.enc.kernel_table()
 
     def _enqueue_march(self):
         L, m, st, n, cap = load(), self.model, self._st(), self.n, self.cap
@@ -184,15 +182,10 @@ class StaticTrainStep:
                                       _p(self.deltas), _p(self.ts), n, cap, st))
 
     # the five network kernels, one method each (bench.py times them one by one on the buffers of a real step)
-    # (the two _k_hash_* are "the position encoder": for a tri-plane model they run its launches)
+    # (the two _k_hash_* are "the position encoder": hash or tri-plane, they run the encoder's launches)
     def _k_hash_fwd(self):
-        L, st, tag = load(), self._st(), (F16 if self.half else F32)
-        if self.tri:
-            check(self.model.pos_encoder.enqueue_encode_dyn(L, _p(self.xyzs), _p(self._table()), _p(self.emb),
-                                                            self.cap, _p(self.counter), self.aabb6, st))
-            return
-        check(L.ngp_hash_encode_fwd_dyn(_p(self.xyzs), _p(self._table()), C.byref(self._clayout), _p(self.emb), tag,
-                                        self.cap, _p(self.counter), self.aabb6, st))
+        check(self.enc.enqueue_encode_dyn(load(), _p(self.xyzs), _p(self._table()), _p(self.emb), self.cap,
+                                          _p(self.counter), self.aabb6, self._st()))
 
     def _k_mlp_fwd(self):
         L, st, tag = load(), self._st(), (F16 if self.half else F32)
@@ -223,21 +216,10 @@ class StaticTrainStep:
                                 _p(self.drgbs), _p(self.demb), _p(gw), self.cap, _p(self.counter),
                                 _p(self.tr.found_inf) if self.inf_at_source else None, st))
 
-    def _k_hash_bwd(self, level_begin=0, level_end=None):
-        L, st, tag = load(), self._st(), (F16 if self.half else F32)
-        if self.tri:
-            if level_begin != 0 or level_end is not None:
-                raise _lib.NgpError("level_begin / level_end select hash levels; all tri-plane levels scatter into "
-                                    "the same three planes")
-            check(self.model.pos_encoder.enqueue_encode_bwd_dyn(
-                L, _p(self.xyzs), _p(self._table()), _p(self.demb), _p(self.tr.flat_grad), self.cap, _p(self.counter),
-                self.aabb6, _p(self.tr.found_inf) if self.inf_at_source else None, st))
-            return
-        level_end = self._clayout.n_levels if level_end is None else level_end
-        check(L.ngp_hash_encode_bwd_levels(_p(self.xyzs), _p(self.demb), tag, C.byref(self._clayout),
-                                           _p(self.tr.flat_grad), self.cap, _p(self.counter), self.aabb6,
-                                           int(level_begin), int(level_end),
-                                           _p(self.tr.found_inf) if self.inf_at_source else None, st))
+    def _k_hash_bwd(self):
+        check(self.enc.enqueue_encode_bwd_dyn(load(), _p(self.xyzs), _p(self._table()), _p(self.demb),
+                                              _p(self.tr.flat_grad), self.cap, _p(self.counter), self.aabb6,
+                                              _p(self.tr.found_inf) if self.inf_at_source else None, self._st()))
 
     # the voxel grid's stages: fields -> fp32 sigma / rgb, and the field gradient into the trainer's flat buffer
     def _k_voxel_fwd(self):
@@ -370,14 +352,14 @@ class StaticTrainStep:
                 self.tr.found_inf.zero_()
             self._enqueue_update()
             self.pending = False
-            if self.tr._shadow is not None:   # (a voxel grid has neither a shadow nor a pos_encoder)
-                self.model.pos_encoder.adopt_shadow(self.tr._shadow)
+            if self.tr._shadow is not None:
+                self.enc.adopt_shadow(self.tr._shadow)
         self.tr.sync_master()   # peer-memory step: the fp32 master table is complete again on every rank
 
     def _finish_step(self):
         self.tr.step_count += 1
         if self.tr._shadow is not None:
-            self.model.pos_encoder.adopt_shadow(self.tr._shadow)
+            self.enc.adopt_shadow(self.tr._shadow)
         return self.loss_sum / (3.0 * self.n)
 
     def attach_ray_source(self, image_bank, poses, directions, seed: int = 0, fixed_img: int = -1):

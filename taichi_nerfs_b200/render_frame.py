@@ -30,7 +30,6 @@ def render_frame(model, rays_o, rays_d, exp_step_factor=0.0, T_threshold=1e-4, m
     rgb = torch.empty(n, 3, device=dev, dtype=torch.float32)
     depth = torch.empty(n, device=dev, dtype=torch.float32)
     opacity = torch.empty(n, device=dev, dtype=torch.float32)
-    enc = getattr(model, 'pos_encoder', None)   # a VoxelGrid has none: it runs the module path below
     fused = bool(model._fusable(rays_o))     # stock architecture: encoder + fused MLP kernels on the raw sample rows
     if fused:
         W = [w.detach() for w in mlp_weights(model)]
@@ -81,7 +80,7 @@ def render_frame(model, rays_o, rays_d, exp_step_factor=0.0, T_threshold=1e-4, m
             rgb[b:e] = 0
             continue
         if fused:
-            emb = enc.encode_world(xyzs, aabb)  # hash or tri-plane kernel, normalisation in-kernel
+            emb = model.pos_encoder.encode_world(xyzs, aabb)  # hash or tri-plane kernel, normalisation in-kernel
             sigmas, rgbs = ops.mlp_fwd(emb, dirs, W)
         else:   # any other NGP configuration (e.g. the reference's L=4 F=4 deployment model), a VoxelGrid: module forward
             with torch.autocast('cuda', dtype=torch.float16):

@@ -32,11 +32,17 @@ class NGPTrainer:
     def __init__(self, model, lr: float = 1e-2, max_steps: int = 20000, loss_scale: float | None = None,
                  betas=(0.9, 0.999), eps: float = 1e-15, process_group=None, dynamic_loss_scale: bool = True,
                  p2p_optimizer: bool | None = None, voxel_reg=None):
+        from modules.hash_encoder import HashEncoder
+        from modules.voxel_grid import VoxelGrid
+        # The model kind, decided here once (StaticTrainStep reads it too): the position encoder, whose one parameter
+        # (its table) must be the first slice of the flat buffers, or None for a VoxelGrid, which has no encoder and
+        # scatters into the .grad views of its own fields.
+        self.encoder = enc = None if isinstance(model, VoxelGrid) else model.pos_encoder
         # voxel_reg = (w_tv_sigma, w_tv_sh, w_sparsity): the voxel grid's regularisers (DESIGN.md §6d), enqueued after
         # the render backward.  None or all zero: nothing is enqueued.
         self.voxel_reg = None
         if voxel_reg is not None:
-            if not (hasattr(model, 'sh_fields') and hasattr(model, 'density_fields')):
+            if enc is not None:
                 raise ValueError("NGPTrainer: voxel_reg (total variation / sparsity) applies to a model with voxel "
                                  "fields (--model_name svox); this model has none")
             w = tuple(float(v) for v in voxel_reg)
@@ -58,6 +64,12 @@ class NGPTrainer:
             self.world_size = torch.distributed.get_world_size(process_group)
 
         self.params = [p for p in model.parameters() if p.requires_grad]
+        if enc is not None:
+            table = list(enc.parameters())
+            if len(table) != 1 or table[0] is not self.params[0]:
+                raise ValueError("NGPTrainer: the position encoder must have one parameter, the model's first")
+        # the fp16 hash encoder gathers from an fp16 copy of its table, which the fused Adam rewrites (the shadow below)
+        shadowed = enc is not None and enc.emb_dtype == torch.float16
         dev = self.params[0].device
         # one flat gradient buffer so the multi-GPU path is a single all-reduce (hash grad | MLP grads)
         sizes = [p.numel() for p in self.params]
@@ -68,13 +80,12 @@ class NGPTrainer:
         # kernel that sums the owned 1/N of the gradient with peer loads, runs Adam on it and stores the new fp16 table
         # slice into every rank's shadow with peer stores (csrc/p2p.cu).  None when unavailable (NCCL fallback below).
         self.p2p = None
-        # a model without a position encoder (VoxelGrid) scatters into the .grad views of its own parameters
-        P_, enc_ = sizes[0], getattr(model, 'pos_encoder', None)
-        if p2p_optimizer and (enc_ is None or hasattr(enc_, 'plane_embedding')):
+        P_ = sizes[0]
+        if p2p_optimizer and not isinstance(enc, HashEncoder):
             raise ValueError("NGPTrainer: the peer-memory optimizer shards the fp16 hash table; a tri-plane or "
                              "voxel-grid model uses the all-reduce of the flat gradient (p2p_optimizer off)")
-        if (p2p_optimizer is not False and self.world_size > 1 and dev.type == "cuda" and hasattr(enc_, "adopt_shadow")
-                and self.params[0] is enc_.hash_table and P_ % (4 * self.world_size) == 0):
+        if (p2p_optimizer is not False and self.world_size > 1 and dev.type == "cuda" and shadowed
+                and P_ % (4 * self.world_size) == 0):
             from .p2p import PeerRegion
             self.p2p = PeerRegion.create(total, dev, process_group)
         self.flat_grad = self.p2p.grad if self.p2p is not None else torch.zeros(total, device=dev, dtype=torch.float32)
@@ -92,11 +103,10 @@ class NGPTrainer:
                 self.flat_param[off:off + s].copy_(p.data.reshape(-1))
             p.data = self.flat_param[off:off + s].view_as(p)
             off += s + q
-            if enc_ is not None and (p is getattr(enc_, 'hash_table', None)
-                                     or p is getattr(enc_, 'plane_embedding', None)):
-                enc_.grad_sink = self.flat_grad[off - s - q:off - q]
-        if enc_ is None:
+        if enc is None:
             model.grad_sink = (model.sh_fields.grad, model.density_fields.grad)
+        else:
+            enc.grad_sink = self.flat_grad[:P_]
         self.found_inf = torch.zeros(1, device=dev, dtype=torch.int32)
         # device-side optimizer scalars (shared with StaticTrainStep): iteration counter, [lr/bc1, sqrt(bc2), 1/(scale*world),
         # Adam step count], GradScaler state [scale, growth tracker]
@@ -107,16 +117,14 @@ class NGPTrainer:
         self.scale_state = torch.tensor([self.loss_scale, 0.0], device=dev, dtype=torch.float32)
         self._views = [(p, p.data_ptr(), p.grad.data_ptr()) for p in self.params]
         self._shadow = self._shadow_full = None
-        enc = enc_
-        if hasattr(enc, "adopt_shadow"):
-            assert self.params[0] is enc.hash_table, "the hash table must be the first parameter"
+        if shadowed:
             # fp16 copy of the whole flat buffer, rewritten by the Adam pass; the encoder reads its first slice
             if self.p2p is not None:
                 self._shadow_full = self.p2p.shadow
                 self._shadow_full.copy_(self.flat_param)
             else:
                 self._shadow_full = self.flat_param.to(torch.float16)
-            self._shadow = self._shadow_full[:enc.hash_table.numel()]
+            self._shadow = self._shadow_full[:P_]
             enc.adopt_shadow(self._shadow)
 
         # Peer-memory step: the optimizer is sharded over the hash table (the MLP weights stay replicated); each rank
@@ -151,11 +159,12 @@ class NGPTrainer:
         for p in self.params:
             p.data = p.data.clone()
             p.grad = None
-        enc = getattr(self.model, 'pos_encoder', self.model)   # a VoxelGrid holds its grad_sink itself
-        if hasattr(enc, 'grad_sink'):
-            enc.grad_sink = None
-        if self._shadow is not None and hasattr(enc, 'adopt_shadow'):
-            enc.adopt_shadow(None)
+        if self.encoder is None:   # a VoxelGrid holds its grad_sink itself
+            self.model.grad_sink = None
+        else:
+            self.encoder.grad_sink = None
+        if self._shadow is not None:
+            self.encoder.adopt_shadow(None)
         self._views = []
 
     def forward_backward(self, rays_o, rays_d, rgb_gt, exp_step_factor=0.0, extra_loss=None):
@@ -280,7 +289,7 @@ class NGPTrainer:
         self.found_inf.zero_()
         self.enqueue_update()
         if self._shadow is not None:
-            self.model.pos_encoder.adopt_shadow(self._shadow)
+            self.encoder.adopt_shadow(self._shadow)
 
     def step(self, rays_o, rays_d, rgb_gt, exp_step_factor=0.0, extra_loss=None):
         loss, results = self.forward_backward(rays_o, rays_d, rgb_gt, exp_step_factor, extra_loss)

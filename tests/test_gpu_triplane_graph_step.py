@@ -501,10 +501,7 @@ def test_static_step_refusals():
     from taichi_nerfs_b200.fast_step import StaticTrainStep
     from taichi_nerfs_b200.trainer import NGPTrainer
     m, tr, _ = _build()
-    fs = StaticTrainStep(tr, 256, samples_per_ray_capacity=64, use_graph=False)
-    for kw in (dict(level_begin=1), dict(level_end=4), dict(level_begin=0, level_end=8)):
-        with pytest.raises(NgpError):
-            fs._k_hash_bwd(**kw)
+    StaticTrainStep(tr, 256, samples_per_ray_capacity=64, use_graph=False)
     m = NGP(scale=0.5, max_res=1024, half_opt=False, pos_encoder_type="triplane").cuda()
     m.xyz_encoder.net_width = 32                 # not the stock architecture
     with pytest.raises(NgpError):
