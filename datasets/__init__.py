@@ -1,7 +1,12 @@
-"""Dataset registry.  The disk loaders of the reference (nsvf/nerf/colmap/ngp) are out of scope
-(SURVEY.md §2.1 row 5: no dataset exists offline) and opt.py rejects those names; the synthetic Lego-shape set
-drives the hot path and the teacher set (views of the reference's shipped trained Lego model) the PSNR protocol."""
+"""Dataset registry.  The reference's four disk loaders (nerf, nsvf, ngp, colmap; DESIGN.md §6f) read the
+formats the reference's training scripts pass with ``--root_dir``; the synthetic Lego-shape set drives the
+benchmark and the teacher set (views of the reference's shipped trained Lego model) the PSNR protocol."""
+from .colmap import ColmapDataset
+from .nerf import NeRFDataset
+from .ngp import NGPDataset
+from .nsvf import NSVFDataset
 from .synthetic import SyntheticLego
 from .teacher import TeacherLego
 
-dataset_dict = {'synthetic': SyntheticLego, 'teacher': TeacherLego}
+dataset_dict = {'synthetic': SyntheticLego, 'teacher': TeacherLego, 'nerf': NeRFDataset, 'nsvf': NSVFDataset,
+                'colmap': ColmapDataset, 'ngp': NGPDataset}

@@ -388,6 +388,21 @@ int ngp_ray_head_fused_distortion(const float* sigmas, const void* rgbs, int rgb
                                   float loss_scale, const float* scale_dev, float T_threshold,
                                   float distortion_w, float* loss_sum, float* opacity_out, float* rgb_out,
                                   float* dL_dsigmas, void* dL_drgbs, int64_t n_rays, void* stream);
+/* --random_bg (DESIGN.md §6f): out[r] = the background colour of training ray r at step s, three floats in [0, 1) from
+ * Philox4x32-10 with counter (r, r >> 32, s, 0x62670001) and key (seed, seed >> 32); s = step_dev[0] if step_dev !=
+ * NULL else step_host (a graph replay reads the step from device memory). */
+int ngp_random_bg(uint64_t seed, const int32_t* step_dev, int32_t step_host, float* out, int64_t n_rays,
+                  void* stream);
+/* The fused head with a per-ray background bg_rgb [n_rays, 3] (ngp_random_bg) instead of a constant: prediction
+ * out = rgb + bg_rgb (1 - opacity); where alpha != NULL ([n_rays], the image's alpha), the target becomes
+ * gt + (bg_rgb - b_load)(1 - alpha), b_load being the colour the loader blended transparent pixels onto.
+ * distortion_w > 0 adds the distortion loss as ngp_ray_head_fused_distortion does (ts then required).  The
+ * constant-background entries above are unchanged. */
+int ngp_ray_head_fused_random_bg(const float* sigmas, const void* rgbs, int rgbs_dtype, const float* deltas,
+                                 const float* ts, const int32_t* rays_a, const float* gt, const float* bg_rgb,
+                                 const float* alpha, float b_load, float loss_scale, const float* scale_dev,
+                                 float T_threshold, float distortion_w, float* loss_sum, float* opacity_out,
+                                 float* rgb_out, float* dL_dsigmas, void* dL_drgbs, int64_t n_rays, void* stream);
 
 /* ---- distortion loss (SURVEY §8f rank 3) -------------------------------------- */
 /* replaces prefix_sums_kernel + _loss_kernel + distortion_loss_fw_kernel

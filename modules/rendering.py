@@ -13,10 +13,11 @@ NEAR_DISTANCE = 0.01
 
 
 def render(model, rays_o, rays_d, test_time=False, exp_step_factor=0, T_threshold=1e-4,
-           max_samples=MAX_SAMPLES):
+           max_samples=MAX_SAMPLES, bg_rgb=None):
     """AABB test, then the train or test rendering path.  Returns the result dict of the
     reference (train: rgb, depth, opacity, ws, deltas, ts, rays_a, rm_samples, vr_samples;
-    test: rgb, depth, opacity, total_samples)."""
+    test: rgb, depth, opacity, total_samples).  ``bg_rgb`` [N, 3] (training path only, --random_bg): each ray's own
+    background colour in place of the fixed white / black one."""
     rays_o = rays_o.contiguous()
     rays_d = rays_d.contiguous()
     hits_t = ray_aabb_intersection(rays_o, rays_d, model.scale)
@@ -29,7 +30,7 @@ def render(model, rays_o, rays_d, test_time=False, exp_step_factor=0, T_threshol
                 return render_frame_compact(model, rays_o, rays_d, exp_step_factor, T_threshold, max_samples)
             return render_frame(model, rays_o, rays_d, exp_step_factor, T_threshold, max_samples)
         return _render_rays_test(model, rays_o, rays_d, hits_t, exp_step_factor, T_threshold, max_samples)
-    return _render_rays_train(model, rays_o, rays_d, hits_t, exp_step_factor, T_threshold)
+    return _render_rays_train(model, rays_o, rays_d, hits_t, exp_step_factor, T_threshold, bg_rgb)
 
 
 def _background(exp_step_factor, device):
@@ -75,7 +76,7 @@ def _render_rays_test(model, rays_o, rays_d, hits_t, exp_step_factor=0, T_thresh
     return results
 
 
-def _render_rays_train(model, rays_o, rays_d, hits_t, exp_step_factor=0, T_threshold=1e-4):
+def _render_rays_train(model, rays_o, rays_d, hits_t, exp_step_factor=0, T_threshold=1e-4, bg_rgb=None):
     results = {}
     (rays_a, xyzs, dirs, results['deltas'], results['ts'], results['rm_samples']) = raymarching_train(
         rays_o, rays_d, hits_t, model.density_bitfield, model.cascades, model.scale, exp_step_factor,
@@ -87,6 +88,6 @@ def _render_rays_train(model, rays_o, rays_d, hits_t, exp_step_factor=0, T_thres
         model.render_func(sigmas, rgbs, results['deltas'], results['ts'], rays_a, T_threshold)
     results['rays_a'] = rays_a
 
-    bg = _background(exp_step_factor, rays_o.device)
+    bg = _background(exp_step_factor, rays_o.device) if bg_rgb is None else bg_rgb
     results['rgb'] = results['rgb'] + bg * (1 - results['opacity'])[:, None]
     return results

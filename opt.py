@@ -1,17 +1,19 @@
 """Command-line flags — same names, defaults and help semantics as the reference's opt.py:4-134 (the
-flag table is restated here as data; `--dataset_name synthetic` and the torchrun-related behaviour are
-the only additions)."""
+flag table is restated here as data; `--dataset_name synthetic | teacher` and the torchrun-related behaviour
+are the additions)."""
 import argparse
 import math
 
 # (flag, kwargs)
 _FLAGS = [
     # dataset parameters
-    ('--root_dir', dict(type=str, default='', help='root directory of dataset (unused by the synthetic dataset)')),
-    ('--dataset_name', dict(type=str, default='synthetic', choices=['synthetic', 'teacher'],
+    ('--root_dir', dict(type=str, default='', help='root directory of dataset (needed by nerf, nsvf, colmap and ngp; '
+                                                  'unused by synthetic and teacher)')),
+    ('--dataset_name', dict(type=str, default='synthetic', choices=['synthetic', 'teacher', 'nerf', 'nsvf', 'colmap',
+                                                                     'ngp'],
                             help='synthetic: analytic scene; teacher: views of the reference\'s shipped trained Lego '
-                                 'model.  The disk loaders nerf/nsvf/colmap/ngp of the reference are out of scope '
-                                 '(SURVEY.md §2.1; no dataset exists offline) and are rejected here')),
+                                 'model; nerf (Blender transforms_*.json), nsvf, colmap (sparse/0/*.bin), ngp '
+                                 '(transforms.json): the reference\'s disk loaders, reading --root_dir')),
     ('--split', dict(type=str, default='train', choices=['train', 'trainval', 'trainvaltest'],
                      help='use which split to train')),
     ('--downsample', dict(type=float, default=1.0, help='downsample factor (<=1.0) for the images')),
@@ -65,6 +67,7 @@ _FLAGS = [
 ]
 
 _VOXEL_REG_FLAGS = ('tv_sigma_loss_w', 'tv_sh_loss_w', 'sparsity_loss_w')
+DISK_DATASETS = ('nerf', 'nsvf', 'colmap', 'ngp')
 
 
 def get_opts(prefix_args=None):
@@ -72,6 +75,8 @@ def get_opts(prefix_args=None):
     for flag, kw in _FLAGS:
         parser.add_argument(flag, **kw)
     hparams = parser.parse_args(prefix_args)
+    if hparams.dataset_name in DISK_DATASETS and not hparams.root_dir:
+        parser.error(f"--dataset_name {hparams.dataset_name} reads a dataset from disk: it needs --root_dir")
     for flag in _VOXEL_REG_FLAGS:
         w = getattr(hparams, flag)
         if not (math.isfinite(w) and w >= 0):

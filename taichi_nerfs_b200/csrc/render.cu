@@ -9,6 +9,7 @@
 // 32-sample chunks, early termination is a ballot, and the per-ray sums are shuffle reductions.
 // Streaming work: HBM/L2-bandwidth bound, ~22 B/sample forward and ~36 B/sample backward.
 #include "common.cuh"
+#include "philox.cuh"
 
 namespace {
 
@@ -304,13 +305,19 @@ __global__ void __launch_bounds__(256) mse_loss_grad_kernel(const float* __restr
 //   dL/dw_k  = coef_d (2 (t_k W_<k - WT_<k) + 2 (WT_>k - t_k W_>k) + 2/3 w_k delta_k),  coef_d = scale w_d / n_rays
 // and dL/dw_k joins G_k, as dL_dws does in composite_train_bwd_kernel.  The prefix carries at every chunk start sit in
 // shared memory beside Tstart (the reverse pass rescans each chunk); the suffixes are accumulated by the reverse walk.
-template <typename T, bool kDist>
+//
+// kRandBg (--random_bg, DESIGN.md §6f): the background is the ray's own colour c_r = bg_rgb[ray] instead of the
+// constant bg; where the image had an alpha channel (alpha != nullptr) the target's loader background b_load is swapped
+// for c_r: gt' = gt + (c_r - b_load)(1 - a).  dL/dopacity = -sum_c c_r,c g_c.
+template <typename T, bool kDist, bool kRandBg = false>
 __global__ void __launch_bounds__(kWarpsPerBlock * 32)
 ray_head_fused_kernel(const float* __restrict__ sigmas, const T* __restrict__ rgbs, const float* __restrict__ deltas,
                       const float* __restrict__ ts, const int32_t* __restrict__ rays_a, const float* __restrict__ gt,
                       float bg, float coef, float coef_d, float w_d, const float* __restrict__ scale_dev, float thr,
                       float* __restrict__ loss_sum, float* __restrict__ opacity_out, float* __restrict__ rgb_out,
-                      float* __restrict__ dsigmas, T* __restrict__ drgbs, int64_t n_rays) {
+                      float* __restrict__ dsigmas, T* __restrict__ drgbs, int64_t n_rays,
+                      const float* __restrict__ bg_rgb = nullptr, const float* __restrict__ alpha = nullptr,
+                      float b_load = 0.0f) {
     __shared__ float Tstart_s[kWarpsPerBlock][kChunkCap];
     __shared__ float Wstart_s[kDist ? kWarpsPerBlock : 1][kDist ? kChunkCap : 1];   // W_<k at every chunk start
     __shared__ float WTstart_s[kDist ? kWarpsPerBlock : 1][kDist ? kChunkCap : 1];  // WT_<k at every chunk start
@@ -400,10 +407,30 @@ ray_head_fused_kernel(const float* __restrict__ sigmas, const T* __restrict__ rg
     b = warp_sum(b);
     op = warp_sum(op);
     // loss head (rendering.py:219-226, train.py:193)
-    const float keep = bg * (1.0f - op);
-    const float d0 = r + keep - gt[ray * 3 + 0], d1 = g + keep - gt[ray * 3 + 1], d2 = b + keep - gt[ray * 3 + 2];
+    float k0, k1, k2, t0 = gt[ray * 3 + 0], t1 = gt[ray * 3 + 1], t2 = gt[ray * 3 + 2];
+    float bc0 = bg, bc1 = bg, bc2 = bg;
+    if constexpr (kRandBg) {
+        bc0 = bg_rgb[ray * 3 + 0];
+        bc1 = bg_rgb[ray * 3 + 1];
+        bc2 = bg_rgb[ray * 3 + 2];
+        const float t = 1.0f - op;
+        k0 = bc0 * t;
+        k1 = bc1 * t;
+        k2 = bc2 * t;
+        if (alpha != nullptr) {
+            const float ta = 1.0f - alpha[ray];
+            t0 += (bc0 - b_load) * ta;
+            t1 += (bc1 - b_load) * ta;
+            t2 += (bc2 - b_load) * ta;
+        }
+    } else {
+        k0 = k1 = k2 = bg * (1.0f - op);
+    }
+    const float d0 = r + k0 - t0, d1 = g + k1 - t1, d2 = b + k2 - t2;
     const float gr = coef * d0, gg = coef * d1, gb = coef * d2;
-    const float go = -bg * (gr + gg + gb);
+    float go;
+    if constexpr (kRandBg) go = -(bc0 * gr + bc1 * gg + bc2 * gb);
+    else go = -bg * (gr + gg + gb);
     if constexpr (kDist) dist = warp_sum(dist);
     if (lane == 0) {
         // kDist: loss_sum / (3 n_rays) = mse + w_d mean(loss_ray)
@@ -411,9 +438,9 @@ ray_head_fused_kernel(const float* __restrict__ sigmas, const T* __restrict__ rg
         else atomicAdd(loss_sum, d0 * d0 + d1 * d1 + d2 * d2);
         if (opacity_out) opacity_out[ray] = op;
         if (rgb_out) {
-            rgb_out[ray * 3 + 0] = r + keep;
-            rgb_out[ray * 3 + 1] = g + keep;
-            rgb_out[ray * 3 + 2] = b + keep;
+            rgb_out[ray * 3 + 0] = r + k0;
+            rgb_out[ray * 3 + 1] = g + k1;
+            rgb_out[ray * 3 + 2] = b + k2;
         }
     }
     __syncwarp();
@@ -732,6 +759,26 @@ composite_round_kernel(const float* __restrict__ sigmas, const T* __restrict__ r
 
 }  // namespace
 
+// ---- --random_bg: one background colour per training ray (DESIGN.md §6f) ------------------------------------------
+// c_r = (unit(v0), unit(v1), unit(v2)) of Philox4x32-10 with counter (r, r >> 32, step, kBgCounterWord) and key
+// (seed, seed >> 32).  The batch sampler (rays.cu) draws with counter word 0, so the two streams never share a counter.
+constexpr uint32_t kBgCounterWord = 0x62670001u;
+
+__device__ __forceinline__ void random_bg_colour(uint64_t seed, uint32_t step, int64_t r, float* out) {
+    const Philox4 v = philox4x32_10((uint32_t)r, (uint32_t)((uint64_t)r >> 32), step, kBgCounterWord, (uint32_t)seed,
+                                    (uint32_t)(seed >> 32));
+    out[0] = philox_unit(v.v[0]);
+    out[1] = philox_unit(v.v[1]);
+    out[2] = philox_unit(v.v[2]);
+}
+
+__global__ void __launch_bounds__(256) random_bg_kernel(uint64_t seed, const int32_t* __restrict__ step_dev,
+                                                        int32_t step_host, float* __restrict__ out, int64_t n) {
+    const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= n) return;
+    random_bg_colour(seed, (uint32_t)(step_dev ? *step_dev : step_host), r, out + r * 3);
+}
+
 extern "C" {
 
 int ngp_mse_loss_grad(const float* rgb, const float* opacity, const float* gt, float bg, float loss_scale,
@@ -804,6 +851,50 @@ int ngp_ray_head_fused_distortion(const float* sigmas, const void* rgbs, int rgb
         ray_head_fused_kernel<float, true><<<grid, kWarpsPerBlock * 32, 0, st>>>(
             sigmas, (const float*)rgbs, deltas, ts, rays_a, gt, bg, coef, coef_d, distortion_w, scale_dev,
             T_threshold, loss_sum, opacity_out, rgb_out, dL_dsigmas, (float*)dL_drgbs, n_rays);
+    NGP_LAUNCHED("ray_head_fused_kernel");
+    return 0;
+}
+
+int ngp_random_bg(uint64_t seed, const int32_t* step_dev, int32_t step_host, float* out, int64_t n_rays, void* stream) {
+    NGP_REQUIRE(n_rays >= 0, "negative n_rays");
+    if (n_rays == 0) return 0;
+    NGP_REQUIRE(out, "null pointer");
+    random_bg_kernel<<<(unsigned)((n_rays + 255) / 256), 256, 0, ngp::as_stream(stream)>>>(seed, step_dev, step_host,
+                                                                                          out, n_rays);
+    NGP_LAUNCHED("random_bg_kernel");
+    return 0;
+}
+
+int ngp_ray_head_fused_random_bg(const float* sigmas, const void* rgbs, int rgbs_dtype, const float* deltas,
+                                 const float* ts, const int32_t* rays_a, const float* gt, const float* bg_rgb,
+                                 const float* alpha, float b_load, float loss_scale, const float* scale_dev,
+                                 float T_threshold, float distortion_w, float* loss_sum, float* opacity_out,
+                                 float* rgb_out, float* dL_dsigmas, void* dL_drgbs, int64_t n_rays, void* stream) {
+    NGP_REQUIRE(n_rays >= 0, "negative n_rays");
+    NGP_REQUIRE(rgbs_dtype == NGP_F32 || rgbs_dtype == NGP_F16, "bad dtype");
+    NGP_REQUIRE(distortion_w >= 0.0f && distortion_w < INFINITY, "distortion_w must be finite and >= 0");
+    if (n_rays == 0) return 0;
+    NGP_REQUIRE(sigmas && rgbs && deltas && rays_a && gt && bg_rgb && loss_sum && dL_dsigmas && dL_drgbs,
+                "null pointer");
+    const bool dist = distortion_w > 0.0f;
+    NGP_REQUIRE(!dist || ts, "null pointer (ts, needed by the distortion loss)");
+    const float scale = scale_dev ? 1.0f : loss_scale;
+    const float coef = scale * 2.0f / (3.0f * (float)n_rays);
+    const float coef_d = scale * distortion_w / (float)n_rays;
+    const unsigned grid = (unsigned)((n_rays + kWarpsPerBlock - 1) / kWarpsPerBlock);
+    cudaStream_t st = ngp::as_stream(stream);
+#define NGP_HEAD_RBG(TT, DD)                                                                                        \
+    ray_head_fused_kernel<TT, DD, true><<<grid, kWarpsPerBlock * 32, 0, st>>>(                                      \
+        sigmas, (const TT*)rgbs, deltas, ts, rays_a, gt, 0.0f, coef, coef_d, distortion_w, scale_dev, T_threshold,   \
+        loss_sum, opacity_out, rgb_out, dL_dsigmas, (TT*)dL_drgbs, n_rays, bg_rgb, alpha, b_load)
+    if (rgbs_dtype == NGP_F16) {
+        if (dist) NGP_HEAD_RBG(__half, true);
+        else NGP_HEAD_RBG(__half, false);
+    } else {
+        if (dist) NGP_HEAD_RBG(float, true);
+        else NGP_HEAD_RBG(float, false);
+    }
+#undef NGP_HEAD_RBG
     NGP_LAUNCHED("ray_head_fused_kernel");
     return 0;
 }

@@ -34,7 +34,8 @@ def _p(t):
 class StaticTrainStep:
     def __init__(self, trainer, n_rays: int, samples_per_ray_capacity: int = 384, exp_step_factor: float = 0.0,
                  T_threshold: float = 1e-4, max_samples: int = 1024, use_graph: bool = True,
-                 dynamic_loss_scale: bool = True, overlap_optimizer: bool = False, distortion_loss_w: float = 0.0):
+                 dynamic_loss_scale: bool = True, overlap_optimizer: bool = False, distortion_loss_w: float = 0.0,
+                 random_bg: bool = False, bg_seed: int = 0, bg_load: float = 1.0):
         self.tr = trainer
         m = self.model = trainer.model
         # the voxel-grid model: fp32 fields and outputs, no encoder and no MLP; its optimizer pass covers the node
@@ -82,6 +83,12 @@ class StaticTrainStep:
         # optimizer scalars on the device: owned by the trainer, shared with the module path (NGPTrainer.step)
         self.step_dev, self.hyper, self.scale_state = trainer.step_dev, trainer.hyper, trainer.scale_state
         self.sample_step = torch.full((1,), trainer.step_count, device=dev, dtype=i32)   # batches drawn so far
+        # --random_bg (DESIGN.md §6f): per-ray background colours of step s drawn on the device; s = bg_step[0], which
+        # the step's reset launch increments, so s = trainer.step_count after the step (as ops.random_bg is called by
+        # the module path).  alpha stays 1 (target unchanged) when step() gets no alpha.
+        self.random_bg, self.bg_seed, self.bg_load = bool(random_bg), int(bg_seed), float(bg_load)
+        self.bg_step = torch.full((1,), trainer.step_count, device=dev, dtype=i32)
+        self.bg_rgb, self.alpha = (z(self.n, 3), torch.ones(self.n, device=dev)) if self.random_bg else (None, None)
         # GradScaler state on the device: [scale, growth_tracker (int bits)]; growth 2x / 2000 clean steps, backoff 0.5
         trainer.dynamic_loss_scale = self.dynamic_loss_scale = bool(dynamic_loss_scale)
         self.aabb6 = (C.c_float * 6)(*[float(v) for v in m.xyz_min.flatten().tolist()],
@@ -196,6 +203,15 @@ class StaticTrainStep:
         # composite forward + background + MSE [+ distortion loss] + composite backward in one launch (per-ray work)
         bg = 1.0 if self.esf == 0 else 0.0
         ctag = F32 if self.vox else F16
+        if self.random_bg:
+            L, st = load(), self._st()
+            check(L.ngp_random_bg(self.bg_seed & 0xFFFFFFFFFFFFFFFF, _p(self.bg_step), 0, _p(self.bg_rgb), self.n, st))
+            check(L.ngp_ray_head_fused_random_bg(
+                _p(self.sig), _p(self.rgbs), ctag, _p(self.deltas), _p(self.ts), _p(self.rays_a), _p(self.gt),
+                _p(self.bg_rgb), _p(self.alpha), self.bg_load, float(self.tr.loss_scale),
+                _p(self.scale_state) if self.dynamic_loss_scale else None, self.T_thr, self.distortion_w,
+                _p(self.loss_sum), _p(self.opacity), _p(self.rgb), _p(self.dsig), _p(self.drgbs), self.n, st))
+            return
         if self.distortion_w > 0:
             check(load().ngp_ray_head_fused_distortion(
                 _p(self.sig), _p(self.rgbs), ctag, _p(self.deltas), _p(self.ts), _p(self.rays_a), _p(self.gt), bg,
@@ -269,7 +285,8 @@ class StaticTrainStep:
         # (with inf_at_source the flag is raised by the previous backward and cleared by its consumer, the optimizer)
         check(load().ngp_step_reset(_p(self.counter), _p(self.loss_sum),
                                     None if self.inf_at_source else _p(self.tr.found_inf),
-                                    _p(self.sample_step) if sampled else None, self._st()))
+                                    _p(self.sample_step) if sampled else _p(self.bg_step) if self.random_bg else None,
+                                    self._st()))
         if mode == "steady":
             # optimizer of the PREVIOUS step beside this step's ray_aabb + marching.  The marching branch runs on
             # a high-priority stream (the priority is kept by the captured kernel nodes): its latency-bound warps
@@ -292,6 +309,7 @@ class StaticTrainStep:
         tr = self.tr
         keep = [p.data.clone() for p in tr.params] + [tr.exp_avg.clone(), tr.exp_avg_sq.clone(), self.step_dev.clone()]
         scale_keep, hyper_keep, sample_keep = self.scale_state.clone(), self.hyper.clone(), self.sample_step.clone()
+        bg_step_keep = self.bg_step.clone()
         shadow = None if tr._shadow_full is None else tr._shadow_full.clone()
         side = torch.cuda.Stream()
         side.wait_stream(torch.cuda.current_stream())
@@ -314,17 +332,26 @@ class StaticTrainStep:
         self.scale_state.copy_(scale_keep)
         self.hyper.copy_(hyper_keep)
         self.sample_step.copy_(sample_keep)
+        self.bg_step.copy_(bg_step_keep)
         tr.flat_grad.zero_()
         if shadow is not None:
             tr._shadow_full.copy_(shadow)
         self._graphs[(sampled, mode)], self._kernels[(sampled, mode)] = graph, kernels
 
     # ---------------------------------------------------------------------------------------------
-    def step(self, rays_o, rays_d, rgb_gt, noise=None):
-        """Enqueues one full training step; returns the (device) loss tensor — nothing is synchronised."""
+    def step(self, rays_o, rays_d, rgb_gt, noise=None, alpha=None):
+        """Enqueues one full training step; returns the (device) loss tensor — nothing is synchronised.  ``alpha`` [N]
+        (random_bg only): the images' alpha, whose transparent part of the target gets the ray's colour."""
         self.rays_o.copy_(rays_o, non_blocking=True)
         self.rays_d.copy_(rays_d, non_blocking=True)
         self.gt.copy_(rgb_gt, non_blocking=True)
+        if alpha is not None and not self.random_bg:
+            raise ValueError("alpha is read by the random background only (StaticTrainStep(random_bg=True))")
+        if self.random_bg:
+            if alpha is None:
+                self.alpha.fill_(1.0)
+            else:
+                self.alpha.copy_(alpha, non_blocking=True)
         if noise is None:
             self.noise.uniform_()
         else:
@@ -366,6 +393,8 @@ class StaticTrainStep:
         """Keep the training set resident (as the reference's ``train_dataset.to(device)``) and let the step draw
         its own batch: ``step_sampled()`` then needs no per-step input at all.  With several ranks pass a
         different ``seed`` per rank."""
+        if self.random_bg:
+            raise _lib.NgpError("the device-sampled step does not support random_bg yet; use step()")
         f = lambda t: t.detach().to(self.dev, torch.float32).contiguous()  # noqa: E731
         bank, poses, directions = f(image_bank), f(poses), f(directions)
         if bank.ndim != 3 or bank.shape[0] != poses.shape[0] or bank.shape[1] != directions.shape[0] or bank.shape[2] < 3:

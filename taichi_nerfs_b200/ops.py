@@ -277,6 +277,22 @@ def distortion_bwd(dL_dloss, ws, deltas, ts, rays_a):
     return out
 
 
+# ---- --random_bg (DESIGN.md §6f) ----------------------------------------------------------------------
+def random_bg(seed, step, n_rays, device, step_dev=None):
+    """[n_rays, 3] fp32 background colours in [0, 1) of training step ``step`` (or of step_dev[0], an int32 device
+    scalar, when given): Philox4x32-10 keyed by ``seed``, counter (ray, step); the graph-captured step draws the same."""
+    out = torch.empty(int(n_rays), 3, device=device, dtype=torch.float32)
+    if step_dev is not None:
+        _need_cuda(step_dev)
+        if step_dev.dtype != torch.int32:
+            raise TypeError("random_bg: step_dev must be int32")
+    elif out.device.type != 'cuda':
+        raise ValueError("random_bg draws on a CUDA device")
+    check(load().ngp_random_bg(int(seed) & 0xFFFFFFFFFFFFFFFF, _ptr(step_dev) if step_dev is not None else None,
+                               int(step), _ptr(out), int(n_rays), _stream()), "random_bg")
+    return out
+
+
 # ---- test-time evaluation --------------------------------------------------------------------------
 def ssim(pred, target, height, width):
     """SSIM (torchmetrics' StructuralSimilarityIndexMeasure, data_range=1; DESIGN.md §6e) of fp32 images [H*W, 3]

@@ -167,10 +167,16 @@ class NGPTrainer:
             self.encoder.adopt_shadow(None)
         self._views = []
 
-    def forward_backward(self, rays_o, rays_d, rgb_gt, exp_step_factor=0.0, extra_loss=None):
+    def forward_backward(self, rays_o, rays_d, rgb_gt, exp_step_factor=0.0, extra_loss=None, bg_rgb=None, alpha=None,
+                         b_load=1.0):
+        """bg_rgb [N, 3] (--random_bg, ops.random_bg): each ray's background colour replaces the fixed one; with
+        ``alpha`` [N] (the image's alpha), the target's loader background ``b_load`` is replaced by it too:
+        rgb_gt + (bg_rgb - b_load)(1 - alpha)."""
         from modules.rendering import render
+        if bg_rgb is not None and alpha is not None:
+            rgb_gt = rgb_gt + (bg_rgb - b_load) * (1 - alpha)[:, None]
         with torch.autocast(device_type='cuda', dtype=torch.float16):
-            results = render(self.model, rays_o, rays_d, exp_step_factor=exp_step_factor)
+            results = render(self.model, rays_o, rays_d, exp_step_factor=exp_step_factor, bg_rgb=bg_rgb)
             loss = F.mse_loss(results['rgb'], rgb_gt)
             if extra_loss is not None:  # e.g. distortion loss (train.py:194-195)
                 loss = loss + extra_loss(results)
@@ -291,7 +297,8 @@ class NGPTrainer:
         if self._shadow is not None:
             self.encoder.adopt_shadow(self._shadow)
 
-    def step(self, rays_o, rays_d, rgb_gt, exp_step_factor=0.0, extra_loss=None):
-        loss, results = self.forward_backward(rays_o, rays_d, rgb_gt, exp_step_factor, extra_loss)
+    def step(self, rays_o, rays_d, rgb_gt, exp_step_factor=0.0, extra_loss=None, bg_rgb=None, alpha=None, b_load=1.0):
+        loss, results = self.forward_backward(rays_o, rays_d, rgb_gt, exp_step_factor, extra_loss, bg_rgb, alpha,
+                                              b_load)
         self.optimizer_step()
         return loss, results

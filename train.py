@@ -22,7 +22,7 @@ from modules.distortion import distortion_loss
 from modules.networks import MODEL_DICT
 from modules.rendering import MAX_SAMPLES, render
 from modules.utils import depth2img, save_deployment_model
-from opt import get_opts
+from opt import DISK_DATASETS, get_opts
 from taichi_nerfs_b200 import ops
 from taichi_nerfs_b200.trainer import NGPTrainer
 
@@ -68,18 +68,19 @@ def main(prefix_args=None):
     warmup_steps, update_interval = 256, 16
 
     dataset = dataset_dict[hparams.dataset_name]
-    extra = {'scene': 'analytic'} if hparams.dataset_name == 'synthetic' else {}
-    train_dataset = dataset(root_dir=hparams.root_dir, split=hparams.split, downsample=hparams.downsample,
-                            seed=seed, **extra).to(device)
+    if hparams.dataset_name in DISK_DATASETS:   # the reference's arguments only (train.py:61-73)
+        train_dataset = dataset(root_dir=hparams.root_dir, split=hparams.split,
+                                downsample=hparams.downsample).to(device)
+        test_dataset = dataset(root_dir=hparams.root_dir, split='test', downsample=hparams.downsample).to(device)
+    else:
+        extra = {'scene': 'analytic'} if hparams.dataset_name == 'synthetic' else {}
+        train_dataset = dataset(root_dir=hparams.root_dir, split=hparams.split, downsample=hparams.downsample,
+                                seed=seed, **extra).to(device)
+        train_dataset._seed = seed + rank  # different rays per rank
+        test_dataset = dataset(root_dir=hparams.root_dir, split='test', downsample=hparams.downsample,
+                               n_images=4, **extra).to(device)
     train_dataset.batch_size = hparams.batch_size
     train_dataset.ray_sampling_strategy = hparams.ray_sampling_strategy
-    if hparams.random_bg:
-        raise SystemExit("--random_bg applies to real scenes with an alpha channel (datasets/colmap.py of the "
-                         "reference), which are out of scope here (SURVEY.md §2.1)")
-    train_dataset._seed = seed + rank  # different rays per rank
-    test_dataset = dataset(root_dir=hparams.root_dir, split='test', downsample=hparams.downsample,
-                           n_images=4, **extra).to(device)
-
     model_config = build_model_config(hparams)
     model = MODEL_DICT[hparams.model_name](**model_config).to(device)
     if hparams.ckpt_path:
@@ -93,6 +94,8 @@ def main(prefix_args=None):
         voxel_reg = (hparams.tv_sigma_loss_w, hparams.tv_sh_loss_w, hparams.sparsity_loss_w)
     trainer = NGPTrainer(model, lr=hparams.lr, max_steps=hparams.max_steps, voxel_reg=voxel_reg)
 
+    # --random_bg (DESIGN.md §6f): every training ray gets its own background colour, drawn on the device
+    bg_load = getattr(train_dataset, 'bg_load', 1.0)
     fast = None
     if hparams.graph_step:
         if not model._fusable(next(model.parameters())):
@@ -101,7 +104,8 @@ def main(prefix_args=None):
             raise ValueError("--graph_step runs the hash encoder only; train a tri-plane model without it")
         from taichi_nerfs_b200.fast_step import StaticTrainStep
         fast = StaticTrainStep(trainer, hparams.batch_size, exp_step_factor=exp_step_factor,
-                               distortion_loss_w=hparams.distortion_loss_w)
+                               distortion_loss_w=hparams.distortion_loss_w, random_bg=hparams.random_bg,
+                               bg_seed=seed + rank, bg_load=bg_load)
 
     tic = time.time()
     for step in range(hparams.max_steps + 1):
@@ -115,11 +119,15 @@ def main(prefix_args=None):
         if hparams.distortion_loss_w > 0:
             extra_loss = lambda res: hparams.distortion_loss_w * distortion_loss(res).mean()  # noqa: E731
         if fast is not None:   # one graph replay, nothing synchronises the host
-            loss = fast.step(rays_o, rays_d, data['rgb'])
+            loss = fast.step(rays_o, rays_d, data['rgb'], alpha=data.get('alpha') if hparams.random_bg else None)
             results = {'rgb': fast.rgb, 'rm_samples': fast.counter[0].clamp(max=fast.cap), 'vr_samples':
                        fast.counter[0].clamp(max=fast.cap), 'dropped_rays': fast.counter[1]}
         else:
-            loss, results = trainer.step(rays_o, rays_d, data['rgb'], exp_step_factor, extra_loss=extra_loss)
+            bg_rgb = None
+            if hparams.random_bg:   # the colours of step trainer.step_count + 1, as the graph step draws them
+                bg_rgb = ops.random_bg(seed + rank, trainer.step_count + 1, len(rays_o), device)
+            loss, results = trainer.step(rays_o, rays_d, data['rgb'], exp_step_factor, extra_loss=extra_loss,
+                                         bg_rgb=bg_rgb, alpha=data.get('alpha'), b_load=bg_load)
 
         if step % 1000 == 0 and rank == 0:
             with torch.no_grad():
