@@ -52,7 +52,7 @@ int ngp_ray_aabb_intersect_cpu(const float* rays_o, const float* rays_d, float s
             t1 = fmaxf(t1, lo); /* :31 */
             t2 = fminf(t2, hi); /* :32 */
         }
-        if (t2 > 0.0f) { /* :34 */
+        if (t2 > 0.0f && t2 < INFINITY) { /* :34; a ray with no finite far hit (zero or NaN direction) misses */
             hits_t[r * 2 + 0] = fmaxf(t1, NEAR_DISTANCE);
             hits_t[r * 2 + 1] = t2;
         } else {
@@ -73,6 +73,16 @@ static inline float calc_dt(float t, float esf, int grid_size, float scale) { /*
     const float hi = SQRT3_2 * scale / (float)grid_size;
     const float v = t * esf;
     return fminf(fmaxf(v, SQRT3_MAX_SAMPLES), hi);
+}
+
+/* The next march position t + dt, or +inf when the add does not increase t: near t = dt * 2^24 the fp32 sum rounds
+ * back to t, and a NaN t never compares greater.  Every march loop advances only through this, so each iteration
+ * strictly increases a finite t or ends the ray (+inf fails `t < t2` and `tn < t_target`); fp32 has finitely many
+ * values, so every loop ends.  The reference adds unconditionally and loops forever on such rays
+ * (ray_march.py:64,72-74). */
+static inline float march_advance(float t, float dt) {
+    const float tn = t + dt;
+    return tn > t ? tn : INFINITY;
 }
 
 static inline int frexp_bit(float x) { /* utils.py:60-75 */
@@ -166,8 +176,8 @@ static inline int march_step(const march_ctx* c, float* t, float* xyz, float* dt
         tmin = fminf(tmin, tx);
     }
     const float t_target = tt + fmaxf(0.0f, tmin);
-    float tn = tt + calc_dt(tt, c->esf, gs, c->scale);
-    while (tn < t_target) tn += calc_dt(tn, c->esf, gs, c->scale);
+    float tn = march_advance(tt, calc_dt(tt, c->esf, gs, c->scale));
+    while (tn < t_target) tn = march_advance(tn, calc_dt(tn, c->esf, gs, c->scale));
     *t = tn;
     return 0;
 }
@@ -215,7 +225,7 @@ int ngp_raymarching_train_count_cpu(const float* rays_o, const float* rays_d, co
         float xyz[3], dt;
         while (0.0f <= t && t < t2 && n < max_samples) { /* :43 */
             if (march_step(&c, &t, xyz, &dt)) {
-                t += dt;
+                t = march_advance(t, dt);
                 n += 1;
             }
         }
@@ -270,7 +280,7 @@ int ngp_raymarching_train_write_cpu(const float* rays_o, const float* rays_d, co
                 dirs[i * 3 + 2] = c.d[2];
                 ts[i] = t;
                 deltas[i] = dt;
-                t += dt;
+                t = march_advance(t, dt);
                 s += 1;
             }
         }
@@ -304,7 +314,7 @@ int ngp_raymarching_test_cpu(const float* rays_o, const float* rays_d, float* hi
                 valid_mask[i] = 1;
                 ts[i] = t;
                 deltas[i] = dt;
-                t += dt;
+                t = march_advance(t, dt);
                 hits_t[r * 2 + 0] = t; /* :257 */
                 s += 1;
             }
@@ -1012,13 +1022,14 @@ static inline float u2f(uint32_t u) { float x; memcpy(&x, &u, 4); return x; }
 
 /* first position of the sequence t, t+dt, (t+dt)+dt, ... that is >= t_target, taking at least one step */
 static inline float advance_const_dt(float t, float dt, float t_target, int64_t* real_adds) {
-    float tn = t + dt;
+    float tn = march_advance(t, dt);
     *real_adds += 1;
     while (tn < t_target) {
         const uint32_t b = f2u(tn), e = b >> 23; /* tn > 0: no sign bit */
         const float t1 = tn + dt;
         const uint32_t b1 = f2u(t1);
         *real_adds += 1;
+        if (!(t1 > tn)) return INFINITY; /* no progress: the ray ends (march_advance) */
         if ((b1 >> 23) != e) { /* this step leaves the binade */
             tn = t1;
             continue;
@@ -1083,7 +1094,7 @@ int ngp_raymarching_cellstep_cpu(const float* rays_o, const float* rays_d, const
             if (last_occ) {
                 ts[start + n] = t;
                 n += 1;
-                t += dt;
+                t = march_advance(t, dt);
                 adds += 1;
                 continue;
             }
@@ -1161,6 +1172,9 @@ int ngp_raymarching_lanes_cpu(const float* rays_o, const float* rays_d, const fl
                 occ[k] = (density_bitfield[idx >> 3] >> (idx & 7u)) & 1;
                 if (!occ[k] && !ok) regular = 0;
             }
+            int stalled = 0; /* a step that does not advance ends the ray: the sequential loop below handles it */
+            for (int k = 0; k < 32; ++k) stalled |= !(pos[k + 1] > pos[k]);
+            if (stalled) regular = 0;
             if (regular) {
                 n_reg += 1;
                 int k = 0;
@@ -1171,13 +1185,13 @@ int ngp_raymarching_lanes_cpu(const float* rays_o, const float* rays_d, const fl
             } else {
                 /* general path: the reference loop over this chunk's span (may overshoot into the next span) */
                 n_gen += 1;
-                const float t_end = pos[32];
+                const float t_end = stalled ? INFINITY : pos[32];
                 float xyz[3], dts;
                 while (0.0f <= t && t < t2 && n < max_samples && t < t_end) {
                     float tt = t;
                     if (march_step(&c, &tt, xyz, &dts)) {
                         ts[start + n++] = t;
-                        t += dts;
+                        t = march_advance(t, dts);
                     } else {
                         t = tt;
                     }

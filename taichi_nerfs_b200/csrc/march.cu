@@ -20,6 +20,16 @@ __device__ __forceinline__ float calc_dt(float t, float esf, float dt_max) {  //
     return fminf(fmaxf(f_mul(t, esf), kSqrt3MaxSamples), dt_max);
 }
 
+// The next march position t + dt, or +inf when the add does not increase t: near t = dt * 2^24 the fp32 sum rounds
+// back to t, and a NaN t never compares greater.  Every march loop advances only through this (the warp march checks
+// the same condition on its 32-position chain), so each iteration strictly increases a finite t or ends the ray (+inf
+// fails `t < t2` and `tn < t_target`); fp32 has finitely many values, so every loop ends.  The reference adds
+// unconditionally and loops forever on such rays (ray_march.py:64,72-74).
+__device__ __forceinline__ float march_advance(float t, float dt) {
+    const float tn = f_add(t, dt);
+    return tn > t ? tn : INFINITY;
+}
+
 __device__ __forceinline__ int frexp_bit(float x) {  // utils.py:60-75
     int exponent = 0;
     if (x != 0.0f) {
@@ -109,8 +119,8 @@ __device__ __forceinline__ bool march_step(const MarchParams& p, const Ray& ray,
         tmin = fminf(tmin, a);
     }
     const float t_target = f_add(tt, fmaxf(0.0f, tmin));
-    float tn = f_add(tt, calc_dt(tt, p.esf, p.dt_max));
-    while (tn < t_target) tn = f_add(tn, calc_dt(tn, p.esf, p.dt_max));
+    float tn = march_advance(tt, calc_dt(tt, p.esf, p.dt_max));
+    while (tn < t_target) tn = march_advance(tn, calc_dt(tn, p.esf, p.dt_max));
     t = tn;
     return false;
 }
@@ -143,7 +153,7 @@ __global__ void __launch_bounds__(256) ray_aabb_kernel(const float* __restrict__
         t2 = fminf(t2, fmaxf(tmin, tmax));
     }
     float2 out;
-    if (t2 > 0.0f) out = make_float2(fmaxf(t1, kNear), t2);
+    if (t2 > 0.0f && t2 < INFINITY) out = make_float2(fmaxf(t1, kNear), t2);
     else out = make_float2(-1.0f, -1.0f);
     reinterpret_cast<float2*>(hits_t)[r] = out;
 }
@@ -305,7 +315,13 @@ __device__ __forceinline__ void march_one_ray(const float* __restrict__ rays_o, 
                 tk = f_add(tk, dk);
             }
         }
-        const bool valid = my_t < t2;
+        // progress: position k+1 is reached only if every step up to it increased t (a step that does not stays put
+        // forever, so the positions after the first stall repeat it and are not on the ray: march_advance)
+        const float t_down = __shfl_down_sync(full, my_t, 1);   // every lane takes part: outside the select below
+        const float t_next = lane < 31 ? t_down : tk;
+        const unsigned stall_mask = __ballot_sync(full, !(t_next > my_t));
+        const unsigned reach = stall_mask ? (2u << (__ffs(stall_mask) - 1)) - 1u : full;
+        const bool valid = my_t < t2 && ((reach >> lane) & 1u);
         const CellTest c = test_cell(p, ray, my_t, my_dt);
         const unsigned valid_mask = __ballot_sync(full, valid);
         const unsigned occ_mask = __ballot_sync(full, valid && c.occ);
@@ -383,11 +399,11 @@ __device__ __forceinline__ void march_one_ray(const float* __restrict__ rays_o, 
             // budget of this round used up: the march resumes at the position after the last emitted sample
             // (occupied -> `t += dt`, ray_march.py:258-262), i.e. the next lane's position or the next chunk's first
             const int q = 31 - __clz(emit);
-            const float nx = __shfl_sync(full, my_t, min(q + 1, 31));
-            t_resume = q < 31 ? nx : tk;
+            const float nx = __shfl_sync(full, t_next, q);
+            t_resume = ((stall_mask >> q) & 1u) ? INFINITY : nx;
             break;
         }
-        if (valid_mask != full) break;  // the ray left the box inside this chunk
+        if (valid_mask != full || stall_mask) break;  // the ray left the box or stopped advancing inside this chunk
         t = tk;
     }
     if (kMode == 0 && lane == 0) {
@@ -555,7 +571,7 @@ __global__ void __launch_bounds__(128) march_test_kernel(const float* __restrict
             valid_mask[i] = 1;
             ts[i] = t;
             deltas[i] = dt;
-            t = f_add(t, dt);
+            t = march_advance(t, dt);
             t_resume = t;
             s += 1;
         }

@@ -42,8 +42,13 @@ MARCH_CFGS = [
     dict(scale=0.5, cascades=1, esf=0.0, occ="random"),
     dict(scale=16.0, cascades=6, esf=1 / 256, occ="random"),
     dict(scale=2.0, cascades=3, esf=1 / 256, occ="sparse"),
+    dict(scale=8.0, cascades=5, esf=1 / 256, occ="random"),     # the scale README.md ships for real scenes
+    dict(scale=1.5, cascades=3, esf=1 / 256, occ="random"),     # top cascade bound 1.5 (not a power of two)
+    dict(scale=3.0, cascades=4, esf=1 / 256, occ="sparse"),     # top cascade bound 3
+    dict(scale=64.0, cascades=8, esf=1 / 256, occ="random"),
 ]
-MARCH_IDS = ["lego", "random", "6casc_esf", "3casc_sparse"]
+MARCH_IDS = ["lego", "random", "6casc_esf", "3casc_sparse", "5casc_scale8", "3casc_scale1.5", "4casc_scale3",
+             "8casc_scale64"]
 
 
 def _march_inputs(cfg, n, seed, rng, rays_factory, lego_bitfield):
@@ -115,14 +120,20 @@ def test_march_train_empty_and_overflow(ops, oracle, rays_factory, lego_bitfield
 
 
 # ---- a3 -------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("max_samples", [1, 4, 64])
-def test_march_test_bit_exact(ops, oracle, rays_factory, lego_bitfield, max_samples):
+# the Lego configuration keeps its ids (the max_samples alone); every other configuration at two chunk sizes
+MARCH_TEST_CASES = [pytest.param(MARCH_CFGS[0], m, id=str(m)) for m in (1, 4, 64)] + [
+    pytest.param(c, m, id=f"{i}-{m}") for c, i in zip(MARCH_CFGS[1:], MARCH_IDS[1:]) for m in (4, 64)]
+
+
+@pytest.mark.parametrize("cfg,max_samples", MARCH_TEST_CASES)
+def test_march_test_bit_exact(ops, oracle, rays_factory, lego_bitfield, cfg, max_samples):
     n = 3001
-    o, d = rays_factory(n, seed=23)
-    hits = oracle.ray_aabb_intersect(o, d, 0.5)
+    o, d, bits = _march_inputs(cfg, n, 23, np.random.default_rng(23), rays_factory, lego_bitfield)
+    sc, casc, esf = cfg["scale"], cfg["cascades"], cfg["esf"]
+    hits = oracle.ray_aabb_intersect(o, d, sc)
     alive = np.random.default_rng(23).permutation(n)[: n // 2].astype(np.int64)
     h_ref = hits.copy()
-    ri, valid, dl, tt, cnt = oracle.raymarching_test(o, d, h_ref, alive, lego_bitfield, 1, 0.5, 0.0, 128, max_samples)
+    ri, valid, dl, tt, cnt = oracle.raymarching_test(o, d, h_ref, alive, bits, casc, sc, esf, 128, max_samples)
     h_gpu = T(hits)
     A, m = alive.shape[0], max_samples
     g_ri = torch.zeros(A * m, device=DEV, dtype=torch.long)
@@ -130,7 +141,7 @@ def test_march_test_bit_exact(ops, oracle, rays_factory, lego_bitfield, max_samp
     g_dl = torch.zeros(A * m, device=DEV)
     g_tt = torch.zeros(A * m, device=DEV)
     g_cnt = torch.zeros(A, device=DEV, dtype=torch.int32)
-    ops.raymarching_test(T(o), T(d), h_gpu, T(alive), T(lego_bitfield), 1, 0.5, 0.0, 128, m, g_ri, g_valid, g_dl, g_tt, g_cnt)
+    ops.raymarching_test(T(o), T(d), h_gpu, T(alive), T(bits), casc, sc, esf, 128, m, g_ri, g_valid, g_dl, g_tt, g_cnt)
     assert np.array_equal(N(g_cnt), cnt)
     assert np.array_equal(N(g_valid), valid)
     v = valid.astype(bool)
@@ -613,7 +624,7 @@ def test_hash_index_known_answers_cuda(ops, max_res):
 
 # ---- f1: fused occupancy-grid update ---------------------------------------------------------------------------
 @pytest.mark.parametrize("warmup", [True, False])
-@pytest.mark.parametrize("cascades,scale", [(1, 0.5), (3, 2.0)])
+@pytest.mark.parametrize("cascades,scale", [(1, 0.5), (3, 2.0), (5, 8.0), (3, 1.5)])
 def test_fused_grid_update_matches_oracle(ops, oracle, warmup, cascades, scale):
     """Cell pick + jittered positions (networks.py:168-209, 263-271): bit-exact vs the oracle restatement (same Philox
     draws); scatter-max + EMA-max + mean + packbits (:272-290): grid bit-exact, mean within 1 fp32 ulp, bitfield equal."""
