@@ -578,6 +578,31 @@ int ngp_adam_step_p2p(float* param, void* const* grad_peers, float* exp_avg, flo
                       float beta1, float beta2, float eps, int64_t own_begin, int64_t own_end, int64_t rep_begin,
                       int64_t rep_end, void* stream);
 
+/* ---- mesh export (DESIGN.md §6g) --------------------------------------------------------------------------------
+ * The density lattice has n nodes per axis (2 <= n <= 1024) over [-bound, bound]^3: spacing s = f_div(2 bound, n - 1),
+ * node i at f_add(-bound, f_mul((float)i, s)); lattice[(ix * n + iy) * n + iz], fp32.
+ * ngp_mesh_lattice_points: world positions xyz [count, 3] of nodes [start, start + count) in linear order, and occ
+ * [count] = 1 where the node lies in an occupied cell of density_bitfield by the marcher's position rule (march.cu,
+ * march_step, cascade from max|x| alone).  0 < bound <= scale.
+ * ngp_mesh_lattice_store: lattice[start + j] = occ[j] && isfinite(sigma[j]) ? sigma[j] : 0. */
+int ngp_mesh_lattice_points(int64_t n, float bound, int64_t start, int64_t count, const uint8_t* density_bitfield,
+                            int cascades, int grid_size, float scale, float* xyz, uint8_t* occ, void* stream);
+int ngp_mesh_lattice_store(const float* sigma, const uint8_t* occ, int64_t start, int64_t count, float* lattice,
+                           void* stream);
+/* Marching cubes over an fp32 lattice at a finite threshold (inside: value > threshold), four launches in order,
+ * no atomics (the output is unique).  workspace: ngp_mc_workspace_bytes(n) bytes (-1: bad n).
+ * ngp_mc_count: per tile, its vertex and face counts.  ngp_mc_scan: totals[0] = V, totals[1] = F (device int64[2]).
+ * ngp_mc_emit_vertices: vertices / normals [V, 3] in edge-id order (node_linear * 3 + axis), vbase [n^3] int32 the
+ * first vertex id of each node that owns one.  ngp_mc_emit_faces: faces [F, 3] int32 in cell order, counter-clockwise
+ * seen from outside.  V and F must be < 2^31 (checked before anything is written). */
+int64_t ngp_mc_workspace_bytes(int64_t n);
+int ngp_mc_count(const float* lattice, int64_t n, float threshold, void* workspace, void* stream);
+int ngp_mc_scan(int64_t n, void* workspace, int64_t* totals, void* stream);
+int ngp_mc_emit_vertices(const float* lattice, int64_t n, float threshold, float bound, void* workspace,
+                         int64_t n_vertices, int32_t* vbase, float* vertices, float* normals, void* stream);
+int ngp_mc_emit_faces(const float* lattice, int64_t n, float threshold, void* workspace, const int32_t* vbase,
+                      int64_t n_faces, int32_t* faces, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

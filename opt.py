@@ -64,6 +64,12 @@ _FLAGS = [
                                'the default module path')),
     ('--deployment', dict(action='store_true', default=False)),
     ('--deployment_model_path', dict(type=str, default='./')),
+    # mesh export (DESIGN.md §6g)
+    ('--extract_mesh', dict(action='store_true', default=False,
+                            help='after evaluation, write results/mesh.ply: marching cubes over the density lattice')),
+    ('--mesh_res', dict(type=int, default=512, help='lattice nodes per axis of the mesh export, in [2, 1024]')),
+    ('--mesh_threshold', dict(type=float, default=10.0, help='density above which a lattice node is inside the mesh')),
+    ('--mesh_bound', dict(type=float, default=0.0, help='half-width of the meshed cube, in (0, scale]; 0 means scale')),
 ]
 
 _VOXEL_REG_FLAGS = ('tv_sigma_loss_w', 'tv_sh_loss_w', 'sparsity_loss_w')
@@ -75,6 +81,12 @@ def get_opts(prefix_args=None):
     for flag, kw in _FLAGS:
         parser.add_argument(flag, **kw)
     hparams = parser.parse_args(prefix_args)
+    if not 2 <= hparams.mesh_res <= 1024:
+        parser.error(f"--mesh_res must be in [2, 1024], got {hparams.mesh_res}")
+    if not math.isfinite(hparams.mesh_threshold):
+        parser.error(f"--mesh_threshold must be finite, got {hparams.mesh_threshold}")
+    if not (hparams.mesh_bound == 0 or (math.isfinite(hparams.mesh_bound) and 0 < hparams.mesh_bound <= hparams.scale)):
+        parser.error(f"--mesh_bound must be 0 (meaning --scale) or in (0, {hparams.scale}], got {hparams.mesh_bound}")
     if hparams.dataset_name in DISK_DATASETS and not hparams.root_dir:
         parser.error(f"--dataset_name {hparams.dataset_name} reads a dataset from disk: it needs --root_dir")
     for flag in _VOXEL_REG_FLAGS:

@@ -112,6 +112,13 @@ def _declare(lib):
         "ngp_grid_workspace_bytes": (i64, [ci, ci]),
         "ngp_grid_sample_cells": (ci, [vp, ci, ci, f32, f32, ci, i64, C.c_uint64, C.c_uint32, vp, vp, vp, vp]),
         "ngp_grid_update": (ci, [vp, vp, vp, i64, ci, ci, vp, f32, f32, vp, vp, vp, vp]),
+        "ngp_mesh_lattice_points": (ci, [i64, f32, i64, i64, vp, ci, ci, f32, vp, vp, vp]),
+        "ngp_mesh_lattice_store": (ci, [vp, vp, i64, i64, vp, vp]),
+        "ngp_mc_workspace_bytes": (i64, [i64]),
+        "ngp_mc_count": (ci, [vp, i64, f32, vp, vp]),
+        "ngp_mc_scan": (ci, [i64, vp, vp, vp]),
+        "ngp_mc_emit_vertices": (ci, [vp, i64, f32, f32, vp, i64, vp, vp, vp, vp]),
+        "ngp_mc_emit_faces": (ci, [vp, i64, f32, vp, vp, i64, vp, vp]),
     }
     for name, (res, args) in sigs.items():
         fn = getattr(lib, name)  # AttributeError if the symbol is missing: fail loudly

@@ -9,6 +9,7 @@
 // count -> single-CTA scan -> write, giving a deterministic, ray-ordered sample layout without
 // the global atomics (ray_march.py:76-81) or the n_rays*1024-row scratch (ray_march.py:149-168).
 #include "common.cuh"
+#include "occupancy.cuh"
 
 namespace {
 
@@ -30,29 +31,6 @@ __device__ __forceinline__ float march_advance(float t, float dt) {
     return tn > t ? tn : INFINITY;
 }
 
-__device__ __forceinline__ int frexp_bit(float x) {  // utils.py:60-75
-    int exponent = 0;
-    if (x != 0.0f) {
-        uint32_t bits = __float_as_uint(x);
-        exponent = (int)((bits & 0x7f800000u) >> 23) - 127;
-        bits = (bits & 0x7fffffu) | 0x3f800000u;
-        const float frac = __uint_as_float(bits);
-        if (frac < 0.5f) exponent -= 1;
-        else if (frac > 1.0f) exponent += 1;
-    }
-    return exponent;
-}
-
-__device__ __forceinline__ uint32_t expand_bits(uint32_t v) {  // utils.py:95-100
-    v = (v * 0x00010001u) & 0xFF0000FFu;
-    v = (v * 0x00000101u) & 0x0F00F00Fu;
-    v = (v * 0x00000011u) & 0xC30C30C3u;
-    v = (v * 0x00000005u) & 0x49249249u;
-    return v;
-}
-__device__ __forceinline__ uint32_t morton3d(uint32_t x, uint32_t y, uint32_t z) {
-    return expand_bits(x) | (expand_bits(y) << 1) | (expand_bits(z) << 2);
-}
 __device__ __forceinline__ float fsign(float v) { return v > 0.0f ? 1.0f : (v < 0.0f ? -1.0f : 0.0f); }
 
 struct Ray {

@@ -8,6 +8,7 @@ PyTorch is plumbing (allocation, streams); all arithmetic happens in the CUDA li
 from __future__ import annotations
 
 import ctypes as C
+import math
 
 import torch
 
@@ -311,6 +312,98 @@ def ssim(pred, target, height, width):
     out = torch.empty(n, device=p.device, dtype=torch.float32)
     check(load().ngp_ssim(_ptr(p), _ptr(t), n, h, w, _ptr(partial), _ptr(out), _stream()), "ssim")
     return out
+
+
+# ---- mesh export (DESIGN.md §6g) --------------------------------------------------------------------------------
+def mesh_lattice_points(n, bound, start, count, bitfield, cascades, grid_size, scale):
+    """World positions [count, 3] fp32 of lattice nodes [start, start + count) and their occupancy [count] uint8 (1:
+    the node lies in an occupied cell by the marcher's position rule)."""
+    _need_cuda(bitfield)
+    xyz = torch.empty(int(count), 3, device=bitfield.device, dtype=torch.float32)
+    occ = torch.empty(int(count), device=bitfield.device, dtype=torch.uint8)
+    check(load().ngp_mesh_lattice_points(int(n), float(bound), int(start), int(count), _ptr(bitfield), int(cascades),
+                                         int(grid_size), float(scale), _ptr(xyz), _ptr(occ), _stream()),
+          "mesh_lattice_points")
+    return xyz, occ
+
+
+def mesh_lattice_store(sigma, occ, start, lattice):
+    """lattice.view(-1)[start + j] = sigma[j] where occ[j] and sigma[j] is finite, else 0."""
+    _need_cuda(sigma, occ, lattice)
+    s = _f32c(sigma.reshape(-1))
+    if occ.dtype != torch.uint8 or lattice.dtype != torch.float32 or not lattice.is_contiguous():
+        raise TypeError("mesh_lattice_store: occ must be uint8 and lattice contiguous fp32")
+    if s.numel() != occ.numel() or int(start) + s.numel() > lattice.numel():
+        raise ValueError("mesh_lattice_store: sizes do not match the lattice")
+    check(load().ngp_mesh_lattice_store(_ptr(s), _ptr(occ), int(start), s.numel(), _ptr(lattice), _stream()),
+          "mesh_lattice_store")
+
+
+class McStages:
+    """The four marching-cubes launches of one fp32 lattice, so that each can be timed on its own; marching_cubes runs
+    them in order."""
+
+    def __init__(self, lattice, threshold, bound):
+        _need_cuda(lattice)
+        if lattice.dtype != torch.float32:
+            raise TypeError("marching_cubes takes an fp32 lattice")
+        n = lattice.shape[0]
+        if lattice.dim() != 3 or tuple(lattice.shape) != (n, n, n) or not 2 <= n <= 1024:
+            raise ValueError(f"marching_cubes expects an [N, N, N] lattice with 2 <= N <= 1024, got "
+                             f"{tuple(lattice.shape)}")
+        if not math.isfinite(threshold):
+            raise ValueError(f"marching_cubes: the threshold must be finite, got {threshold}")
+        if not (math.isfinite(bound) and bound > 0):
+            raise ValueError(f"marching_cubes: the bound must be finite and > 0, got {bound}")
+        self.lattice = lattice.contiguous()
+        self.n, self.threshold, self.bound = n, float(threshold), float(bound)
+        dev = lattice.device
+        self.workspace = torch.empty(int(load().ngp_mc_workspace_bytes(n)), device=dev, dtype=torch.uint8)
+        self.totals = torch.zeros(2, device=dev, dtype=torch.int64)
+        self.vbase = None
+
+    def count(self):
+        check(load().ngp_mc_count(_ptr(self.lattice), self.n, self.threshold, _ptr(self.workspace), _stream()),
+              "mc_count")
+
+    def scan(self):
+        check(load().ngp_mc_scan(self.n, _ptr(self.workspace), _ptr(self.totals), _stream()), "mc_scan")
+
+    def sizes(self):
+        """(V, F), read back to the host: the one synchronisation of the extraction."""
+        v, f = (int(x) for x in self.totals.cpu())
+        if v >= 2 ** 31 or f >= 2 ** 31:
+            raise _lib.NgpError(f"marching_cubes: {v} vertices and {f} faces; both must stay below 2^31")
+        return v, f
+
+    def emit_vertices(self, n_vertices, vertices, normals):
+        if self.vbase is None:
+            self.vbase = torch.empty(self.n ** 3, device=self.lattice.device, dtype=torch.int32)
+        check(load().ngp_mc_emit_vertices(_ptr(self.lattice), self.n, self.threshold, self.bound,
+                                          _ptr(self.workspace), int(n_vertices), _ptr(self.vbase), _ptr(vertices),
+                                          _ptr(normals), _stream()), "mc_emit_vertices")
+
+    def emit_faces(self, n_faces, faces):
+        check(load().ngp_mc_emit_faces(_ptr(self.lattice), self.n, self.threshold, _ptr(self.workspace),
+                                       _ptr(self.vbase), int(n_faces), _ptr(faces), _stream()), "mc_emit_faces")
+
+
+def marching_cubes(lattice, threshold, bound):
+    """Marching cubes over an fp32 CUDA lattice [N, N, N] (indexed [ix, iy, iz], z fastest) spanning [-bound, bound]^3:
+    (vertices [V, 3] fp32, normals [V, 3] fp32 unit, outward = toward lower values, faces [F, 3] int32 counter-clockwise
+    seen from outside).  A node is inside when its value > threshold.  No mask, no model: DESIGN.md §6g."""
+    st = McStages(lattice, threshold, bound)
+    st.count()
+    st.scan()
+    nv, nf = st.sizes()
+    dev = lattice.device
+    vertices = torch.empty(nv, 3, device=dev, dtype=torch.float32)
+    normals = torch.empty(nv, 3, device=dev, dtype=torch.float32)
+    faces = torch.empty(nf, 3, device=dev, dtype=torch.int32)
+    st.emit_vertices(nv, vertices, normals)
+    st.emit_faces(nf, faces)
+    st.vbase = None
+    return vertices, normals, faces
 
 
 # ---- occupancy grid helpers ------------------------------------------------------------------------

@@ -2,7 +2,8 @@
 seeds (:39-42), model_config (:86-117), mark_invisible_cells (:129), loss scale 2**16 | 2**19 (:137-141),
 Adam(lr, eps=1e-15) + cosine annealing to lr/30 (:143-163), density-grid update every 16 steps with a
 256-step warm-up (:57-58,178-182), log line every 1000 steps (:203-219), results/model.pth (:232-235),
-test-split PSNR and SSIM (:237-304).  The step body runs on the sm_90a kernels through NGPTrainer (fused Adam,
+test-split PSNR and SSIM (:237-304); with --extract_mesh, results/mesh.ply after the evaluation (DESIGN.md §6g).
+The step body runs on the sm_90a kernels through NGPTrainer (fused Adam,
 no host sync for the inf check); under torchrun every rank trains on its own rays and the gradients are summed
 once per step: by the peer-memory optimizer kernel when all ranks share one NVLink box, else by an fp16 NCCL
 all-reduce of the flat gradient buffer.
@@ -40,6 +41,14 @@ def build_model_config(hparams):
                 'rgb_net_depth': 1}
     return {'scale': hparams.scale, 'pos_encoder_type': hparams.encoder_type,
             'max_res': 1024 if hparams.scale == 0.5 else 4096, 'half_opt': hparams.half_opt}
+
+
+def save_mesh(model, hparams, path):
+    """Marching cubes of the model's density lattice (--mesh_res, --mesh_threshold, --mesh_bound) written as PLY."""
+    from taichi_nerfs_b200.mesh import extract_mesh, write_ply
+    mesh = extract_mesh(model, hparams.mesh_res, hparams.mesh_threshold, hparams.mesh_bound)
+    write_ply(path, mesh)
+    print(f"mesh: {len(mesh.vertices)} vertices, {len(mesh.faces)} faces -> {path}")
 
 
 def psnr_of(mse):
@@ -168,6 +177,8 @@ def main(prefix_args=None):
     if psnrs:
         ssim_avg = float(torch.cat(ssims).double().mean())
         print(f"evaluation: psnr_avg={sum(psnrs) / len(psnrs)} | ssim_avg={ssim_avg}")
+    if hparams.extract_mesh:
+        save_mesh(model, hparams, os.path.join(val_dir, 'mesh.ply'))
 
     if hparams.gui:
         from gui import NGPGUI
