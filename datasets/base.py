@@ -7,6 +7,10 @@ Other splits return the pose of view ``idx`` and, when the split has images, its
 ``rays`` is [N, H*W, 3], or [N, H*W, 4] when an image had an alpha channel: the fourth column is the resized alpha,
 and ``rgb`` (the reference's value) stays ``rays[..., :3]``; samples then also carry ``alpha``.  ``bg_load`` is the
 colour the loader blended transparent pixels onto (1 white, 0 black), which ``--random_bg`` replaces.
+
+A loader that reads depth (the ngp loader's ``depth_path``, DESIGN.md §6h) sets ``depths`` [N, H*W] fp32 z-depth, 0
+where there is none; samples then also carry ``depth``, indexed as ``rgb`` is.  Loaders without depth set nothing and
+their samples are unchanged.
 """
 from __future__ import annotations
 
@@ -50,6 +54,8 @@ class BaseDataset(Dataset):
         self.poses = self.poses.to(device)
         self.K = self.K.to(device)
         self.directions = self.directions.to(device)
+        if getattr(self, 'depths', None) is not None:
+            self.depths = self.depths.to(device)
         return self
 
     def __getitem__(self, idx):
@@ -65,11 +71,15 @@ class BaseDataset(Dataset):
             rays = self.rays[img_idxs, pix_idxs]
             sample = {'img_idxs': img_idxs, 'pix_idxs': pix_idxs, 'pose': self.poses[img_idxs],
                       'direction': self.directions[pix_idxs], 'rgb': rays[:, :3]}
+            if getattr(self, 'depths', None) is not None:
+                sample['depth'] = self.depths[img_idxs, pix_idxs]
         else:
             sample = {'pose': self.poses[idx], 'img_idxs': idx}
             if len(self.rays) > 0:
                 rays = self.rays[idx]
                 sample['rgb'] = rays[:, :3]
+                if getattr(self, 'depths', None) is not None:
+                    sample['depth'] = self.depths[idx]
             else:
                 return sample
         if rays.shape[-1] == 4:

@@ -43,8 +43,10 @@ def analytic_scene(x):
 
 
 @torch.no_grad()
-def render_teacher(rays_o, rays_d, n_samples: int = 192, scale: float = 0.5):
-    """Quadrature volume rendering of `analytic_scene` on a white background (synthetic-scene convention)."""
+def render_teacher(rays_o, rays_d, n_samples: int = 192, scale: float = 0.5, return_depth: bool = False):
+    """Quadrature volume rendering of `analytic_scene` on a white background (synthetic-scene convention).  With
+    ``return_depth`` also the quadrature's expected depth sum_k w_k t_k (no background term): z-depth, since ``rays_d``
+    is the unnormalised camera-frame direction (u', v', 1) rotated to the world."""
     inv = 1.0 / rays_d
     t0 = ((-scale - rays_o) * inv)
     t1 = ((scale - rays_o) * inv)
@@ -60,13 +62,13 @@ def render_teacher(rays_o, rays_d, n_samples: int = 192, scale: float = 0.5):
     T = torch.cumprod(torch.cat([torch.ones_like(alpha[:, :1]), 1 - alpha + 1e-10], 1), 1)[:, :-1]
     w = alpha * T * hit[:, None]
     out = (w[..., None] * rgb).sum(1) + (1 - w.sum(1))[:, None]
-    return out
+    return (out, (w * t).sum(1)) if return_depth else out
 
 
 class SyntheticLego:
     def __init__(self, n_images: int = 100, img_wh=(800, 800), focal: float = 1111.111, radius: float = 1.4,
                  split: str = 'train', batch_size: int = 8192, seed: int = 23, with_rgb: bool = True,
-                 scene: str = 'random', root_dir: str = '', downsample: float = 1.0, **_):
+                 scene: str = 'random', root_dir: str = '', downsample: float = 1.0, with_depth: bool = False, **_):
         w, h = int(img_wh[0] * downsample), int(img_wh[1] * downsample)
         focal = focal * downsample
         if split != 'train' and not split.startswith('train'):
@@ -83,6 +85,10 @@ class SyntheticLego:
         self.rays = None
         self._seed = seed
         self.with_rgb = with_rgb
+        # with_depth (the analytic scene): samples also carry 'depth', the teacher's expected z-depth (DESIGN.md §6h)
+        if with_depth and scene != 'analytic':
+            raise ValueError("SyntheticLego: with_depth needs scene='analytic' (the random scene has no geometry)")
+        self.with_depth = with_depth
 
     def __len__(self):
         return len(self.poses)
@@ -139,7 +145,10 @@ class SyntheticLego:
                 if self.scene == 'analytic':
                     from .ray_utils import get_rays
                     o, d = get_rays(sample['direction'], sample['pose'])
-                    sample['rgb'] = render_teacher(o, d)
+                    if self.with_depth:
+                        sample['rgb'], sample['depth'] = render_teacher(o, d, return_depth=True)
+                    else:
+                        sample['rgb'] = render_teacher(o, d)
                 else:
                     sample['rgb'] = torch.rand(n, 3, device=dev, generator=self._gen)
             return sample
@@ -147,6 +156,10 @@ class SyntheticLego:
         if self.scene == 'analytic':
             from .ray_utils import get_rays
             o, d = get_rays(self.directions, self.poses[idx])
-            sample['rgb'] = torch.cat([render_teacher(o[i:i + 65536], d[i:i + 65536])
-                                       for i in range(0, o.shape[0], 65536)])
+            parts = [render_teacher(o[i:i + 65536], d[i:i + 65536], return_depth=self.with_depth)
+                     for i in range(0, o.shape[0], 65536)]
+            if self.with_depth:
+                sample['rgb'], sample['depth'] = (torch.cat(p) for p in zip(*parts))
+            else:
+                sample['rgb'] = torch.cat(parts)
         return sample

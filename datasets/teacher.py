@@ -40,30 +40,36 @@ def load_teacher(device):
 
 
 @torch.no_grad()
-def render_views(model, directions, poses, T_threshold=1e-2):
-    """[n_views, H*W, 3] fp32 images of ``model`` (white background) for (3,4) camera-to-world ``poses``."""
+def render_views(model, directions, poses, T_threshold=1e-2, return_depth=False):
+    """[n_views, H*W, 3] fp32 images of ``model`` (white background) for (3,4) camera-to-world ``poses``; with
+    ``return_depth`` also [n_views, H*W] fp32 the render's expected z-depth sum_k w_k t_k."""
     from modules.rendering import render
-    out = []
+    out, dep = [], []
     for pose in poses:
         rays_o, rays_d = get_rays(directions, pose)
         with torch.autocast('cuda', dtype=torch.float16):
             res = render(model, rays_o, rays_d, test_time=True, T_threshold=T_threshold, exp_step_factor=0.0)
         out.append(res['rgb'].float().clamp(0, 1))
-    return torch.stack(out)
+        dep.append(res['depth'].float())
+    return (torch.stack(out), torch.stack(dep)) if return_depth else torch.stack(out)
 
 
 class TeacherLego(SyntheticLego):
     """``SyntheticLego`` geometry with target colours rendered from the shipped Lego model."""
 
-    def __init__(self, n_images: int = 48, radius: float = 1.396, **kw):
+    def __init__(self, n_images: int = 48, radius: float = 1.396, with_depth: bool = False, **kw):
         kw.pop('scene', None)
         super().__init__(n_images=n_images, radius=radius, scene='teacher', **kw)
         self.images = None            # [n_images, H*W, 3] once rendered (needs the GPU)
+        self.with_depth = with_depth  # samples also carry 'depth', the teacher render's z-depth (DESIGN.md §6h)
+        self.depths = None            # [n_images, H*W] once rendered, with_depth only
 
     def to(self, device):
         super().to(device)
         if self.images is not None:
             self.images = self.images.to(device)
+        if self.depths is not None:
+            self.depths = self.depths.to(device)
         return self
 
     def build_image_bank(self, teacher=None):
@@ -73,7 +79,10 @@ class TeacherLego(SyntheticLego):
             if teacher is None:
                 raise FileNotFoundError("teacher model not staged: run __graft_entry__.build(), "
                                         "or set NGP_TEACHER_DIR to a folder with the six .bin files")
-            self.images = render_views(teacher, self.directions, self.poses)
+            if self.with_depth:
+                self.images, self.depths = render_views(teacher, self.directions, self.poses, return_depth=True)
+            else:
+                self.images = render_views(teacher, self.directions, self.poses)
         self.rays = self.images
         return self.rays
 
@@ -83,6 +92,12 @@ class TeacherLego(SyntheticLego):
         dev = self.poses.device
         if self.split.startswith('train'):
             img, pix = self._draw(idx, self.batch_size, dev)
-            return {'img_idxs': img, 'pix_idxs': pix, 'pose': self.poses[img], 'direction': self.directions[pix],
-                    'rgb': self.images[img, pix]}
-        return {'pose': self.poses[idx], 'img_idxs': idx, 'rgb': self.images[idx]}
+            sample = {'img_idxs': img, 'pix_idxs': pix, 'pose': self.poses[img], 'direction': self.directions[pix],
+                      'rgb': self.images[img, pix]}
+            if self.with_depth:
+                sample['depth'] = self.depths[img, pix]
+            return sample
+        sample = {'pose': self.poses[idx], 'img_idxs': idx, 'rgb': self.images[idx]}
+        if self.with_depth:
+            sample['depth'] = self.depths[idx]
+        return sample

@@ -403,6 +403,21 @@ int ngp_ray_head_fused_random_bg(const float* sigmas, const void* rgbs, int rgbs
                                  const float* alpha, float b_load, float loss_scale, const float* scale_dev,
                                  float T_threshold, float distortion_w, float* loss_sum, float* opacity_out,
                                  float* rgb_out, float* dL_dsigmas, void* dL_drgbs, int64_t n_rays, void* stream);
+/* The fused head with depth supervision (--depth_loss_w, DESIGN.md §6h): the loss gains
+ * depth_w (1 / n_rays) sum_r v_r (D_r - depth_gt[r])^2, D_r = sum_k w_k t_k over the ray's composited samples (the depth
+ * of ngp_composite_train_fwd, no background term), v_r = 1 where depth_gt[r] is finite and > 0, else 0 (0 means "no
+ * depth here").  Its dL/dD_r = depth_w 2 v_r (D_r - depth_gt[r]) / n_rays, times the loss scale, enters the composite
+ * backward as dL_ddepth does in ngp_composite_train_bwd; the colours get no gradient from it.  *loss_sum accumulates
+ * the other heads' sum plus 3 depth_w sum_r v_r (D_r - depth_gt[r])^2, so loss_sum / (3 n_rays) stays the total loss.
+ * depth_gt [n_rays] is indexed by ray id and required; depth_w >= 0, and 0 computes exactly what the head without it
+ * computes.  The other arguments are those of ngp_ray_head_fused_random_bg, with bg_rgb == NULL meaning the constant
+ * background bg (alpha must then be NULL); ts is required. */
+int ngp_ray_head_fused_depth(const float* sigmas, const void* rgbs, int rgbs_dtype, const float* deltas, const float* ts,
+                             const int32_t* rays_a, const float* gt, float bg, const float* bg_rgb, const float* alpha,
+                             float b_load, float loss_scale, const float* scale_dev, float T_threshold,
+                             float distortion_w, const float* depth_gt, float depth_w, float* loss_sum,
+                             float* opacity_out, float* rgb_out, float* dL_dsigmas, void* dL_drgbs, int64_t n_rays,
+                             void* stream);
 
 /* ---- distortion loss (SURVEY §8f rank 3) -------------------------------------- */
 /* replaces prefix_sums_kernel + _loss_kernel + distortion_loss_fw_kernel

@@ -38,6 +38,9 @@ _FLAGS = [
                                                           '(svox only)')),
     # loss parameters
     ('--distortion_loss_w', dict(type=float, default=0, help='weight of distortion loss, 0 to disable (default)')),
+    ('--depth_loss_w', dict(type=float, default=0.,
+                            help='weight of the depth loss w mean(v (D - D^)^2) against per-ray target z-depth, 0 to '
+                                 'disable (default); needs a dataset with depth: ngp (depth_path), synthetic, teacher')),
     ('--tv_sigma_loss_w', dict(type=float, default=0., help='weight of the total-variation loss on the voxel grid\'s '
                                                            'density, 0 to disable (default; svox only)')),
     ('--tv_sh_loss_w', dict(type=float, default=0., help='weight of the total-variation loss on the voxel grid\'s sh '
@@ -95,6 +98,11 @@ def get_opts(prefix_args=None):
             parser.error(f"--{flag} must be finite and >= 0, got {w}")
         if w != 0 and hparams.model_name != 'svox':
             parser.error(f"--{flag} regularises the voxel grid: it needs --model_name svox")
+    if not (math.isfinite(hparams.depth_loss_w) and hparams.depth_loss_w >= 0):
+        parser.error(f"--depth_loss_w must be finite and >= 0, got {hparams.depth_loss_w}")
+    if hparams.depth_loss_w > 0 and hparams.dataset_name in ('nerf', 'nsvf', 'colmap'):
+        parser.error(f"--depth_loss_w: the {hparams.dataset_name} loader reads no depth (the ngp loader reads "
+                     f"transforms.json's depth_path)")
     if hparams.model_name == 'svox':
         for flag, bad, why in (
                 ('encoder_type', hparams.encoder_type == 'triplane',

@@ -81,6 +81,8 @@ def _declare(lib):
         "ngp_random_bg": (ci, [C.c_uint64, vp, i32, vp, i64, vp]),
         "ngp_ray_head_fused_random_bg": (ci, [vp, vp, ci, vp, vp, vp, vp, vp, vp, f32, f32, vp, f32, f32, vp, vp, vp,
                                               vp, vp, i64, vp]),
+        "ngp_ray_head_fused_depth": (ci, [vp, vp, ci, vp, vp, vp, vp, f32, vp, vp, f32, f32, vp, f32, f32, vp, f32, vp,
+                                          vp, vp, vp, vp, i64, vp]),
         "ngp_distortion_fwd": (ci, [vp, vp, vp, vp, vp, i64, i64, vp]),
         "ngp_distortion_bwd": (ci, [vp, vp, vp, vp, vp, vp, i64, i64, vp]),
         "ngp_ssim": (ci, [vp, vp, i64, ci, ci, vp, vp, vp]),

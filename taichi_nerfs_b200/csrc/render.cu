@@ -309,7 +309,12 @@ __global__ void __launch_bounds__(256) mse_loss_grad_kernel(const float* __restr
 // kRandBg (--random_bg, DESIGN.md §6f): the background is the ray's own colour c_r = bg_rgb[ray] instead of the
 // constant bg; where the image had an alpha channel (alpha != nullptr) the target's loader background b_load is swapped
 // for c_r: gt' = gt + (c_r - b_load)(1 - a).  dL/dopacity = -sum_c c_r,c g_c.
-template <typename T, bool kDist, bool kRandBg = false>
+//
+// kDepth (--depth_loss_w, DESIGN.md §6h) adds w_z (1 / n_rays) sum_r v_r (D_r - D^_r)^2 with D_r = sum_k w_k t_k the
+// ray's expected depth and D^_r = depth_gt[ray]; v_r = 1 where D^_r is finite and > 0, else 0.  Its dL/dD_r =
+// coef_z v_r (D_r - D^_r), coef_z = scale 2 w_z / n_rays, enters G_k as dL_ddepth t_k does in
+// composite_train_bwd_kernel.
+template <typename T, bool kDist, bool kRandBg = false, bool kDepth = false>
 __global__ void __launch_bounds__(kWarpsPerBlock * 32)
 ray_head_fused_kernel(const float* __restrict__ sigmas, const T* __restrict__ rgbs, const float* __restrict__ deltas,
                       const float* __restrict__ ts, const int32_t* __restrict__ rays_a, const float* __restrict__ gt,
@@ -317,7 +322,8 @@ ray_head_fused_kernel(const float* __restrict__ sigmas, const T* __restrict__ rg
                       float* __restrict__ loss_sum, float* __restrict__ opacity_out, float* __restrict__ rgb_out,
                       float* __restrict__ dsigmas, T* __restrict__ drgbs, int64_t n_rays,
                       const float* __restrict__ bg_rgb = nullptr, const float* __restrict__ alpha = nullptr,
-                      float b_load = 0.0f) {
+                      float b_load = 0.0f, const float* __restrict__ depth_gt = nullptr, float coef_z = 0.0f,
+                      float w_z = 0.0f) {
     __shared__ float Tstart_s[kWarpsPerBlock][kChunkCap];
     __shared__ float Wstart_s[kDist ? kWarpsPerBlock : 1][kDist ? kChunkCap : 1];   // W_<k at every chunk start
     __shared__ float WTstart_s[kDist ? kWarpsPerBlock : 1][kDist ? kChunkCap : 1];  // WT_<k at every chunk start
@@ -327,6 +333,7 @@ ray_head_fused_kernel(const float* __restrict__ sigmas, const T* __restrict__ rg
     if (scale_dev != nullptr) {
         coef *= *scale_dev;
         if constexpr (kDist) coef_d *= *scale_dev;
+        if constexpr (kDepth) coef_z *= *scale_dev;
     }
     const int64_t ray = rays_a[n * 3 + 0], start = rays_a[n * 3 + 1];
     const int N = rays_a[n * 3 + 2];
@@ -339,6 +346,7 @@ ray_head_fused_kernel(const float* __restrict__ sigmas, const T* __restrict__ rg
     int last_chunk = -1;
     float r = 0.f, g = 0.f, b = 0.f, op = 0.f;
     float dist = 0.f;  // kDist: this lane's share of loss_ray
+    float dep = 0.f;   // kDepth: this lane's share of D
     {
         float Tc = 1.0f;
         float Wc = 0.f, WTc = 0.f;  // kDist: W_<k, WT_<k at the chunk start
@@ -354,6 +362,7 @@ ray_head_fused_kernel(const float* __restrict__ sigmas, const T* __restrict__ rg
                     a = 1.0f - expf(-sigmas[s] * dl);
                 } else {
                     a = 1.0f - expf(-sigmas[s] * deltas[s]);
+                    if constexpr (kDepth) tm = ts[s];
                 }
                 c0 = load_as_float(rgbs, s * 3 + 0);
                 c1 = load_as_float(rgbs, s * 3 + 1);
@@ -369,6 +378,7 @@ ray_head_fused_kernel(const float* __restrict__ sigmas, const T* __restrict__ rg
             g += w * c1;
             b += w * c2;
             op += w;
+            if constexpr (kDepth) dep += w * tm;
             if constexpr (kDist) {
                 const float wt = w * tm;
                 const float wi = warp_scan_add(w, lane), wti = warp_scan_add(wt, lane);
@@ -432,10 +442,23 @@ ray_head_fused_kernel(const float* __restrict__ sigmas, const T* __restrict__ rg
     if constexpr (kRandBg) go = -(bc0 * gr + bc1 * gg + bc2 * gb);
     else go = -bg * (gr + gg + gb);
     if constexpr (kDist) dist = warp_sum(dist);
+    float gz = 0.f, lz = 0.f;  // kDepth: dL/dD (scaled) and v (D - D^)^2
+    if constexpr (kDepth) {
+        dep = warp_sum(dep);
+        const float dh = depth_gt[ray];
+        if (dh > 0.0f && dh < INFINITY) {  // NaN fails both
+            const float dd = dep - dh;
+            lz = dd * dd;
+            gz = coef_z * dd;
+        }
+    }
     if (lane == 0) {
-        // kDist: loss_sum / (3 n_rays) = mse + w_d mean(loss_ray)
-        if constexpr (kDist) atomicAdd(loss_sum, d0 * d0 + d1 * d1 + d2 * d2 + 3.0f * w_d * dist);
-        else atomicAdd(loss_sum, d0 * d0 + d1 * d1 + d2 * d2);
+        // kDist: loss_sum / (3 n_rays) = mse + w_d mean(loss_ray); kDepth adds w_z mean(v (D - D^)^2)
+        float l;
+        if constexpr (kDist) l = d0 * d0 + d1 * d1 + d2 * d2 + 3.0f * w_d * dist;
+        else l = d0 * d0 + d1 * d1 + d2 * d2;
+        if constexpr (kDepth) l += 3.0f * w_z * lz;
+        atomicAdd(loss_sum, l);
         if (opacity_out) opacity_out[ray] = op;
         if (rgb_out) {
             rgb_out[ray * 3 + 0] = r + k0;
@@ -445,8 +468,8 @@ ray_head_fused_kernel(const float* __restrict__ sigmas, const T* __restrict__ rg
     }
     __syncwarp();
 
-    // backward: exact reverse suffix accumulation (same as composite_train_bwd_kernel with g_depth = 0, and g_ws = 0
-    // or the distortion term)
+    // backward: exact reverse suffix accumulation (same as composite_train_bwd_kernel with g_depth = 0 or the depth
+    // term, and g_ws = 0 or the distortion term)
     float suffix = 0.0f;
     float sW = 0.f, sWT = 0.f;  // kDist: sums of w and w t over the later chunks
     for (int c = last_chunk; c >= 0; --c) {
@@ -495,7 +518,7 @@ ray_head_fused_kernel(const float* __restrict__ sigmas, const T* __restrict__ rg
             c0 = load_as_float(rgbs, s * 3 + 0);
             c1 = load_as_float(rgbs, s * 3 + 1);
             c2v = load_as_float(rgbs, s * 3 + 2);
-            if constexpr (kDist) tm = ts[s];
+            if constexpr (kDist || kDepth) tm = ts[s];
         }
         const float incl = warp_scan_mul(1.0f - a, lane);
         float excl = __shfl_up_sync(0xffffffffu, incl, 1);
@@ -528,6 +551,7 @@ ray_head_fused_kernel(const float* __restrict__ sigmas, const T* __restrict__ rg
             sW += __shfl_sync(0xffffffffu, rw, 0);
             sWT += __shfl_sync(0xffffffffu, rwt, 0);
         }
+        if constexpr (kDepth) G += gz * tm;
         const float wG = w * G;
         float rs = wG;
 #pragma unroll
@@ -895,6 +919,53 @@ int ngp_ray_head_fused_random_bg(const float* sigmas, const void* rgbs, int rgbs
         else NGP_HEAD_RBG(float, false);
     }
 #undef NGP_HEAD_RBG
+    NGP_LAUNCHED("ray_head_fused_kernel");
+    return 0;
+}
+
+int ngp_ray_head_fused_depth(const float* sigmas, const void* rgbs, int rgbs_dtype, const float* deltas, const float* ts,
+                             const int32_t* rays_a, const float* gt, float bg, const float* bg_rgb, const float* alpha,
+                             float b_load, float loss_scale, const float* scale_dev, float T_threshold,
+                             float distortion_w, const float* depth_gt, float depth_w, float* loss_sum,
+                             float* opacity_out, float* rgb_out, float* dL_dsigmas, void* dL_drgbs, int64_t n_rays,
+                             void* stream) {
+    NGP_REQUIRE(n_rays >= 0, "negative n_rays");
+    NGP_REQUIRE(rgbs_dtype == NGP_F32 || rgbs_dtype == NGP_F16, "bad dtype");
+    NGP_REQUIRE(distortion_w >= 0.0f && distortion_w < INFINITY, "distortion_w must be finite and >= 0");
+    NGP_REQUIRE(depth_w >= 0.0f && depth_w < INFINITY, "depth_w must be finite and >= 0");
+    NGP_REQUIRE(bg_rgb || !alpha, "alpha is read with bg_rgb only");
+    if (n_rays == 0) return 0;
+    NGP_REQUIRE(sigmas && rgbs && deltas && ts && rays_a && gt && depth_gt && loss_sum && dL_dsigmas && dL_drgbs,
+                "null pointer");
+    const float scale = scale_dev ? 1.0f : loss_scale;
+    const float coef = scale * 2.0f / (3.0f * (float)n_rays);
+    const float coef_d = scale * distortion_w / (float)n_rays;
+    const float coef_z = scale * 2.0f * depth_w / (float)n_rays;   // d(w_z mean(v (D - D^)^2)) / d(D - D^) / v
+    const unsigned grid = (unsigned)((n_rays + kWarpsPerBlock - 1) / kWarpsPerBlock);
+    cudaStream_t st = ngp::as_stream(stream);
+    // depth_w == 0 runs the depth-free instantiation: the result of ngp_ray_head_fused_{distortion,random_bg}
+    const bool dist = distortion_w > 0.0f, rbg = bg_rgb != nullptr, depth = depth_w > 0.0f;
+#define NGP_HEAD_Z(TT, DD, RB, ZZ)                                                                                  \
+    ray_head_fused_kernel<TT, DD, RB, ZZ><<<grid, kWarpsPerBlock * 32, 0, st>>>(                                    \
+        sigmas, (const TT*)rgbs, deltas, ts, rays_a, gt, RB ? 0.0f : bg, coef, coef_d, distortion_w, scale_dev,      \
+        T_threshold, loss_sum, opacity_out, rgb_out, dL_dsigmas, (TT*)dL_drgbs, n_rays, bg_rgb, alpha, b_load,      \
+        depth_gt, coef_z, depth_w)
+#define NGP_HEAD_Z_RB(TT, DD, ZZ)        \
+    if (rbg) NGP_HEAD_Z(TT, DD, true, ZZ); \
+    else NGP_HEAD_Z(TT, DD, false, ZZ)
+#define NGP_HEAD_Z_DD(TT, ZZ)                  \
+    if (dist) { NGP_HEAD_Z_RB(TT, true, ZZ); } \
+    else { NGP_HEAD_Z_RB(TT, false, ZZ); }
+    if (rgbs_dtype == NGP_F16) {
+        if (depth) { NGP_HEAD_Z_DD(__half, true) }
+        else { NGP_HEAD_Z_DD(__half, false) }
+    } else {
+        if (depth) { NGP_HEAD_Z_DD(float, true) }
+        else { NGP_HEAD_Z_DD(float, false) }
+    }
+#undef NGP_HEAD_Z_DD
+#undef NGP_HEAD_Z_RB
+#undef NGP_HEAD_Z
     NGP_LAUNCHED("ray_head_fused_kernel");
     return 0;
 }

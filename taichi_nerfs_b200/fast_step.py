@@ -5,7 +5,7 @@ the C-ABI kernels, enqueued in a fixed order on fixed buffers:
 
   [ray-batch sampler] -> ray_aabb -> single-pass march (capacity buffers, one atomic row reservation per ray) ->
   hash (or tri-plane) fwd (+AABB normalisation) -> fused MLP fwd -> fused per-ray head (composite fwd + background + MSE
-  [+ distortion loss] + composite bwd) -> MLP bwd -> hash (or tri-plane) bwd -> [gradient exchange] -> check_finite -> device-side LR/bias-correction update
+  [+ distortion loss] [+ depth loss] + composite bwd) -> MLP bwd -> hash (or tri-plane) bwd -> [gradient exchange] -> check_finite -> device-side LR/bias-correction update
   -> fused Adam (+fp16 shadow, grad zero) -> device-side GradScaler update
 
 A voxel-grid model (--model_name svox) has no network: the march feeds the voxel forward (fp32 sigma / rgb) -> head ->
@@ -35,7 +35,7 @@ class StaticTrainStep:
     def __init__(self, trainer, n_rays: int, samples_per_ray_capacity: int = 384, exp_step_factor: float = 0.0,
                  T_threshold: float = 1e-4, max_samples: int = 1024, use_graph: bool = True,
                  dynamic_loss_scale: bool = True, overlap_optimizer: bool = False, distortion_loss_w: float = 0.0,
-                 random_bg: bool = False, bg_seed: int = 0, bg_load: float = 1.0):
+                 random_bg: bool = False, bg_seed: int = 0, bg_load: float = 1.0, depth_loss_w: float = 0.0):
         self.tr = trainer
         m = self.model = trainer.model
         # the voxel-grid model: fp32 fields and outputs, no encoder and no MLP; its optimizer pass covers the node
@@ -56,6 +56,10 @@ class StaticTrainStep:
         self.distortion_w = float(distortion_loss_w)
         if not self.distortion_w >= 0.0 or self.distortion_w == float("inf"):
             raise ValueError(f"distortion_loss_w must be finite and >= 0, got {distortion_loss_w}")
+        # weight of the depth loss (train.py --depth_loss_w, DESIGN.md §6h): loss += w * mean(v (D - D^)^2)
+        self.depth_w = float(depth_loss_w)
+        if not self.depth_w >= 0.0 or self.depth_w == float("inf"):
+            raise ValueError(f"depth_loss_w must be finite and >= 0, got {depth_loss_w}")
         # fp16 embeddings (the --half_opt hash encoder): the MLP kernels run their fp16-embedding instantiations
         self.half = not self.vox and enc.emb_dtype == torch.float16
         edt = torch.float16 if self.half else torch.float32
@@ -89,6 +93,7 @@ class StaticTrainStep:
         self.random_bg, self.bg_seed, self.bg_load = bool(random_bg), int(bg_seed), float(bg_load)
         self.bg_step = torch.full((1,), trainer.step_count, device=dev, dtype=i32)
         self.bg_rgb, self.alpha = (z(self.n, 3), torch.ones(self.n, device=dev)) if self.random_bg else (None, None)
+        self.depth_gt = z(self.n) if self.depth_w > 0 else None   # per-ray target z-depth, 0 = none
         # GradScaler state on the device: [scale, growth_tracker (int bits)]; growth 2x / 2000 clean steps, backoff 0.5
         trainer.dynamic_loss_scale = self.dynamic_loss_scale = bool(dynamic_loss_scale)
         self.aabb6 = (C.c_float * 6)(*[float(v) for v in m.xyz_min.flatten().tolist()],
@@ -200,12 +205,22 @@ class StaticTrainStep:
                                 _p(self.mlp_save), self.cap, _p(self.counter), st))
 
     def _k_head(self):
-        # composite forward + background + MSE [+ distortion loss] + composite backward in one launch (per-ray work)
+        # composite forward + background + MSE [+ distortion loss] [+ depth loss] + composite backward in one launch
+        # (per-ray work)
         bg = 1.0 if self.esf == 0 else 0.0
         ctag = F32 if self.vox else F16
         if self.random_bg:
             L, st = load(), self._st()
             check(L.ngp_random_bg(self.bg_seed & 0xFFFFFFFFFFFFFFFF, _p(self.bg_step), 0, _p(self.bg_rgb), self.n, st))
+        if self.depth_w > 0:
+            check(load().ngp_ray_head_fused_depth(
+                _p(self.sig), _p(self.rgbs), ctag, _p(self.deltas), _p(self.ts), _p(self.rays_a), _p(self.gt), bg,
+                _p(self.bg_rgb), _p(self.alpha), self.bg_load, float(self.tr.loss_scale),
+                _p(self.scale_state) if self.dynamic_loss_scale else None, self.T_thr, self.distortion_w,
+                _p(self.depth_gt), self.depth_w, _p(self.loss_sum), _p(self.opacity), _p(self.rgb), _p(self.dsig),
+                _p(self.drgbs), self.n, self._st()))
+            return
+        if self.random_bg:
             check(L.ngp_ray_head_fused_random_bg(
                 _p(self.sig), _p(self.rgbs), ctag, _p(self.deltas), _p(self.ts), _p(self.rays_a), _p(self.gt),
                 _p(self.bg_rgb), _p(self.alpha), self.bg_load, float(self.tr.loss_scale),
@@ -339,9 +354,16 @@ class StaticTrainStep:
         self._graphs[(sampled, mode)], self._kernels[(sampled, mode)] = graph, kernels
 
     # ---------------------------------------------------------------------------------------------
-    def step(self, rays_o, rays_d, rgb_gt, noise=None, alpha=None):
+    def step(self, rays_o, rays_d, rgb_gt, noise=None, alpha=None, depth=None):
         """Enqueues one full training step; returns the (device) loss tensor — nothing is synchronised.  ``alpha`` [N]
-        (random_bg only): the images' alpha, whose transparent part of the target gets the ray's colour."""
+        (random_bg only): the images' alpha, whose transparent part of the target gets the ray's colour.  ``depth`` [N]
+        (depth_loss_w > 0 only, where it is required): each ray's target z-depth, 0 where there is none."""
+        if depth is None and self.depth_w > 0:
+            raise ValueError("depth_loss_w > 0 needs each ray's target depth: step(..., depth=...)")
+        if depth is not None and self.depth_w == 0:
+            raise ValueError("depth is read by the depth loss only (StaticTrainStep(depth_loss_w=...))")
+        if depth is not None:
+            self.depth_gt.copy_(depth, non_blocking=True)
         self.rays_o.copy_(rays_o, non_blocking=True)
         self.rays_d.copy_(rays_d, non_blocking=True)
         self.gt.copy_(rgb_gt, non_blocking=True)
@@ -395,6 +417,8 @@ class StaticTrainStep:
         different ``seed`` per rank."""
         if self.random_bg:
             raise _lib.NgpError("the device-sampled step does not support random_bg yet; use step()")
+        if self.depth_w > 0:
+            raise _lib.NgpError("the device-sampled step does not support depth supervision yet; use step(depth=...)")
         f = lambda t: t.detach().to(self.dev, torch.float32).contiguous()  # noqa: E731
         bank, poses, directions = f(image_bank), f(poses), f(directions)
         if bank.ndim != 3 or bank.shape[0] != poses.shape[0] or bank.shape[1] != directions.shape[0] or bank.shape[2] < 3:

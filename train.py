@@ -3,6 +3,7 @@ seeds (:39-42), model_config (:86-117), mark_invisible_cells (:129), loss scale 
 Adam(lr, eps=1e-15) + cosine annealing to lr/30 (:143-163), density-grid update every 16 steps with a
 256-step warm-up (:57-58,178-182), log line every 1000 steps (:203-219), results/model.pth (:232-235),
 test-split PSNR and SSIM (:237-304); with --extract_mesh, results/mesh.ply after the evaluation (DESIGN.md §6g).
+With --depth_loss_w the loss gains the depth term (DESIGN.md §6h) and a test split with depth reports depth_mae.
 The step body runs on the sm_90a kernels through NGPTrainer (fused Adam,
 no host sync for the inf check); under torchrun every rank trains on its own rays and the gradients are summed
 once per step: by the peer-memory optimizer kernel when all ranks share one NVLink box, else by an fp16 NCCL
@@ -19,6 +20,7 @@ import torch.nn.functional as F
 
 from datasets import dataset_dict
 from datasets.ray_utils import get_rays
+from modules.depth import depth_loss, depth_valid
 from modules.distortion import distortion_loss
 from modules.networks import MODEL_DICT
 from modules.rendering import MAX_SAMPLES, render
@@ -83,6 +85,8 @@ def main(prefix_args=None):
         test_dataset = dataset(root_dir=hparams.root_dir, split='test', downsample=hparams.downsample).to(device)
     else:
         extra = {'scene': 'analytic'} if hparams.dataset_name == 'synthetic' else {}
+        if hparams.depth_loss_w > 0:
+            extra['with_depth'] = True
         train_dataset = dataset(root_dir=hparams.root_dir, split=hparams.split, downsample=hparams.downsample,
                                 seed=seed, **extra).to(device)
         train_dataset._seed = seed + rank  # different rays per rank
@@ -114,7 +118,7 @@ def main(prefix_args=None):
         from taichi_nerfs_b200.fast_step import StaticTrainStep
         fast = StaticTrainStep(trainer, hparams.batch_size, exp_step_factor=exp_step_factor,
                                distortion_loss_w=hparams.distortion_loss_w, random_bg=hparams.random_bg,
-                               bg_seed=seed + rank, bg_load=bg_load)
+                               bg_seed=seed + rank, bg_load=bg_load, depth_loss_w=hparams.depth_loss_w)
 
     tic = time.time()
     for step in range(hparams.max_steps + 1):
@@ -124,11 +128,21 @@ def main(prefix_args=None):
             if step % update_interval == 0:
                 model.update_density_grid(0.01 * MAX_SAMPLES / 3 ** 0.5, warmup=step < warmup_steps)
         rays_o, rays_d = get_rays(data['direction'], data['pose'])
-        extra_loss = None
+        depth = None
+        if hparams.depth_loss_w > 0:
+            depth = data.get('depth')
+            if depth is None:
+                raise ValueError(f"--depth_loss_w: the {hparams.dataset_name} dataset at {hparams.root_dir!r} has no "
+                                 f"depth (an ngp scene needs depth_path frames)")
+        terms = []
         if hparams.distortion_loss_w > 0:
-            extra_loss = lambda res: hparams.distortion_loss_w * distortion_loss(res).mean()  # noqa: E731
+            terms.append(lambda res: hparams.distortion_loss_w * distortion_loss(res).mean())
+        if depth is not None:
+            terms.append(lambda res: hparams.depth_loss_w * depth_loss(res, depth).mean())
+        extra_loss = (lambda res: sum(f(res) for f in terms)) if terms else None  # noqa: E731
         if fast is not None:   # one graph replay, nothing synchronises the host
-            loss = fast.step(rays_o, rays_d, data['rgb'], alpha=data.get('alpha') if hparams.random_bg else None)
+            loss = fast.step(rays_o, rays_d, data['rgb'], alpha=data.get('alpha') if hparams.random_bg else None,
+                             depth=depth)
             results = {'rgb': fast.rgb, 'rm_samples': fast.counter[0].clamp(max=fast.cap), 'vr_samples':
                        fast.counter[0].clamp(max=fast.cap), 'dropped_rays': fast.counter[1]}
         else:
@@ -158,7 +172,7 @@ def main(prefix_args=None):
     # test loop (train.py:237-304): PSNR and SSIM per held-out view; first view saved as PNG
     model.eval()
     w, h = test_dataset.img_wh
-    psnrs, ssims = [], []
+    psnrs, ssims, depth_maes = [], [], []
     with torch.no_grad():
         for i in range(len(test_dataset)):
             td = test_dataset[i]
@@ -168,6 +182,10 @@ def main(prefix_args=None):
             if 'rgb' in td:
                 psnrs.append(float(psnr_of(F.mse_loss(results['rgb'].float(), td['rgb']))))
                 ssims.append(ops.ssim(results['rgb'].float(), td['rgb'], h, w))
+            if 'depth' in td:   # mean |D - D^| over the view's pixels with a target
+                v = depth_valid(td['depth'])
+                if bool(v.any()):
+                    depth_maes.append(float((results['depth'].float() - td['depth'])[v].abs().mean()))
             if i == 0:
                 from PIL import Image
                 img = (results['rgb'].float().clamp(0, 1).reshape(h, w, 3).cpu().numpy() * 255).astype(np.uint8)
@@ -176,7 +194,8 @@ def main(prefix_args=None):
                     os.path.join(val_dir, 'depth_000.png'))
     if psnrs:
         ssim_avg = float(torch.cat(ssims).double().mean())
-        print(f"evaluation: psnr_avg={sum(psnrs) / len(psnrs)} | ssim_avg={ssim_avg}")
+        print(f"evaluation: psnr_avg={sum(psnrs) / len(psnrs)} | ssim_avg={ssim_avg}"
+              + (f" | depth_mae={sum(depth_maes) / len(depth_maes)}" if depth_maes else ""))
     if hparams.extract_mesh:
         save_mesh(model, hparams, os.path.join(val_dir, 'mesh.ply'))
 
