@@ -283,6 +283,7 @@ int ngp_hash_bwd_level_groups(const ngp_hash_layout* layout, int level_begin, in
                               int32_t* bounds);
 int ngp_mlp_fwd_dyn(const void* emb, int emb_dtype, const float* dirs, const ngp_mlp_weights* w, float* sigmas,
                     void* rgbs_f16, void* save, int64_t n_max, const int32_t* n_dev, void* stream);
+/* found_inf_or_null: set to 1 when the weight gradient or a row of dL/demb below the device count is not finite. */
 int ngp_mlp_bwd_dyn(const void* emb, int emb_dtype, const float* dirs, const ngp_mlp_weights* w, const void* save,
                     const float* dsigmas, const void* drgbs_f16, void* demb, float* grad_w, int64_t n_max,
                     const int32_t* n_dev, int32_t* found_inf_or_null, void* stream);

@@ -86,7 +86,8 @@ __device__ __forceinline__ uint32_t load_pair(const uint8_t* buf, int K, int row
     return *reinterpret_cast<const uint32_t*>(buf + chunk_off(row, col >> 3, K) + (col & 7) * 2);
 }
 // backward hidden epilogue: fp16(D) masked by relu'(act) (act = the post-ReLU forward activation, a [64 x 64]
-// buffer), as select semantics like threshold_backward -> fragments + the dst buffer
+// buffer), as select semantics like threshold_backward -> fragments + the dst buffer.  threshold_backward zeroes the
+// gradient where act <= 0, so a NaN activation passes it (unordered compare), as in torch
 __device__ __forceinline__ void relu_bwd_frags(const float* d, const uint8_t* act, uint8_t* dst, int r0, int t,
                                                uint32_t (*f)[4]) {
 #pragma unroll
@@ -95,7 +96,7 @@ __device__ __forceinline__ void relu_bwd_frags(const float* d, const uint8_t* ac
         for (int q = 0; q < 4; ++q) {
             const uint32_t a = load_pair(act, 64, r0 + 8 * (q & 1), 16 * kk + 8 * (q >> 1) + 2 * t);
             f[kk][q] = pack_h2(d[8 * kk + 2 * q], d[8 * kk + 2 * q + 1]) &
-                       __hgt2_mask(*reinterpret_cast<const __half2*>(&a), __float2half2_rn(0.0f));
+                       __hgtu2_mask(*reinterpret_cast<const __half2*>(&a), __float2half2_rn(0.0f));
         }
         store_frag(dst, 64, kk, f[kk], r0, t);
     }
@@ -308,6 +309,7 @@ __global__ void __launch_bounds__(kThreads, 2) mlp_bwd_kernel(const TEmb* __rest
 #pragma unroll
     for (int j = 0; j < 4; ++j) gW5T[j] = 0.f;
 
+    bool bad = false;   // a non-finite dL/demb or weight gradient (GradScaler's inf check, raised at the source)
     const int64_t n_tiles = (n + kTile - 1) / kTile;
     uint4 cur[2];
     load_emb(emb, (int64_t)blockIdx.x * kTile + srow, (int64_t)blockIdx.x * kTile + srow < n, q2, cur);
@@ -499,8 +501,10 @@ __global__ void __launch_bounds__(kThreads, 2) mlp_bwd_kernel(const TEmb* __rest
 #pragma unroll
             for (int j = 0; j < 4; ++j) {
                 const float a = a32[4 * j + 2 * k], b = a32[4 * j + 2 * k + 1];
+                const uint32_t p = pack_h2(a, b);
+                bad = bad || (p & 0x7c00u) == 0x7c00u || (p & 0x7c000000u) == 0x7c000000u;   // fp16 inf / NaN
                 if constexpr (sizeof(TEmb) == 2) {
-                    *reinterpret_cast<uint32_t*>(demb + ii[k] * 32 + 8 * j + 2 * t) = pack_h2(a, b);
+                    *reinterpret_cast<uint32_t*>(demb + ii[k] * 32 + 8 * j + 2 * t) = p;
                 } else {   // fp16-rounded like the autocast graph, stored as fp32
                     *reinterpret_cast<float2*>(demb + ii[k] * 32 + 8 * j + 2 * t) = make_float2(r16(a), r16(b));
                 }
@@ -511,7 +515,6 @@ __global__ void __launch_bounds__(kThreads, 2) mlp_bwd_kernel(const TEmb* __rest
 
     // ---- flush the weight-gradient accumulators: thread element 4j + 2k + c is (row r0 + 8k, column 8j + 2t + c)
     if ((int64_t)blockIdx.x >= n_tiles) return;
-    bool bad = false;   // non-finite weight gradient (GradScaler's inf check, raised at the source)
     constexpr int o2 = NGP_MLP_W1, o3 = o2 + NGP_MLP_W2, o4 = o3 + NGP_MLP_W3, o5 = o4 + NGP_MLP_W4;
     flush_acc<64>(gW4, r0, t, bad, [&](int m, int c) { return grad_w + o4 + m * 64 + c; });
     flush_acc<32>(gW3, r0, t, bad, [&](int m, int c) { return grad_w + o3 + m * 32 + c; });

@@ -83,6 +83,17 @@ def test_mlp_bwd_v2_equals_v1(n):
     """Backward restarting from the saved activations (v2) against recomputing the whole forward (v1): the saved h and
     fp16 rgb are exactly what the recompute produces, so dL/dE is bit-identical; the weight gradients are per-CTA
     register sums flushed with fp32 atomics, whose order may differ between launches."""
+    _bwd_v2_equals_v1(n, "xavier")
+
+
+@pytest.mark.parametrize("n", [128, 129, 5000, 148 * 3 * 128 + 1, 300 * 128 * 2 + 77])
+def test_mlp_bwd_v2_equals_v1_trained(n):
+    """The same on the finite regimes of tests/mlp_tolerance.py::trained_inputs, where a saved rgb rounded otherwise
+    than the recompute's shows on the saturated channels, and the TruncExp clamp on both sides of +-15."""
+    _bwd_v2_equals_v1(n, "trained")
+
+
+def _bwd_v2_equals_v1(n, magnitude):
     from taichi_nerfs_b200 import ops
     rng = np.random.default_rng(n)
     emb = T(rng.standard_normal((n, 32)).astype(np.float16))
@@ -90,6 +101,10 @@ def test_mlp_bwd_v2_equals_v1(n):
     ws = [T(w) for w in _weights(rng)]
     dsig = T((rng.standard_normal(n) * 1e-2).astype(np.float32))
     drgb = T((rng.standard_normal((n, 3)) * 1e-2).astype(np.float16))
+    if magnitude == "trained":
+        from mlp_tolerance import trained_inputs
+        emb, dirs, ws, dsig, drgb = [T(a) if not isinstance(a, list) else [T(w) for w in a]
+                                     for a in trained_inputs(n, n)[:5]]
     _, _, save = ops.mlp_fwd(emb, dirs, ws, with_save=True)
     de1, gw1 = ops.mlp_bwd(emb, dirs, ws, dsig, drgb)
     de2, gw2 = ops.mlp_bwd(emb, dirs, ws, dsig, drgb, save=save)

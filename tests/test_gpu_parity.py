@@ -246,10 +246,25 @@ def _weights(rng):
 @pytest.mark.parametrize("emb_half", [True, False])
 @pytest.mark.parametrize("n", [1, 128, 1000, 70001])
 def test_mlp_fwd_tcgen05_matches_oracle(ops, oracle, emb_half, n):
+    _mlp_fwd_matches_oracle(ops, oracle, emb_half, n, "xavier")
+
+
+@pytest.mark.parametrize("emb_half", [True, False])
+@pytest.mark.parametrize("n", [1, 128, 1000, 70001])
+def test_mlp_fwd_tcgen05_matches_oracle_trained(ops, oracle, emb_half, n):
+    """The same comparison on the finite regimes of tests/mlp_tolerance.py::trained_inputs (h0 beyond and within an
+    ulp16 of +-15, |h0| in 8..11, fp16 sigmoid exactly 0 / 1) at the first / last row and on 64-row tile edges."""
+    _mlp_fwd_matches_oracle(ops, oracle, emb_half, n, "trained")
+
+
+def _mlp_fwd_matches_oracle(ops, oracle, emb_half, n, magnitude):
     rng = np.random.default_rng(29)
     emb = rng.standard_normal((n, 32)).astype(np.float16 if emb_half else np.float32)
     dirs = rng.standard_normal((n, 3)).astype(np.float32)
     ws = _weights(rng)
+    if magnitude == "trained":
+        from mlp_tolerance import trained_inputs
+        emb, dirs, ws, _, _, _ = trained_inputs(n, 29, np.float16 if emb_half else np.float32)
     sig_ref, rgb_ref = oracle.mlp_fwd(emb, dirs, ws)
     sig, rgb = ops.mlp_fwd(T(emb), T(dirs), [T(w) for w in ws])
     sig, rgb = N(sig), N(rgb).astype(np.float32)
@@ -395,12 +410,30 @@ def test_adam_fused(ops, oracle, n):
 @pytest.mark.parametrize("emb_half", [True, False])
 @pytest.mark.parametrize("n", [1, 128, 5000, 40000])
 def test_mlp_bwd_tcgen05_matches_oracle(ops, oracle, emb_half, n, saved):
+    _mlp_bwd_matches_oracle(ops, oracle, emb_half, n, saved, "xavier")
+
+
+@pytest.mark.parametrize("saved", [False, True])
+@pytest.mark.parametrize("emb_half", [True, False])
+@pytest.mark.parametrize("n", [1, 128, 5000, 40000])
+def test_mlp_bwd_tcgen05_matches_oracle_trained(ops, oracle, emb_half, n, saved):
+    """The same comparison on the finite regimes of tests/mlp_tolerance.py::trained_inputs; on its probe rows the
+    TruncExp gradient (r16(dsig exp(+-15)) where h0 is clamped) must also reach dL/demb exactly, through the
+    recompute and the saved-activation backward."""
+    _mlp_bwd_matches_oracle(ops, oracle, emb_half, n, saved, "trained")
+
+
+def _mlp_bwd_matches_oracle(ops, oracle, emb_half, n, saved, magnitude):
     rng = np.random.default_rng(35)
     emb = (rng.standard_normal((n, 32)) * 0.5).astype(np.float16 if emb_half else np.float32)
     dirs = rng.standard_normal((n, 3)).astype(np.float32)
     ws = _weights(rng)
     dsig = (rng.standard_normal(n) * 0.1).astype(np.float32)
     drgb = (rng.standard_normal((n, 3)) * 0.1).astype(np.float16)
+    rows = None
+    if magnitude == "trained":
+        from mlp_tolerance import trained_inputs
+        emb, dirs, ws, dsig, drgb, rows = trained_inputs(n, 35, np.float16 if emb_half else np.float32)
     demb_ref, gw_ref = oracle.mlp_bwd(emb, dirs, ws, dsig, drgb)
     save = None
     if saved:   # backward restarting from the activations the forward kept (h + fp16 rgb) instead of recomputing
@@ -411,6 +444,10 @@ def test_mlp_bwd_tcgen05_matches_oracle(ops, oracle, emb_half, n, saved):
         assert torch.equal(kept[n * 16:n * 16 + n * 4].view(n, 4)[:, :3], rgb_f)
     demb, gw = ops.mlp_bwd(T(emb), T(dirs), [T(w) for w in ws], T(dsig), T(drgb), save=save)
     demb, gw = N(demb).astype(np.float32), N(gw)
+    if rows is not None:
+        from test_gpu_mlp_magnitudes import check_probe_rows
+        sig_k, _ = ops.mlp_fwd(T(emb), T(dirs), [T(w) for w in ws])
+        assert check_probe_rows(demb, N(sig_k), dsig, rows) > 0
     demb_ref = demb_ref.astype(np.float32)
     # Error model (scripts/measure_mlp_bwd_error.py).  Every intermediate gradient is rounded to fp16 on both
     # sides and the tensor core sums K in a different order, so individual roundings flip by one fp16 ulp: the bulk of
