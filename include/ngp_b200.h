@@ -180,6 +180,15 @@ int ngp_hash_encode_bwd(const float* xyz, const void* dout, int dout_dtype,
 int ngp_hash_encode_bwd_input(const float* xyz, const void* table, const void* dout, int dtype,
                               const ngp_hash_layout* layout, float* dx,
                               int64_t n, void* stream);
+/* ngp_hash_encode_bwd_input with a device row count and the AABB fold of ngp_hash_encode_fwd_dyn (graph-capturable):
+ * rows = min(n, max(*n_dev, 0)) when n_dev is non-null, rows past them are not written.  aabb6 (HOST pointer, may be
+ * null) = {xyz_min[3], xyz_max - xyz_min[3]}: xyz are world positions, normalised as the forward does, and dx is the
+ * gradient wrt the world position (the [0,1] gradient divided by the span, strict fp32).  Any feature_per_level in
+ * [1, 8]; with feature_per_level == 2, n_dev null and aabb6 null the values are ngp_hash_encode_bwd_input's, bit for
+ * bit.  Camera extrinsics refinement (DESIGN.md §6i) reads it. */
+int ngp_hash_encode_bwd_input_dyn(const float* xyz, const void* table, const void* dout, int dtype,
+                                  const ngp_hash_layout* layout, float* dx, int64_t n, const int32_t* n_dev,
+                                  const float* aabb6, void* stream);
 
 /* ---- tri-plane encoding ---------------------------------------------------- */
 /* forward: replaces triplane_encoder_kernel, modules/triplane.py:35-98.  xyz [n,3] in [0,1] ->
@@ -618,6 +627,31 @@ int ngp_mc_emit_vertices(const float* lattice, int64_t n, float threshold, float
                          int64_t n_vertices, int32_t* vbase, float* vertices, float* normals, void* stream);
 int ngp_mc_emit_faces(const float* lattice, int64_t n, float threshold, void* workspace, const int32_t* vbase,
                       int64_t n_faces, int32_t* faces, void* stream);
+
+/* ---- camera extrinsics refinement (DESIGN.md §6i) ---------------------------------------------------------------
+ * Per-image corrections corr [n_img, 8] fp32 = (omega[3], 0, tau[3], 0), 16-byte aligned; the pose gradient and the
+ * Adam moments have the same layout.  Image indices are int64 and are clamped to [0, n_img) as ngp_sample_ray_batch
+ * clamps them.
+ * ngp_pose_apply: per ray, R' = Exp(omega) R (Rodrigues, fp64, rounded once to fp32; omega = 0 keeps R), o' = o + tau
+ * (tau = 0 keeps o), rays_d = R' c in the strict fp32 order of ngp_sample_ray_batch, rays_o = o'.  directions [n,3]
+ * camera-frame, poses [n_img, 3, 4] camera-to-world.  With zero corrections the rays equal ngp_sample_ray_batch's
+ * given the same image and pixel, bit for bit.
+ * ngp_pose_grad: for each of the first min(n_rays, *n_rays_dev) rows (ray, start, count) of rays_a, with g_s = dx[s]
+ * and t_s = ts[s] over rows [start, start + count) (clipped to n_rows): G_o = sum g_s, G_d = sum t_s g_s, and
+ * grad[img(ray)] += (rays_d[ray] x G_d, 0, G_o, 0).  Sums over a ray are in a fixed order; the per-image sums use
+ * atomics, so their order (and last bits) vary between runs.  found_inf (optional) is set to 1 when a ray's
+ * contribution is not finite.
+ * ngp_pose_adam: per image, the omega gradient becomes J_l(omega)^T g (left Jacobian of SO(3), fp64), then the Adam of
+ * ngp_adam_step_dyn with lr/bc1 = lr_ratio * hyper_dev[0], sqrt(bc2) = hyper_dev[1], inv_scale = hyper_dev[2];
+ * nothing but the gradient changes when *found_inf != 0; the gradient is zeroed on every call. */
+int ngp_pose_apply(const float* directions, const int64_t* img_idxs, const float* poses, const float* corr,
+                   int64_t n_img, float* rays_o, float* rays_d, int64_t n_rays, void* stream);
+int ngp_pose_grad(const float* dx, const float* ts, const int32_t* rays_a, const int64_t* img_idxs,
+                  const float* rays_d, int64_t n_rays, const int32_t* n_rays_dev, int64_t n_rows, int64_t n_img,
+                  float* grad, int32_t* found_inf_or_null, void* stream);
+int ngp_pose_adam(float* corr, float* grad, float* exp_avg, float* exp_avg_sq, const int32_t* found_inf_or_null,
+                  const float* hyper_dev, float lr_ratio, float beta1, float beta2, float eps, int64_t n_img,
+                  void* stream);
 
 #ifdef __cplusplus
 }

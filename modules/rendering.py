@@ -13,11 +13,13 @@ NEAR_DISTANCE = 0.01
 
 
 def render(model, rays_o, rays_d, test_time=False, exp_step_factor=0, T_threshold=1e-4,
-           max_samples=MAX_SAMPLES, bg_rgb=None):
+           max_samples=MAX_SAMPLES, bg_rgb=None, position_grad=False):
     """AABB test, then the train or test rendering path.  Returns the result dict of the
     reference (train: rgb, depth, opacity, ws, deltas, ts, rays_a, rm_samples, vr_samples;
     test: rgb, depth, opacity, total_samples).  ``bg_rgb`` [N, 3] (training path only, --random_bg): each ray's own
-    background colour in place of the fixed white / black one."""
+    background colour in place of the fixed white / black one.  ``position_grad`` (training path only, camera
+    extrinsics refinement, DESIGN.md §6i): the sample positions require grad and are returned as results['xyzs'], whose
+    .grad the backward fills."""
     rays_o = rays_o.contiguous()
     rays_d = rays_d.contiguous()
     hits_t = ray_aabb_intersection(rays_o, rays_d, model.scale)
@@ -30,7 +32,7 @@ def render(model, rays_o, rays_d, test_time=False, exp_step_factor=0, T_threshol
                 return render_frame_compact(model, rays_o, rays_d, exp_step_factor, T_threshold, max_samples)
             return render_frame(model, rays_o, rays_d, exp_step_factor, T_threshold, max_samples)
         return _render_rays_test(model, rays_o, rays_d, hits_t, exp_step_factor, T_threshold, max_samples)
-    return _render_rays_train(model, rays_o, rays_d, hits_t, exp_step_factor, T_threshold, bg_rgb)
+    return _render_rays_train(model, rays_o, rays_d, hits_t, exp_step_factor, T_threshold, bg_rgb, position_grad)
 
 
 def _background(exp_step_factor, device):
@@ -76,11 +78,14 @@ def _render_rays_test(model, rays_o, rays_d, hits_t, exp_step_factor=0, T_thresh
     return results
 
 
-def _render_rays_train(model, rays_o, rays_d, hits_t, exp_step_factor=0, T_threshold=1e-4, bg_rgb=None):
+def _render_rays_train(model, rays_o, rays_d, hits_t, exp_step_factor=0, T_threshold=1e-4, bg_rgb=None,
+                       position_grad=False):
     results = {}
     (rays_a, xyzs, dirs, results['deltas'], results['ts'], results['rm_samples']) = raymarching_train(
         rays_o, rays_d, hits_t, model.density_bitfield, model.cascades, model.scale, exp_step_factor,
         model.grid_size, MAX_SAMPLES)
+    if position_grad:
+        results['xyzs'] = xyzs.requires_grad_(True)
 
     sigmas, rgbs = model(xyzs, dirs)
 

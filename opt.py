@@ -55,6 +55,9 @@ _FLAGS = [
     ('--max_steps', dict(type=int, default=20000, help='number of steps to train')),
     ('--lr', dict(type=float, default=1e-2, help='learning rate')),
     ('--random_bg', dict(action='store_true', default=False, help='train with random bg color (real scene only)')),
+    ('--extrinsics_lr', dict(type=float, default=0.,
+                             help='learning rate of the per-image camera pose corrections (rotation and translation, '
+                                  'DESIGN.md §6i), 0 to disable (default); hash encoder only, one GPU')),
     # misc
     ('--exp_name', dict(type=str, default='exp', help='experiment name')),
     ('--gpu', dict(type=int, default=0, help='set cuda device (ignored under torchrun: LOCAL_RANK wins)')),
@@ -103,6 +106,18 @@ def get_opts(prefix_args=None):
     if hparams.depth_loss_w > 0 and hparams.dataset_name in ('nerf', 'nsvf', 'colmap'):
         parser.error(f"--depth_loss_w: the {hparams.dataset_name} loader reads no depth (the ngp loader reads "
                      f"transforms.json's depth_path)")
+    if not (math.isfinite(hparams.extrinsics_lr) and hparams.extrinsics_lr >= 0):
+        parser.error(f"--extrinsics_lr must be finite and >= 0, got {hparams.extrinsics_lr}")
+    if hparams.extrinsics_lr > 0:
+        if not (math.isfinite(hparams.lr) and hparams.lr > 0):
+            parser.error(f"--extrinsics_lr is set relative to the model's learning rate: it needs a finite --lr > 0, got "
+                         f"{hparams.lr}")
+        if hparams.model_name == 'svox':
+            parser.error("--extrinsics_lr does not combine with --model_name svox: the voxel grid gives no gradient "
+                         "wrt the sample positions")
+        if hparams.encoder_type == 'triplane':
+            parser.error("--extrinsics_lr does not combine with --encoder_type triplane: the tri-plane encoder gives no "
+                         "gradient wrt the sample positions")
     if hparams.model_name == 'svox':
         for flag, bad, why in (
                 ('encoder_type', hparams.encoder_type == 'triplane',

@@ -47,6 +47,7 @@ def _declare(lib):
         "ngp_hash_encode_fwd": (ci, [vp, vp, lay, vp, ci, i64, vp]),
         "ngp_hash_encode_bwd": (ci, [vp, vp, ci, lay, vp, i64, vp]),
         "ngp_hash_encode_bwd_input": (ci, [vp, vp, vp, ci, lay, vp, i64, vp]),
+        "ngp_hash_encode_bwd_input_dyn": (ci, [vp, vp, vp, ci, lay, vp, i64, vp, vp, vp]),
         "ngp_hash_encode_fwd_dyn": (ci, [vp, vp, lay, vp, ci, i64, vp, vp, vp]),
         "ngp_hash_encode_bwd_dyn": (ci, [vp, vp, ci, lay, vp, i64, vp, vp, vp]),
         "ngp_hash_encode_bwd_levels": (ci, [vp, vp, ci, lay, vp, i64, vp, vp, ci, ci, vp, vp]),
@@ -121,6 +122,9 @@ def _declare(lib):
         "ngp_mc_scan": (ci, [i64, vp, vp, vp]),
         "ngp_mc_emit_vertices": (ci, [vp, i64, f32, f32, vp, i64, vp, vp, vp, vp]),
         "ngp_mc_emit_faces": (ci, [vp, i64, f32, vp, vp, i64, vp, vp]),
+        "ngp_pose_apply": (ci, [vp, vp, vp, vp, i64, vp, vp, i64, vp]),
+        "ngp_pose_grad": (ci, [vp, vp, vp, vp, vp, i64, vp, i64, i64, vp, vp, vp]),
+        "ngp_pose_adam": (ci, [vp, vp, vp, vp, vp, vp, f32, f32, f32, f32, i64, vp]),
     }
     for name, (res, args) in sigs.items():
         fn = getattr(lib, name)  # AttributeError if the symbol is missing: fail loudly

@@ -549,18 +549,41 @@ __device__ __forceinline__ uint32_t corner_index(const LevelMeta& m, const uint3
 
 // ---- backward wrt input position ----------------------------------------------------------------
 // The derivative of the forward inside the cell of x: the fp16 kernel takes it at the forward's fraction p - f16(g),
-// which differs from p - g for odd g above 2048 (levels 14-15 at max_res 4096).
+// which differs from p - g for odd g above 2048 (levels 14-15 at max_res 4096).  With the AABB fold (dyn.normalize) x
+// is the world position, normalised as the forward does, and dx is the world gradient: the [0,1] gradient divided by
+// the span, as autograd divides it through NGP.density's normalisation.
+__device__ __forceinline__ void load_input_pos(const float* __restrict__ xyz, int64_t i, const Dyn& dyn, float x[3]) {
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+        x[k] = xyz[i * 3 + k];
+        if (dyn.normalize) x[k] = f_div(f_sub(x[k], dyn.lo[k]), dyn.span[k]);
+    }
+}
+
+__device__ __forceinline__ void store_input_grad(float* __restrict__ dx, int64_t i, const Dyn& dyn, float gx, float gy,
+                                                 float gz) {
+    if (dyn.normalize) {
+        gx = f_div(gx, dyn.span[0]);
+        gy = f_div(gy, dyn.span[1]);
+        gz = f_div(gz, dyn.span[2]);
+    }
+    dx[i * 3 + 0] = gx;
+    dx[i * 3 + 1] = gy;
+    dx[i * 3 + 2] = gz;
+}
+
 template <typename T>
 __global__ void __launch_bounds__(256) hash_bwd_input_kernel(const float* __restrict__ xyz,
                                                              const T* __restrict__ table,
                                                              const T* __restrict__ dout,
                                                              const __grid_constant__ ngp_hash_layout lay,
-                                                             float* __restrict__ dx, int64_t n) {
+                                                             float* __restrict__ dx, int64_t n_max, const Dyn dyn) {
     using V2 = typename Vec2<T>::type;
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
+    if (i >= effective_n(dyn, n_max)) return;
     const int L = lay.n_levels;
-    const float x[3] = {xyz[i * 3 + 0], xyz[i * 3 + 1], xyz[i * 3 + 2]};
+    float x[3];
+    load_input_pos(xyz, i, dyn, x);
     float gx = 0.f, gy = 0.f, gz = 0.f;
     for (int l = 0; l < L; ++l) {
         const LevelMeta m = level_meta(lay, l);
@@ -586,9 +609,45 @@ __global__ void __launch_bounds__(256) hash_bwd_input_kernel(const float* __rest
             gz += ((c & 4) ? v : -v) * wx * wy;
         }
     }
-    dx[i * 3 + 0] = gx;
-    dx[i * 3 + 1] = gy;
-    dx[i * 3 + 2] = gz;
+    store_input_grad(dx, i, dyn, gx, gy, gz);
+}
+
+// any feature width in [1, 8] (the --deployment model has 4): the same terms, the feature sum in feature order
+template <typename T>
+__global__ void __launch_bounds__(256) hash_bwd_input_generic_kernel(const float* __restrict__ xyz,
+                                                                     const T* __restrict__ table,
+                                                                     const T* __restrict__ dout,
+                                                                     const __grid_constant__ ngp_hash_layout lay,
+                                                                     float* __restrict__ dx, int64_t n_max,
+                                                                     const Dyn dyn) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= effective_n(dyn, n_max)) return;
+    const int L = lay.n_levels, F = lay.feat_dim;
+    float x[3];
+    load_input_pos(xyz, i, dyn, x);
+    float gx = 0.f, gy = 0.f, gz = 0.f;
+    for (int l = 0; l < L; ++l) {
+        const LevelMeta m = level_meta(lay, l);
+        uint32_t g[3], idx[8];
+        float pos[3];
+        grid_pos<sizeof(T) == 2>(x, m, g, pos);
+        corner_indices(m, g, idx);
+        float dy[8];
+        for (int f = 0; f < F; ++f) dy[f] = load_as_float(dout, (i * L + l) * F + f);
+#pragma unroll
+        for (int c = 0; c < 8; ++c) {
+            float dot = 0.0f;
+            for (int f = 0; f < F; ++f) dot += load_as_float(table, (int64_t)idx[c] * F + f) * dy[f];
+            const float v = dot * m.scale;
+            const float wx = (c & 1) ? pos[0] : 1.0f - pos[0];
+            const float wy = (c & 2) ? pos[1] : 1.0f - pos[1];
+            const float wz = (c & 4) ? pos[2] : 1.0f - pos[2];
+            gx += ((c & 1) ? v : -v) * wy * wz;
+            gy += ((c & 2) ? v : -v) * wx * wz;
+            gz += ((c & 4) ? v : -v) * wx * wy;
+        }
+    }
+    store_input_grad(dx, i, dyn, gx, gy, gz);
 }
 
 size_t smem_bytes(int n_levels, int vec_bytes) {
@@ -769,12 +828,32 @@ int ngp_hash_encode_bwd_input(const float* xyz, const void* table, const void* d
     if (n == 0) return 0;
     NGP_REQUIRE(xyz && table && dout && dx, "null pointer");
     NGP_REQUIRE(layout->feat_dim == 2, "dL/dx is implemented for feature_per_level == 2");
+    return ngp_hash_encode_bwd_input_dyn(xyz, table, dout, dtype, layout, dx, n, nullptr, nullptr, stream);
+}
+
+int ngp_hash_encode_bwd_input_dyn(const float* xyz, const void* table, const void* dout, int dtype,
+                                  const ngp_hash_layout* layout, float* dx, int64_t n, const int32_t* n_dev,
+                                  const float* aabb6, void* stream) {
+    const Dyn dyn = make_dyn(n_dev, aabb6);
+    if (int rc = check_layout(layout)) return rc;
+    NGP_REQUIRE(n >= 0, "negative n");
+    NGP_REQUIRE(dtype == NGP_F32 || dtype == NGP_F16, "bad dtype");
+    if (n == 0) return 0;
+    NGP_REQUIRE(xyz && table && dout && dx, "null pointer");
     const unsigned grid = (unsigned)((n + 255) / 256);
     cudaStream_t st = ngp::as_stream(stream);
+    if (layout->feat_dim != 2) {
+        if (dtype == NGP_F16)
+            hash_bwd_input_generic_kernel<__half><<<grid, 256, 0, st>>>(xyz, (const __half*)table, (const __half*)dout, *layout, dx, n, dyn);
+        else
+            hash_bwd_input_generic_kernel<float><<<grid, 256, 0, st>>>(xyz, (const float*)table, (const float*)dout, *layout, dx, n, dyn);
+        NGP_LAUNCHED("hash_bwd_input_generic_kernel");
+        return 0;
+    }
     if (dtype == NGP_F16)
-        hash_bwd_input_kernel<__half><<<grid, 256, 0, st>>>(xyz, (const __half*)table, (const __half*)dout, *layout, dx, n);
+        hash_bwd_input_kernel<__half><<<grid, 256, 0, st>>>(xyz, (const __half*)table, (const __half*)dout, *layout, dx, n, dyn);
     else
-        hash_bwd_input_kernel<float><<<grid, 256, 0, st>>>(xyz, (const float*)table, (const float*)dout, *layout, dx, n);
+        hash_bwd_input_kernel<float><<<grid, 256, 0, st>>>(xyz, (const float*)table, (const float*)dout, *layout, dx, n, dyn);
     NGP_LAUNCHED("hash_bwd_input_kernel");
     return 0;
 }

@@ -8,6 +8,10 @@ the C-ABI kernels, enqueued in a fixed order on fixed buffers:
   [+ distortion loss] [+ depth loss] + composite bwd) -> MLP bwd -> hash (or tri-plane) bwd -> [gradient exchange] -> check_finite -> device-side LR/bias-correction update
   -> fused Adam (+fp16 shadow, grad zero) -> device-side GradScaler update
 
+With camera extrinsics refinement (DESIGN.md §6i) the rays come from the pose-apply kernel (the graph's first node, on
+camera directions and image indices), the hash backward is followed by the position gradient and the pose gradient,
+and the corrections' Adam runs next to the model's.
+
 A voxel-grid model (--model_name svox) has no network: the march feeds the voxel forward (fp32 sigma / rgb) -> head ->
 voxel backward -> [regularisers] -> finite check and Adam over the fields' node block B only (DESIGN.md §6b).
 
@@ -35,7 +39,8 @@ class StaticTrainStep:
     def __init__(self, trainer, n_rays: int, samples_per_ray_capacity: int = 384, exp_step_factor: float = 0.0,
                  T_threshold: float = 1e-4, max_samples: int = 1024, use_graph: bool = True,
                  dynamic_loss_scale: bool = True, overlap_optimizer: bool = False, distortion_loss_w: float = 0.0,
-                 random_bg: bool = False, bg_seed: int = 0, bg_load: float = 1.0, depth_loss_w: float = 0.0):
+                 random_bg: bool = False, bg_seed: int = 0, bg_load: float = 1.0, depth_loss_w: float = 0.0,
+                 extrinsics=None):
         self.tr = trainer
         m = self.model = trainer.model
         # the voxel-grid model: fp32 fields and outputs, no encoder and no MLP; its optimizer pass covers the node
@@ -48,6 +53,14 @@ class StaticTrainStep:
                 raise _lib.NgpError("StaticTrainStep runs a voxel-grid model on one rank only")
         elif not m._fusable(next(m.parameters())):
             raise _lib.NgpError("StaticTrainStep needs the stock NGP architecture (fused MLP)")
+        # extrinsics: the trainer's PoseRefinement (NGPTrainer(extrinsics=...)), shared with the module path, or None
+        if extrinsics is not trainer.extrinsics:
+            raise ValueError("StaticTrainStep: extrinsics must be the trainer's PoseRefinement "
+                             "(NGPTrainer(extrinsics=...)), or None for a trainer without one")
+        self.ext = extrinsics
+        if self.ext is not None and overlap_optimizer:
+            raise _lib.NgpError("StaticTrainStep: extrinsics refinement does not combine with overlap_optimizer (the "
+                                "next step's march would read poses one update stale)")
         dev = next(m.parameters()).device
         self.dev, self.n = dev, int(n_rays)
         self.cap = C_ = int(n_rays) * int(samples_per_ray_capacity)
@@ -94,6 +107,11 @@ class StaticTrainStep:
         self.bg_step = torch.full((1,), trainer.step_count, device=dev, dtype=i32)
         self.bg_rgb, self.alpha = (z(self.n, 3), torch.ones(self.n, device=dev)) if self.random_bg else (None, None)
         self.depth_gt = z(self.n) if self.depth_w > 0 else None   # per-ray target z-depth, 0 = none
+        # extrinsics refinement: camera directions and image indices in, dL/dx of every sample row
+        if self.ext is not None:
+            self.cam_dirs, self.img_idx = z(self.n, 3), torch.zeros(self.n, device=dev, dtype=torch.int64)
+            self.cam_dirs[:, 2] = -1.0   # valid placeholder rays for the capture (a zero direction never advances)
+            self.dx = z(C_, 3)
         # GradScaler state on the device: [scale, growth_tracker (int bits)]; growth 2x / 2000 clean steps, backoff 0.5
         trainer.dynamic_loss_scale = self.dynamic_loss_scale = bool(dynamic_loss_scale)
         self.aabb6 = (C.c_float * 6)(*[float(v) for v in m.xyz_min.flatten().tolist()],
@@ -252,6 +270,22 @@ class StaticTrainStep:
                                               _p(self.tr.flat_grad), self.cap, _p(self.counter), self.aabb6,
                                               _p(self.tr.found_inf) if self.inf_at_source else None, self._st()))
 
+    # extrinsics refinement (DESIGN.md §6i): rays from the corrected poses; dL/dx of the rows; the pose gradient
+    def _k_pose_apply(self):
+        e = self.ext
+        check(load().ngp_pose_apply(_p(self.cam_dirs), _p(self.img_idx), _p(e.poses), _p(e.corr), e.n_img,
+                                    _p(self.rays_o), _p(self.rays_d), self.n, self._st()))
+
+    def _k_hash_dx(self):
+        check(load().ngp_hash_encode_bwd_input_dyn(_p(self.xyzs), _p(self._table()), _p(self.demb),
+                                                   self.enc._tag(), C.byref(self.enc._clayout), _p(self.dx),
+                                                   self.cap, _p(self.counter), self.aabb6, self._st()))
+
+    def _k_pose_grad(self):
+        e = self.ext
+        check(load().ngp_pose_grad(_p(self.dx), _p(self.ts), _p(self.rays_a), _p(self.img_idx), _p(self.rays_d),
+                                   self.n, None, self.cap, e.n_img, _p(e.grad), _p(self.tr.found_inf), self._st()))
+
     # the voxel grid's stages: fields -> fp32 sigma / rgb, and the field gradient into the trainer's flat buffer
     def _k_voxel_fwd(self):
         m = self.model
@@ -279,6 +313,9 @@ class StaticTrainStep:
         self._k_head()
         self._k_mlp_bwd()
         self._k_hash_bwd()
+        if self.ext is not None:
+            self._k_hash_dx()
+            self._k_pose_grad()
 
     def _enqueue_sampler(self):
         """datasets/base.py:34-61 + ray_utils.py:51-80 + the marching jitter, keyed by (seed, batch counter, ray)."""
@@ -293,6 +330,8 @@ class StaticTrainStep:
         self.tr.enqueue_update(check_finite=not self.inf_at_source, voxel_block=self.block if self.vox else None)
 
     def _enqueue(self, sampled=False, mode="sync"):
+        if self.ext is not None:
+            self._k_pose_apply()
         if sampled:
             self._enqueue_sampler()
         # march counter, loss accumulator, found_inf <- 0 and (own batch counter: step_dev moves with the optimizer,
@@ -325,6 +364,7 @@ class StaticTrainStep:
         keep = [p.data.clone() for p in tr.params] + [tr.exp_avg.clone(), tr.exp_avg_sq.clone(), self.step_dev.clone()]
         scale_keep, hyper_keep, sample_keep = self.scale_state.clone(), self.hyper.clone(), self.sample_step.clone()
         bg_step_keep = self.bg_step.clone()
+        ext_keep = [] if self.ext is None else [t.clone() for t in self.ext.state()]
         shadow = None if tr._shadow_full is None else tr._shadow_full.clone()
         side = torch.cuda.Stream()
         side.wait_stream(torch.cuda.current_stream())
@@ -348,24 +388,39 @@ class StaticTrainStep:
         self.hyper.copy_(hyper_keep)
         self.sample_step.copy_(sample_keep)
         self.bg_step.copy_(bg_step_keep)
+        if self.ext is not None:
+            for t, k in zip(self.ext.state(), ext_keep):
+                t.copy_(k)
         tr.flat_grad.zero_()
         if shadow is not None:
             tr._shadow_full.copy_(shadow)
         self._graphs[(sampled, mode)], self._kernels[(sampled, mode)] = graph, kernels
 
     # ---------------------------------------------------------------------------------------------
-    def step(self, rays_o, rays_d, rgb_gt, noise=None, alpha=None, depth=None):
+    def step(self, rays_o, rays_d, rgb_gt, noise=None, alpha=None, depth=None, directions=None, img_idxs=None):
         """Enqueues one full training step; returns the (device) loss tensor — nothing is synchronised.  ``alpha`` [N]
         (random_bg only): the images' alpha, whose transparent part of the target gets the ray's colour.  ``depth`` [N]
-        (depth_loss_w > 0 only, where it is required): each ray's target z-depth, 0 where there is none."""
+        (depth_loss_w > 0 only, where it is required): each ray's target z-depth, 0 where there is none.  With
+        extrinsics refinement the step forms its rays itself: rays_o and rays_d are None and ``directions`` [N, 3]
+        (camera frame) and ``img_idxs`` [N] (or one index for the whole batch) are required."""
+        if self.ext is not None:
+            if directions is None or img_idxs is None or rays_o is not None or rays_d is not None:
+                raise ValueError("extrinsics refinement: step(None, None, rgb, ..., directions=..., img_idxs=...) "
+                                 "(the step forms the rays from the corrected poses)")
+            self.cam_dirs.copy_(directions, non_blocking=True)
+            self.img_idx.copy_(torch.as_tensor(img_idxs, device=self.dev).reshape(-1), non_blocking=True)
+        elif directions is not None or img_idxs is not None:
+            raise ValueError("directions / img_idxs are read by extrinsics refinement only "
+                             "(StaticTrainStep(extrinsics=...))")
         if depth is None and self.depth_w > 0:
             raise ValueError("depth_loss_w > 0 needs each ray's target depth: step(..., depth=...)")
         if depth is not None and self.depth_w == 0:
             raise ValueError("depth is read by the depth loss only (StaticTrainStep(depth_loss_w=...))")
         if depth is not None:
             self.depth_gt.copy_(depth, non_blocking=True)
-        self.rays_o.copy_(rays_o, non_blocking=True)
-        self.rays_d.copy_(rays_d, non_blocking=True)
+        if self.ext is None:
+            self.rays_o.copy_(rays_o, non_blocking=True)
+            self.rays_d.copy_(rays_d, non_blocking=True)
         self.gt.copy_(rgb_gt, non_blocking=True)
         if alpha is not None and not self.random_bg:
             raise ValueError("alpha is read by the random background only (StaticTrainStep(random_bg=True))")
@@ -419,6 +474,9 @@ class StaticTrainStep:
             raise _lib.NgpError("the device-sampled step does not support random_bg yet; use step()")
         if self.depth_w > 0:
             raise _lib.NgpError("the device-sampled step does not support depth supervision yet; use step(depth=...)")
+        if self.ext is not None:
+            raise _lib.NgpError("the device-sampled step does not support extrinsics refinement yet; use "
+                                "step(directions=..., img_idxs=...)")
         f = lambda t: t.detach().to(self.dev, torch.float32).contiguous()  # noqa: E731
         bank, poses, directions = f(image_bank), f(poses), f(directions)
         if bank.ndim != 3 or bank.shape[0] != poses.shape[0] or bank.shape[1] != directions.shape[0] or bank.shape[2] < 3:

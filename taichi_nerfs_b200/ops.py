@@ -126,11 +126,20 @@ def hash_encode_bwd(xyz, dout, clayout, grad_table):
 
 
 def hash_encode_bwd_input(xyz, table, dout, clayout):
-    _need_cuda(xyz, table, dout)
-    dx = torch.empty(xyz.shape[0], 3, device=xyz.device, dtype=torch.float32)
-    check(load().ngp_hash_encode_bwd_input(_ptr(xyz), _ptr(table), _ptr(dout), _tag(table), C.byref(clayout),
-                                           _ptr(dx), xyz.shape[0], _stream()),
-          "hash_encode_bwd_input")
+    """dL/dx [n, 3] fp32 of positions xyz in [0,1]; any feature width (the fixed-count entry takes F = 2 only, the
+    device-counted one every width, with the same values at F = 2)."""
+    return hash_encode_bwd_input_dyn(xyz, table, dout, clayout)
+
+
+def hash_encode_bwd_input_dyn(xyz, table, dout, clayout, n_dev=None, aabb=None, out=None):
+    """dL/dx [n, 3] fp32 over rows [0, min(n, n_dev[0])) (n_dev: int32 [1] device count, None: all n rows).  aabb =
+    (xyz_min[3], xyz_max-xyz_min[3]): xyz are world positions and dx the world gradient (DESIGN.md §6i)."""
+    _need_cuda(xyz, table, dout, n_dev, out)
+    dx = torch.empty(xyz.shape[0], 3, device=xyz.device, dtype=torch.float32) if out is None else out
+    a6 = None if aabb is None else (C.c_float * 6)(*[float(v) for v in aabb])
+    check(load().ngp_hash_encode_bwd_input_dyn(_ptr(xyz), _ptr(table), _ptr(dout), _tag(table), C.byref(clayout),
+                                               _ptr(dx), xyz.shape[0], _ptr(n_dev), a6, _stream()),
+          "hash_encode_bwd_input_dyn")
     return dx
 
 
@@ -481,6 +490,67 @@ def sample_ray_batch(image_bank, poses, directions, n_rays, *, img_idxs=None, pi
     if return_indices:
         res["img_idxs"], res["pix_idxs"] = ii, pi
     return res
+
+
+# ---- camera extrinsics refinement (DESIGN.md §6i) ---------------------------------------------------------------
+def _pose_buffers(*ts):
+    for t in ts:
+        if t.dtype != torch.float32 or not t.is_contiguous() or t.dim() != 2 or t.shape[1] != 8:
+            raise TypeError("pose corrections, gradients and moments are contiguous fp32 [n_img, 8]")
+
+
+def _img_index(img_idxs, n):
+    i = img_idxs.to(torch.int64).reshape(-1)
+    if i.numel() == 1 and n != 1:   # one image for the whole batch (--ray_sampling_strategy same_image)
+        i = i.expand(n)
+    if i.numel() != n:
+        raise ValueError(f"{i.numel()} image indices for {n} rays")
+    return i.contiguous()
+
+
+def pose_apply(directions, img_idxs, poses, corr, rays_o=None, rays_d=None):
+    """Rays (rays_o [n,3], rays_d [n,3] fp32) of camera directions [n,3] of images img_idxs [n] (or one index) under
+    the corrected poses: R' = Exp(omega) R, o' = o + tau; poses [n_img, 3, 4], corr [n_img, 8]."""
+    _need_cuda(directions, img_idxs, poses, corr, rays_o, rays_d)
+    _pose_buffers(corr)
+    d = _f32c(directions)
+    n = d.shape[0]
+    P = _f32c(poses)
+    if P.dim() != 3 or tuple(P.shape[1:]) != (3, 4) or P.shape[0] != corr.shape[0]:
+        raise ValueError(f"poses {tuple(P.shape)} must be [n_img, 3, 4] with n_img = {corr.shape[0]}")
+    idx = _img_index(img_idxs, n)
+    o = torch.empty(n, 3, device=d.device, dtype=torch.float32) if rays_o is None else rays_o
+    dd = torch.empty(n, 3, device=d.device, dtype=torch.float32) if rays_d is None else rays_d
+    check(load().ngp_pose_apply(_ptr(d), _ptr(idx), _ptr(P), _ptr(corr), P.shape[0], _ptr(o), _ptr(dd), n,
+                                _stream()), "pose_apply")
+    return o, dd
+
+
+def pose_grad(dx, ts, rays_a, img_idxs, rays_d, grad, n_rays_dev=None, found_inf=None):
+    """grad [n_img, 8] += per image (d' x G_d, 0, G_o, 0) of the rays in rays_a [n, 3] (ray, start, count), from
+    the sample gradients dx [S, 3] and sample times ts [S]; img_idxs [n] (or one index) and rays_d [n, 3] by ray id."""
+    _need_cuda(dx, ts, rays_a, img_idxs, rays_d, grad, n_rays_dev, found_inf)
+    _pose_buffers(grad)
+    if dx.dtype != torch.float32 or ts.dtype != torch.float32 or rays_a.dtype != torch.int32:
+        raise TypeError("pose_grad: dx and ts are fp32, rays_a int32")
+    n = rays_a.shape[0]
+    idx = _img_index(img_idxs, n)
+    dxc, tsc, d = dx.contiguous(), ts.contiguous(), _f32c(rays_d)
+    if d.shape[0] != n or tsc.shape[0] != dxc.shape[0]:
+        raise ValueError("pose_grad: rays_d needs one row per ray and ts one value per row of dx")
+    check(load().ngp_pose_grad(_ptr(dxc), _ptr(tsc), _ptr(rays_a.contiguous()), _ptr(idx), _ptr(d), n,
+                               _ptr(n_rays_dev), dxc.shape[0], grad.shape[0], _ptr(grad), _ptr(found_inf), _stream()),
+          "pose_grad")
+
+
+def pose_adam(corr, grad, exp_avg, exp_avg_sq, hyper, lr_ratio, found_inf=None, beta1=0.9, beta2=0.999, eps=1e-15):
+    """One Adam step of the corrections with the model's device scalars ``hyper`` (ngp_adam_hyper_update) and a
+    learning rate lr_ratio times the model's; the gradient goes through J_l(omega)^T first and is zeroed."""
+    _need_cuda(corr, grad, exp_avg, exp_avg_sq, hyper, found_inf)
+    _pose_buffers(corr, grad, exp_avg, exp_avg_sq)
+    check(load().ngp_pose_adam(_ptr(corr), _ptr(grad), _ptr(exp_avg), _ptr(exp_avg_sq), _ptr(found_inf), _ptr(hyper),
+                               float(lr_ratio), float(beta1), float(beta2), float(eps), corr.shape[0], _stream()),
+          "pose_adam")
 
 
 def morton3d(coords):

@@ -31,9 +31,10 @@ def _p(t):
 class NGPTrainer:
     def __init__(self, model, lr: float = 1e-2, max_steps: int = 20000, loss_scale: float | None = None,
                  betas=(0.9, 0.999), eps: float = 1e-15, process_group=None, dynamic_loss_scale: bool = True,
-                 p2p_optimizer: bool | None = None, voxel_reg=None):
+                 p2p_optimizer: bool | None = None, voxel_reg=None, extrinsics=None):
         from modules.hash_encoder import HashEncoder
         from modules.voxel_grid import VoxelGrid
+        from .extrinsics import PoseRefinement
         # The model kind, decided here once (StaticTrainStep reads it too): the position encoder, whose one parameter
         # (its table) must be the first slice of the flat buffers, or None for a VoxelGrid, which has no encoder and
         # scatters into the .grad views of its own fields.
@@ -62,6 +63,19 @@ class NGPTrainer:
         self.world_size = 1
         if process_group is not None or (torch.distributed.is_available() and torch.distributed.is_initialized()):
             self.world_size = torch.distributed.get_world_size(process_group)
+
+        # camera extrinsics refinement (DESIGN.md §6i): a PoseRefinement whose Adam step runs with the model's, or None
+        if extrinsics is not None:
+            if not isinstance(extrinsics, PoseRefinement):
+                raise TypeError("NGPTrainer: extrinsics must be a taichi_nerfs_b200.extrinsics.PoseRefinement")
+            if not isinstance(enc, HashEncoder):
+                raise ValueError("NGPTrainer: extrinsics refinement needs the gradient wrt the sample positions, which "
+                                 "only the hash encoder provides (not the tri-plane encoder or the voxel grid)")
+            if self.world_size > 1:
+                raise ValueError("NGPTrainer: extrinsics refinement runs on one rank (the pose gradient is not "
+                                 "exchanged between ranks)")
+        self.extrinsics = extrinsics
+        self._pose_batch = None   # (xyzs, ts, rays_a, img_idxs, rays_d) of the last forward_backward
 
         self.params = [p for p in model.parameters() if p.requires_grad]
         if enc is not None:
@@ -168,15 +182,22 @@ class NGPTrainer:
         self._views = []
 
     def forward_backward(self, rays_o, rays_d, rgb_gt, exp_step_factor=0.0, extra_loss=None, bg_rgb=None, alpha=None,
-                         b_load=1.0):
+                         b_load=1.0, img_idxs=None):
         """bg_rgb [N, 3] (--random_bg, ops.random_bg): each ray's background colour replaces the fixed one; with
         ``alpha`` [N] (the image's alpha), the target's loader background ``b_load`` is replaced by it too:
-        rgb_gt + (bg_rgb - b_load)(1 - alpha)."""
+        rgb_gt + (bg_rgb - b_load)(1 - alpha).  With extrinsics refinement, ``img_idxs`` [N] (or one index) names each
+        ray's image and rays_o / rays_d are the PoseRefinement's rays; the pose gradient is formed by optimizer_step."""
         from modules.rendering import render
+        refine = self.extrinsics is not None
+        if refine and img_idxs is None:
+            raise ValueError("NGPTrainer: extrinsics refinement needs each ray's image index (img_idxs=...)")
+        if not refine and img_idxs is not None:
+            raise ValueError("NGPTrainer: img_idxs is read by extrinsics refinement only (NGPTrainer(extrinsics=...))")
         if bg_rgb is not None and alpha is not None:
             rgb_gt = rgb_gt + (bg_rgb - b_load) * (1 - alpha)[:, None]
         with torch.autocast(device_type='cuda', dtype=torch.float16):
-            results = render(self.model, rays_o, rays_d, exp_step_factor=exp_step_factor, bg_rgb=bg_rgb)
+            results = render(self.model, rays_o, rays_d, exp_step_factor=exp_step_factor, bg_rgb=bg_rgb,
+                             position_grad=refine)
             loss = F.mse_loss(results['rgb'], rgb_gt)
             if extra_loss is not None:  # e.g. distortion loss (train.py:194-195)
                 loss = loss + extra_loss(results)
@@ -185,7 +206,19 @@ class NGPTrainer:
         (loss * scale).backward()
         if self.voxel_reg is not None:
             self.add_voxel_reg()
+        if refine:
+            self._pose_batch = (results.pop('xyzs'), results['ts'], results['rays_a'], img_idxs, rays_d)
         return loss, results
+
+    def enqueue_pose_grad(self):
+        """Extrinsics refinement: the pose gradient of the last forward_backward (its sample positions' .grad) into the
+        PoseRefinement's buffer, raising found_inf on a non-finite contribution."""
+        xyzs, ts, rays_a, img_idxs, rays_d = self._pose_batch
+        self._pose_batch = None
+        dx = xyzs.grad
+        if dx is None:   # no sample reached the network
+            return
+        self.extrinsics.accumulate(dx, ts, rays_a, img_idxs, rays_d.float(), found_inf=self.found_inf)
 
     def add_voxel_reg(self, loss=None):
         """Add loss_scale * the gradient of the voxel regularisers into the flat gradient (the model's grad_sink), from
@@ -268,6 +301,8 @@ class NGPTrainer:
             check(L.ngp_adam_step_dyn(_p(self.flat_param), _p(fg), _p(self.exp_avg), _p(self.exp_avg_sq),
                                       _p(self._shadow_full), _p(self.found_inf), _p(self.hyper), self.betas[0],
                                       self.betas[1], self.eps, 1, fg.numel(), st))
+        if self.extrinsics is not None:   # the pose corrections' Adam, on the same device scalars (one rank)
+            self.extrinsics.enqueue_adam(self)
         if self.dynamic_loss_scale:  # GradScaler.update(): adjusts the scale used by the NEXT step
             # a flag raised at the source is not reset by the next step, so this launch clears it
             raised_at_source = not check_finite and g16 is None
@@ -293,12 +328,15 @@ class NGPTrainer:
         self.check_aliasing()
         self.step_count += 1
         self.found_inf.zero_()
+        if self._pose_batch is not None:
+            self.enqueue_pose_grad()
         self.enqueue_update()
         if self._shadow is not None:
             self.encoder.adopt_shadow(self._shadow)
 
-    def step(self, rays_o, rays_d, rgb_gt, exp_step_factor=0.0, extra_loss=None, bg_rgb=None, alpha=None, b_load=1.0):
+    def step(self, rays_o, rays_d, rgb_gt, exp_step_factor=0.0, extra_loss=None, bg_rgb=None, alpha=None, b_load=1.0,
+             img_idxs=None):
         loss, results = self.forward_backward(rays_o, rays_d, rgb_gt, exp_step_factor, extra_loss, bg_rgb, alpha,
-                                              b_load)
+                                              b_load, img_idxs)
         self.optimizer_step()
         return loss, results

@@ -4,6 +4,8 @@ Adam(lr, eps=1e-15) + cosine annealing to lr/30 (:143-163), density-grid update 
 256-step warm-up (:57-58,178-182), log line every 1000 steps (:203-219), results/model.pth (:232-235),
 test-split PSNR and SSIM (:237-304); with --extract_mesh, results/mesh.ply after the evaluation (DESIGN.md §6g).
 With --depth_loss_w the loss gains the depth term (DESIGN.md §6h) and a test split with depth reports depth_mae.
+With --extrinsics_lr every training image's pose is refined with the model (DESIGN.md §6i): the training rays come from
+the corrected poses, results/poses_refined.npy holds them at the end; the test split keeps its poses as loaded.
 The step body runs on the sm_90a kernels through NGPTrainer (fused Adam,
 no host sync for the inf check); under torchrun every rank trains on its own rays and the gradients are summed
 once per step: by the peer-memory optimizer kernel when all ranks share one NVLink box, else by an fp16 NCCL
@@ -66,6 +68,8 @@ def main(prefix_args=None):
         raise RuntimeError("train.py needs a CUDA device: the hot path has no CPU fallback")
     device = torch.device("cuda", local)
     torch.cuda.set_device(device)
+    if world > 1 and hparams.extrinsics_lr > 0:
+        raise ValueError("--extrinsics_lr trains on one GPU: the pose gradient is not exchanged between ranks")
     if world > 1:
         torch.distributed.init_process_group("nccl", device_id=device)
 
@@ -105,7 +109,12 @@ def main(prefix_args=None):
     voxel_reg = None
     if hparams.model_name == 'svox':   # total variation / sparsity weights; all 0 (the default) enqueue nothing
         voxel_reg = (hparams.tv_sigma_loss_w, hparams.tv_sh_loss_w, hparams.sparsity_loss_w)
-    trainer = NGPTrainer(model, lr=hparams.lr, max_steps=hparams.max_steps, voxel_reg=voxel_reg)
+    extrinsics = None
+    if hparams.extrinsics_lr > 0:   # per-image pose corrections (DESIGN.md §6i)
+        from taichi_nerfs_b200.extrinsics import PoseRefinement
+        extrinsics = PoseRefinement(train_dataset.poses, hparams.extrinsics_lr / hparams.lr)
+    trainer = NGPTrainer(model, lr=hparams.lr, max_steps=hparams.max_steps, voxel_reg=voxel_reg,
+                         extrinsics=extrinsics)
 
     # --random_bg (DESIGN.md §6f): every training ray gets its own background colour, drawn on the device
     bg_load = getattr(train_dataset, 'bg_load', 1.0)
@@ -118,7 +127,8 @@ def main(prefix_args=None):
         from taichi_nerfs_b200.fast_step import StaticTrainStep
         fast = StaticTrainStep(trainer, hparams.batch_size, exp_step_factor=exp_step_factor,
                                distortion_loss_w=hparams.distortion_loss_w, random_bg=hparams.random_bg,
-                               bg_seed=seed + rank, bg_load=bg_load, depth_loss_w=hparams.depth_loss_w)
+                               bg_seed=seed + rank, bg_load=bg_load, depth_loss_w=hparams.depth_loss_w,
+                               extrinsics=extrinsics)
 
     tic = time.time()
     for step in range(hparams.max_steps + 1):
@@ -127,7 +137,13 @@ def main(prefix_args=None):
         with torch.autocast(device_type='cuda', dtype=torch.float16):
             if step % update_interval == 0:
                 model.update_density_grid(0.01 * MAX_SAMPLES / 3 ** 0.5, warmup=step < warmup_steps)
-        rays_o, rays_d = get_rays(data['direction'], data['pose'])
+        img_idxs = rays_o = rays_d = None
+        if extrinsics is not None:   # same_image gives one index: the kernels broadcast it
+            img_idxs = torch.as_tensor(data['img_idxs'], device=device)
+            if fast is None:         # the graph step forms the rays from the corrected poses itself
+                rays_o, rays_d = extrinsics.rays(data['direction'], img_idxs)
+        else:
+            rays_o, rays_d = get_rays(data['direction'], data['pose'])
         depth = None
         if hparams.depth_loss_w > 0:
             depth = data.get('depth')
@@ -141,8 +157,12 @@ def main(prefix_args=None):
             terms.append(lambda res: hparams.depth_loss_w * depth_loss(res, depth).mean())
         extra_loss = (lambda res: sum(f(res) for f in terms)) if terms else None  # noqa: E731
         if fast is not None:   # one graph replay, nothing synchronises the host
-            loss = fast.step(rays_o, rays_d, data['rgb'], alpha=data.get('alpha') if hparams.random_bg else None,
-                             depth=depth)
+            if extrinsics is not None:   # the step forms the rays from the corrected poses itself
+                loss = fast.step(None, None, data['rgb'], alpha=data.get('alpha') if hparams.random_bg else None,
+                                 depth=depth, directions=data['direction'], img_idxs=img_idxs)
+            else:
+                loss = fast.step(rays_o, rays_d, data['rgb'],
+                                 alpha=data.get('alpha') if hparams.random_bg else None, depth=depth)
             results = {'rgb': fast.rgb, 'rm_samples': fast.counter[0].clamp(max=fast.cap), 'vr_samples':
                        fast.counter[0].clamp(max=fast.cap), 'dropped_rays': fast.counter[1]}
         else:
@@ -150,7 +170,7 @@ def main(prefix_args=None):
             if hparams.random_bg:   # the colours of step trainer.step_count + 1, as the graph step draws them
                 bg_rgb = ops.random_bg(seed + rank, trainer.step_count + 1, len(rays_o), device)
             loss, results = trainer.step(rays_o, rays_d, data['rgb'], exp_step_factor, extra_loss=extra_loss,
-                                         bg_rgb=bg_rgb, alpha=data.get('alpha'), b_load=bg_load)
+                                         bg_rgb=bg_rgb, alpha=data.get('alpha'), b_load=bg_load, img_idxs=img_idxs)
 
         if step % 1000 == 0 and rank == 0:
             with torch.no_grad():
@@ -168,6 +188,11 @@ def main(prefix_args=None):
         save_deployment_model(model=model, dataset=train_dataset, save_dir=hparams.deployment_model_path)
     os.makedirs(val_dir, exist_ok=True)
     torch.save(model.state_dict(), os.path.join(val_dir, 'model.pth'))
+    if extrinsics is not None:
+        np.save(os.path.join(val_dir, 'poses_refined.npy'), extrinsics.refined_poses())
+        rot_deg, trans = extrinsics.mean_correction()
+        print(f"extrinsics: mean |omega| = {rot_deg:.4f} deg | mean |tau| = {trans:.6f} -> "
+              f"{os.path.join(val_dir, 'poses_refined.npy')}")
 
     # test loop (train.py:237-304): PSNR and SSIM per held-out view; first view saved as PNG
     model.eval()
