@@ -333,13 +333,16 @@ __global__ void __launch_bounds__(kThreads) hash_fwd_kernel(const float* __restr
 // new cell is a neighbour of the old one, only the corners that leave are scattered and the shared ones
 // keep accumulating (cell_step): another 25 % fewer atomics on the lego_half sample stream
 // (scripts/hash_corner_reuse.py).  The forward does not carry corners: there it saved loads but not time.
+// At most 56 registers (ptxas alone picks 63): the scatter waits on L2 atomics and loads, and what hides that latency
+// is warps per SM.  56 lets three CTAs of the coarse level group (11 levels, 352 threads) fit per SM instead of two,
+// and seven of the fine group (5 levels) instead of six; 48 would spill.  DESIGN.md §4 has the measurements.
 template <typename T>
-__global__ void __launch_bounds__(kThreads) hash_bwd_kernel(const float* __restrict__ xyz,
-                                                            const T* __restrict__ dout,
-                                                            const __grid_constant__ ngp_hash_layout lay,
-                                                            float* __restrict__ grad_table, int64_t n_max,
-                                                            const Dyn dyn, int level_begin, int level_end,
-                                                            int32_t* __restrict__ found_inf, int grouped) {
+__global__ void __maxnreg__(56) hash_bwd_kernel(const float* __restrict__ xyz,
+                                                const T* __restrict__ dout,
+                                                const __grid_constant__ ngp_hash_layout lay,
+                                                float* __restrict__ grad_table, int64_t n_max,
+                                                const Dyn dyn, int level_begin, int level_end,
+                                                int32_t* __restrict__ found_inf, int grouped) {
     // blockDim.x = 32 * (level_end - level_begin): warp w scatters level level_begin + w.  The host launches one level
     // group at a time (bwd_level_groups), so only the group's dL/dout columns are staged: tile row w = level
     // level_begin + w.
