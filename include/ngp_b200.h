@@ -161,13 +161,20 @@ int ngp_raymarching_test(const float* rays_o, const float* rays_d, float* hits_t
 /* forward: replaces hash_encoder_kernel, modules/hash_encoder.py:89-143 (fp32
  * table, fp32 out [n, L*F]) and modules/hash_encoder_half.py:112-161 (fp16 table,
  * fp16 accumulate, fp16 out [n, L, F]).  `dtype` selects NGP_F32 / NGP_F16 for
- * both `table` and `out`. */
+ * both `table` and `out`.  With feature_per_level == 2 the gather loads two
+ * neighbouring entries as one vector: `table` must be aligned to two entries
+ * (16 bytes fp32, 8 bytes fp16) and `out` to one (8 bytes fp32, 4 bytes fp16).
+ * Other widths need only element alignment.  The same holds for _dyn. */
 int ngp_hash_encode_fwd(const float* xyz, const void* table, const ngp_hash_layout* layout,
                         void* out, int dtype, int64_t n, void* stream);
 /* backward wrt the table: replaces hash_encoder_kernel.grad (Taichi autodiff,
  * modules/hash_encoder.py:265-277) and hash_encoder_backward_kernel
  * (modules/hash_encoder_half.py:164-213).  grad_table is fp32 [entries*F] and is
- * ACCUMULATED into (caller zeroes it, hash_encoder_half.py:350-352). */
+ * ACCUMULATED into (caller zeroes it, hash_encoder_half.py:350-352).  grad_table
+ * must be 8-byte aligned; with feature_per_level == 2 it must be 16-byte aligned
+ * (two neighbouring entries are added by one 16-byte reduction) and `dout`
+ * aligned to one entry (8 bytes fp32, 4 bytes fp16).  The same holds for _dyn
+ * and _levels. */
 int ngp_hash_encode_bwd(const float* xyz, const void* dout, int dout_dtype,
                         const ngp_hash_layout* layout, float* grad_table,
                         int64_t n, void* stream);

@@ -739,6 +739,13 @@ int ngp_hash_encode_fwd_dyn(const float* xyz, const void* table, const ngp_hash_
         NGP_LAUNCHED("hash_fwd_generic_kernel");
         return 0;
     }
+    // the gather loads an x-pair of entries as one vector from tab + (idx & ~1), and every access to out is at least
+    // one entry wide
+    const uintptr_t entry = dtype == NGP_F16 ? 4 : 8;
+    NGP_REQUIRE((reinterpret_cast<uintptr_t>(table) & (2 * entry - 1)) == 0,
+                "table must be aligned to two entries (16 bytes for fp32, 8 for fp16) when feature_per_level == 2");
+    NGP_REQUIRE((reinterpret_cast<uintptr_t>(out) & (entry - 1)) == 0,
+                "out must be aligned to one entry (8 bytes for fp32, 4 for fp16) when feature_per_level == 2");
     const unsigned grid = (unsigned)((n + kTile - 1) / kTile);
     if (int rc = configure_smem()) return rc;
     if (dtype == NGP_F16)
@@ -782,6 +789,12 @@ int ngp_hash_encode_bwd_levels(const float* xyz, const void* dout, int dout_dtyp
         NGP_LAUNCHED("hash_bwd_generic_kernel");
         return 0;
     }
+    // a flush scatters an x-pair of entries as one 16-byte reduction at g2 + (idx & ~1), and dL/dout is read at least
+    // one entry at a time
+    NGP_REQUIRE((reinterpret_cast<uintptr_t>(grad_table) & 15) == 0,
+                "grad_table must be 16-byte aligned when feature_per_level == 2");
+    NGP_REQUIRE((reinterpret_cast<uintptr_t>(dout) & (dout_dtype == NGP_F16 ? 3 : 7)) == 0,
+                "dout must be aligned to one entry (8 bytes for fp32, 4 for fp16) when feature_per_level == 2");
     const unsigned grid = (unsigned)((n + kTile - 1) / kTile);
     if (int rc = configure_smem()) return rc;
     // one launch per level group, in level order: each launch's scatter stays inside an L2-sized gradient slice

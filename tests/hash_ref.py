@@ -137,10 +137,12 @@ def np_hash_dx_f64(xn, table, dout, lay, half):
 
 
 def _level_ranges(lay):
+    """Level ranges of the table backward.  "inner" drops the first and the last level: at L = 16 both its ends are
+    odd, so the 16-byte staging of dL/dout (2 fp32 or 4 fp16 levels per load) must drop a column at either end."""
     L, fh = lay.levels, lay.begin_fast_hash_level
     mid = fh + (L - fh) // 2
     return {"all": (0, L), "dense": (0, fh), "hashed_coarse": (fh, mid), "hashed_fine": (mid, L),
-            "last": (L - 1, L), "level3": (3, 4)}
+            "last": (L - 1, L), "level3": (3, 4), "inner": (1, L - 1)}
 
 
 def _level_slice(lay, a, b):

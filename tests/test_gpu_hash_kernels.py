@@ -456,3 +456,29 @@ def test_hash_argument_validation_needs_no_gpu(lib):
     assert bwd_x(fake, fake, None, F32, C.byref(lay2), fake, 8, None) < 0
     assert b"null" in lib.ngp_last_error()
     assert fwd(fake, fake, None, fake, F32, 8, None) < 0
+    # F = 2: the forward loads an x-pair of entries as one vector and the backward adds one as a 16-byte reduction, so
+    # table must be aligned to two entries, grad_table to 16 bytes, out and dout to one entry
+    at = lambda off: C.c_void_p(0x10000 + off)   # noqa: E731
+    for dt, entry in ((F32, 8), (F16, 4)):
+        for off in (entry, 2, 2 * entry + entry // 2):
+            assert fwd(fake, at(off), C.byref(lay2), fake, dt, 8, None) < 0, (dt, off)
+            assert b"table must be aligned to two entries" in lib.ngp_last_error()
+            assert fwd_dyn(fake, at(off), C.byref(lay2), fake, dt, 8, None, None, None) < 0, (dt, off)
+        for off in (entry // 2, entry + entry // 2):
+            assert fwd(fake, fake, C.byref(lay2), at(off), dt, 8, None) < 0, (dt, off)
+            assert b"out must be aligned to one entry" in lib.ngp_last_error()
+            assert bwd(fake, at(off), dt, C.byref(lay2), fake, 8, None) < 0, (dt, off)
+            assert b"dout must be aligned to one entry" in lib.ngp_last_error()
+        assert bwd(fake, fake, dt, C.byref(lay2), at(8), 8, None) < 0
+        assert b"grad_table must be 16-byte aligned" in lib.ngp_last_error()
+        assert bwd_dyn(fake, fake, dt, C.byref(lay2), at(24), 8, None, None, None) < 0
+        assert b"grad_table must be 16-byte aligned" in lib.ngp_last_error()
+        for a, b in ((0, 16), (3, 7), (15, 16)):
+            assert bwd_lv(fake, fake, dt, C.byref(lay2), at(8), 8, None, None, a, b, None, None) < 0, (a, b)
+            assert b"grad_table must be 16-byte aligned" in lib.ngp_last_error()
+        assert bwd(fake, fake, dt, C.byref(lay2), at(4), 8, None) < 0
+        assert b"grad_table must be 8-byte aligned" in lib.ngp_last_error()
+    # other widths keep their element-wise rule: grad_table 8-byte aligned
+    lay4 = make_hash_layout(2 ** 16, 6, 16, 512, 4).as_ctypes()
+    assert bwd(fake, fake, F32, C.byref(lay4), at(4), 8, None) < 0
+    assert b"grad_table must be 8-byte aligned" in lib.ngp_last_error()

@@ -122,7 +122,7 @@ def _bwd_inputs(rng, n, half):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("group", ["all", "dense", "hashed_coarse", "hashed_fine", "last", "level3"])
+@pytest.mark.parametrize("group", ["all", "dense", "hashed_coarse", "hashed_fine", "last", "level3", "inner"])
 @pytest.mark.parametrize("half", [False, True])
 def test_hash_bwd_levels_fp64_bound(lib, half, group):
     lay = _layout(1024)
