@@ -58,6 +58,18 @@ class BaseDataset(Dataset):
             self.depths = self.depths.to(device)
         return self
 
+    def gather(self, img_idxs, pix_idxs):
+        """The training sample of the rays (img_idxs[i], pix_idxs[i]): the dict a training split's ``dataset[idx]``
+        returns for those indices (``img_idxs`` may be one index for the whole batch, as 'same_image' gives)."""
+        rays = self.rays[img_idxs, pix_idxs]
+        sample = {'img_idxs': img_idxs, 'pix_idxs': pix_idxs, 'pose': self.poses[img_idxs],
+                  'direction': self.directions[pix_idxs], 'rgb': rays[:, :3]}
+        if getattr(self, 'depths', None) is not None:
+            sample['depth'] = self.depths[img_idxs, pix_idxs]
+        if rays.shape[-1] == 4:
+            sample['alpha'] = rays[:, 3]
+        return sample
+
     def __getitem__(self, idx):
         if self.split.startswith('train'):
             dev = self.rays.device
@@ -68,11 +80,7 @@ class BaseDataset(Dataset):
             else:
                 raise ValueError(f"unknown ray_sampling_strategy {self.ray_sampling_strategy!r}")
             pix_idxs = torch.randint(0, self.img_wh[0] * self.img_wh[1], size=(self.batch_size,), device=dev)
-            rays = self.rays[img_idxs, pix_idxs]
-            sample = {'img_idxs': img_idxs, 'pix_idxs': pix_idxs, 'pose': self.poses[img_idxs],
-                      'direction': self.directions[pix_idxs], 'rgb': rays[:, :3]}
-            if getattr(self, 'depths', None) is not None:
-                sample['depth'] = self.depths[img_idxs, pix_idxs]
+            return self.gather(img_idxs, pix_idxs)
         else:
             sample = {'pose': self.poses[idx], 'img_idxs': idx}
             if len(self.rays) > 0:

@@ -133,6 +133,25 @@ class SyntheticLego:
         pix = torch.randint(0, self.img_wh[0] * self.img_wh[1], (n,), device=dev, generator=self._gen)
         return img, pix
 
+    def gather(self, img, pix):
+        """The training sample of the rays (img[i], pix[i]), as ``dataset[idx]`` returns it for those indices.  The
+        random scene's colours are not a function of the pixel: they are drawn from the dataset's generator."""
+        sample = {'img_idxs': img, 'pix_idxs': pix, 'pose': self.poses[img], 'direction': self.directions[pix]}
+        if self.with_rgb:
+            if self.scene == 'analytic':
+                from .ray_utils import get_rays
+                o, d = get_rays(sample['direction'], sample['pose'])
+                if self.with_depth:
+                    sample['rgb'], sample['depth'] = render_teacher(o, d, return_depth=True)
+                else:
+                    sample['rgb'] = render_teacher(o, d)
+            else:
+                dev = self.poses.device
+                if self._gen is None or self._gen.device != dev:
+                    self._gen = torch.Generator(device=dev).manual_seed(self._seed)
+                sample['rgb'] = torch.rand(pix.shape[0], 3, device=dev, generator=self._gen)
+        return sample
+
     def __getitem__(self, idx):
         dev = self.poses.device
         if self._gen is None or self._gen.device != dev:
@@ -140,18 +159,7 @@ class SyntheticLego:
         n = self.batch_size
         if self.split.startswith('train'):
             img, pix = self._draw(idx, n, dev)
-            sample = {'img_idxs': img, 'pix_idxs': pix, 'pose': self.poses[img], 'direction': self.directions[pix]}
-            if self.with_rgb:
-                if self.scene == 'analytic':
-                    from .ray_utils import get_rays
-                    o, d = get_rays(sample['direction'], sample['pose'])
-                    if self.with_depth:
-                        sample['rgb'], sample['depth'] = render_teacher(o, d, return_depth=True)
-                    else:
-                        sample['rgb'] = render_teacher(o, d)
-                else:
-                    sample['rgb'] = torch.rand(n, 3, device=dev, generator=self._gen)
-            return sample
+            return self.gather(img, pix)
         sample = {'pose': self.poses[idx], 'img_idxs': idx}
         if self.scene == 'analytic':
             from .ray_utils import get_rays

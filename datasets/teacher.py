@@ -86,17 +86,23 @@ class TeacherLego(SyntheticLego):
         self.rays = self.images
         return self.rays
 
+    def gather(self, img, pix):
+        """The training sample of the rays (img[i], pix[i]), as ``dataset[idx]`` returns it for those indices."""
+        if self.images is None:
+            self.build_image_bank()
+        sample = {'img_idxs': img, 'pix_idxs': pix, 'pose': self.poses[img], 'direction': self.directions[pix],
+                  'rgb': self.images[img, pix]}
+        if self.with_depth:
+            sample['depth'] = self.depths[img, pix]
+        return sample
+
     def __getitem__(self, idx):
         if self.images is None:
             self.build_image_bank()
         dev = self.poses.device
         if self.split.startswith('train'):
             img, pix = self._draw(idx, self.batch_size, dev)
-            sample = {'img_idxs': img, 'pix_idxs': pix, 'pose': self.poses[img], 'direction': self.directions[pix],
-                      'rgb': self.images[img, pix]}
-            if self.with_depth:
-                sample['depth'] = self.depths[img, pix]
-            return sample
+            return self.gather(img, pix)
         sample = {'pose': self.poses[idx], 'img_idxs': idx, 'rgb': self.images[idx]}
         if self.with_depth:
             sample['depth'] = self.depths[idx]

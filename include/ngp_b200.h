@@ -660,6 +660,42 @@ int ngp_pose_adam(float* corr, float* grad, float* exp_avg, float* exp_avg_sq, c
                   const float* hyper_dev, float lr_ratio, float beta1, float beta2, float eps, int64_t n_img,
                   void* stream);
 
+/* ---- error-map ray sampling (DESIGN.md §6j) ---------------------------------------------------------------------
+ * Each of n_img images (W x H) is cut into R x R tiles (0 < R <= min(W, H), n_img W H < 2^40); pixel pix = y W + x
+ * lies in tile t = img R^2 + floor(y R / H) R + floor(x R / W) of T = n_img R^2.  Map state: E [T] uint64 (per-tile
+ * error, fixed point 2^30), acc [T] uint64, cnt [T] uint32, cdf [T] uint64 (inclusive prefix sum of the masses).
+ * ngp_error_map_sample: per ray i, Philox4x32-10 with counter (i, i >> 32, step, 0x656d0001) and key (seed, seed >> 32)
+ * gives r0..r2; v = floor(((r0 << 32) | r1) M / 2^64) with M = cdf[T-1]; t = the first tile with cdf[t] > v; the pixel
+ * is number floor(r2 n_t / 2^32) of tile t in row-major order; w = (float)(((double)M n_t) / ((double)N_pix m_t)),
+ * N_pix = n_img W H, m_t = cdf[t] - cdf[t-1].  step = *step_dev when step_dev is given (graph-capturable).
+ * ngp_error_map_accumulate: per ray, target' = target + (bg_rgb - b_load)(1 - alpha) when bg_rgb and alpha are given
+ * (the random-background head's target, strict fp32), e = sum_c (pred_c - target'_c)^2 (strict fp32), clamped to
+ * [0, 3] (NaN counts as 3), u = floor(e 2^30); img and pix are clamped as ngp_sample_ray_batch clamps them;
+ * acc[t] += u, cnt[t] += 1 with integer atomics (bit-reproducible).
+ * ngp_error_map_rebuild: where cnt > 0, E += (acc / cnt - E) >> ema_shift (integer division, arithmetic shift); acc
+ * and cnt are cleared.  Then E' = E >> k with k the least shift such that max E' <= lim, lim = floor(((q - p)(2^53 -
+ * N_pix) - 1) / (N_pix q)), p / q = floor_num / floor_den (the floor alpha); S = sum n_t E'_t;
+ * c = max(1, ceil(p S / ((q - p) N_pix))); m_t = n_t (E'_t + c) >= 1; cdf = inclusive scan of m.  So every pixel has
+ * probability >= alpha / N_pix, every weight is <= 1 / alpha and M = cdf[T-1] < 2^53.  workspace: at least
+ * ngp_error_map_workspace_bytes(T) bytes of device memory; its words 0..5 are (max E, S, M, status, k, c) afterwards,
+ * status = 1 if M >= 2^53 (cannot happen when lim holds).  Capture-safe (one memset node, five kernels).
+ * ngp_ray_grad_weight: for each row (ray, start, count) of rays_a (count clipped to n_rows), the per-sample gradients
+ * dL_dsigmas[s] and dL_drgbs[s, 0..2] (fp32 or fp16, rgbs_dtype) of rows [start, start + count) become their product
+ * with w[ray], rounded once; found_inf (optional) is set to 1 when a stored result is not finite (fp16 overflow
+ * included). */
+int64_t ngp_error_map_workspace_bytes(int64_t n_tiles);
+int ngp_error_map_sample(const uint64_t* cdf, int64_t n_img, int64_t W, int64_t H, int64_t R, uint64_t seed,
+                         const int32_t* step_dev, int32_t step_host, int64_t* img_out, int64_t* pix_out, float* w_out,
+                         int64_t n_rays, void* stream);
+int ngp_error_map_accumulate(const float* pred, const float* target, const float* bg_rgb, const float* alpha,
+                             float b_load, const int64_t* img_idxs, const int64_t* pix_idxs, int64_t n_img, int64_t W,
+                             int64_t H, int64_t R, uint64_t* acc, uint32_t* cnt, int64_t n_rays, void* stream);
+int ngp_error_map_rebuild(uint64_t* E, uint64_t* acc, uint32_t* cnt, uint64_t* cdf, int64_t n_img, int64_t W,
+                          int64_t H, int64_t R, int ema_shift, int floor_num, int floor_den, void* workspace,
+                          int64_t workspace_bytes, void* stream);
+int ngp_ray_grad_weight(const int32_t* rays_a, const float* w, float* dL_dsigmas, void* dL_drgbs, int rgbs_dtype,
+                        int32_t* found_inf_or_null, int64_t n_rays, int64_t n_rows, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -3,6 +3,7 @@ flag table is restated here as data; `--dataset_name synthetic | teacher` and th
 are the additions)."""
 import argparse
 import math
+import os
 
 # (flag, kwargs)
 _FLAGS = [
@@ -49,9 +50,15 @@ _FLAGS = [
                                                            'densities, 0 to disable (default; svox only)')),
     # training options
     ('--batch_size', dict(type=int, default=8192, help='number of rays in a batch')),
-    ('--ray_sampling_strategy', dict(type=str, default='all_images', choices=['all_images', 'same_image'],
+    ('--ray_sampling_strategy', dict(type=str, default='all_images', choices=['all_images', 'same_image', 'error_map'],
                                      help='all_images: uniformly from all pixels of ALL images; '
-                                          'same_image: uniformly from all pixels of a SAME image')),
+                                          'same_image: uniformly from all pixels of a SAME image; '
+                                          'error_map: from all pixels of all images in proportion to their tile\'s '
+                                          'recent error, each ray\'s loss weighted to keep the objective unbiased '
+                                          '(DESIGN.md §6j; one GPU)')),
+    ('--error_map_res', dict(type=int, default=64,
+                             help='tiles per image side of the error map (clamped to the image size), '
+                                  'with --ray_sampling_strategy error_map')),
     ('--max_steps', dict(type=int, default=20000, help='number of steps to train')),
     ('--lr', dict(type=float, default=1e-2, help='learning rate')),
     ('--random_bg', dict(action='store_true', default=False, help='train with random bg color (real scene only)')),
@@ -106,6 +113,10 @@ def get_opts(prefix_args=None):
     if hparams.depth_loss_w > 0 and hparams.dataset_name in ('nerf', 'nsvf', 'colmap'):
         parser.error(f"--depth_loss_w: the {hparams.dataset_name} loader reads no depth (the ngp loader reads "
                      f"transforms.json's depth_path)")
+    if not 1 <= hparams.error_map_res <= 4096:
+        parser.error(f"--error_map_res must be in [1, 4096], got {hparams.error_map_res}")
+    if hparams.ray_sampling_strategy == 'error_map' and int(os.environ.get("WORLD_SIZE", "1")) > 1:
+        parser.error("--ray_sampling_strategy error_map trains on one GPU: the error map is not shared between ranks")
     if not (math.isfinite(hparams.extrinsics_lr) and hparams.extrinsics_lr >= 0):
         parser.error(f"--extrinsics_lr must be finite and >= 0, got {hparams.extrinsics_lr}")
     if hparams.extrinsics_lr > 0:

@@ -12,6 +12,11 @@ With camera extrinsics refinement (DESIGN.md §6i) the rays come from the pose-a
 camera directions and image indices), the hash backward is followed by the position gradient and the pose gradient,
 and the corrections' Adam runs next to the model's.
 
+With error-map sampling (DESIGN.md §6j) each ray carries a weight w_r: the head is followed by the error-map accumulate
+(the rays' errors into their tiles) and by the gradient weight (every per-sample gradient of ray r times w_r), so the
+backward sees the gradient of the weighted loss; loss_sum, the logged value, stays the unweighted one.  The sampled step
+draws its pixels with the error-map sampler, whose indices the batch sampler then reads.
+
 A voxel-grid model (--model_name svox) has no network: the march feeds the voxel forward (fp32 sigma / rgb) -> head ->
 voxel backward -> [regularisers] -> finite check and Adam over the fields' node block B only (DESIGN.md §6b).
 
@@ -40,7 +45,7 @@ class StaticTrainStep:
                  T_threshold: float = 1e-4, max_samples: int = 1024, use_graph: bool = True,
                  dynamic_loss_scale: bool = True, overlap_optimizer: bool = False, distortion_loss_w: float = 0.0,
                  random_bg: bool = False, bg_seed: int = 0, bg_load: float = 1.0, depth_loss_w: float = 0.0,
-                 extrinsics=None):
+                 extrinsics=None, error_map=None):
         self.tr = trainer
         m = self.model = trainer.model
         # the voxel-grid model: fp32 fields and outputs, no encoder and no MLP; its optimizer pass covers the node
@@ -58,6 +63,8 @@ class StaticTrainStep:
             raise ValueError("StaticTrainStep: extrinsics must be the trainer's PoseRefinement "
                              "(NGPTrainer(extrinsics=...)), or None for a trainer without one")
         self.ext = extrinsics
+        # error_map: a taichi_nerfs_b200.error_map.ErrorMap over the training images, or None (nothing is enqueued)
+        self.em = error_map
         if self.ext is not None and overlap_optimizer:
             raise _lib.NgpError("StaticTrainStep: extrinsics refinement does not combine with overlap_optimizer (the "
                                 "next step's march would read poses one update stale)")
@@ -112,6 +119,10 @@ class StaticTrainStep:
             self.cam_dirs, self.img_idx = z(self.n, 3), torch.zeros(self.n, device=dev, dtype=torch.int64)
             self.cam_dirs[:, 2] = -1.0   # valid placeholder rays for the capture (a zero direction never advances)
             self.dx = z(C_, 3)
+        if self.em is not None:   # each ray's image, pixel and loss weight
+            self.em_img = torch.zeros(self.n, device=dev, dtype=torch.int64)
+            self.em_pix = torch.zeros(self.n, device=dev, dtype=torch.int64)
+            self.ray_w = torch.ones(self.n, device=dev)
         # GradScaler state on the device: [scale, growth_tracker (int bits)]; growth 2x / 2000 clean steps, backoff 0.5
         trainer.dynamic_loss_scale = self.dynamic_loss_scale = bool(dynamic_loss_scale)
         self.aabb6 = (C.c_float * 6)(*[float(v) for v in m.xyz_min.flatten().tolist()],
@@ -299,18 +310,36 @@ class StaticTrainStep:
                                        _p(self.drgbs), C.byref(self._clayout), _p(dsh), _p(dden), self.cap,
                                        _p(self.counter), None, self._st()))
 
+    # error-map sampling (DESIGN.md §6j): the rays' errors into the map, then the per-ray loss weights
+    def _k_em_accumulate(self):
+        em = self.em
+        rbg = self.random_bg
+        check(load().ngp_error_map_accumulate(_p(self.rgb), _p(self.gt), _p(self.bg_rgb) if rbg else None,
+                                              _p(self.alpha) if rbg else None, self.bg_load, _p(self.em_img),
+                                              _p(self.em_pix), *em.geom, _p(em.acc), _p(em.cnt), self.n, self._st()))
+
+    def _k_grad_weight(self):
+        check(load().ngp_ray_grad_weight(_p(self.rays_a), _p(self.ray_w), _p(self.dsig), _p(self.drgbs),
+                                         F32 if self.vox else F16, _p(self.tr.found_inf), self.n, self.cap, self._st()))
+
+    def _k_head_weighted(self):
+        self._k_head()
+        if self.em is not None:
+            self._k_em_accumulate()
+            self._k_grad_weight()
+
     def _enqueue_network(self):
         # counter[0] = number of valid sample rows, read on the device by every kernel
         if self.vox:
             self._k_voxel_fwd()
-            self._k_head()
+            self._k_head_weighted()
             self._k_voxel_bwd()
             if self.tr.voxel_reg is not None:   # TV / sparsity over B, scaled by the device loss scale
                 self.tr.add_voxel_reg()
             return
         self._k_hash_fwd()
         self._k_mlp_fwd()
-        self._k_head()
+        self._k_head_weighted()
         self._k_mlp_bwd()
         self._k_hash_bwd()
         if self.ext is not None:
@@ -320,8 +349,13 @@ class StaticTrainStep:
     def _enqueue_sampler(self):
         """datasets/base.py:34-61 + ray_utils.py:51-80 + the marching jitter, keyed by (seed, batch counter, ray)."""
         src = self.src
+        em, img, pix = self.em, None, None
+        if em is not None:   # the pixels come from the error map; the batch sampler gathers them
+            check(load().ngp_error_map_sample(_p(em.cdf), *em.geom, em.seed & 0xFFFFFFFFFFFFFFFF, _p(self.sample_step),
+                                              0, _p(self.em_img), _p(self.em_pix), _p(self.ray_w), self.n, self._st()))
+            img, pix = _p(self.em_img), _p(self.em_pix)
         check(load().ngp_sample_ray_batch(_p(src["bank"]), src["bank"].shape[2], _p(src["poses"]), _p(src["dirs"]),
-                                          src["poses"].shape[0], src["dirs"].shape[0], None, None, src["fixed_img"],
+                                          src["poses"].shape[0], src["dirs"].shape[0], img, pix, src["fixed_img"],
                                           src["seed"], _p(self.sample_step), 0, _p(self.rays_o), _p(self.rays_d),
                                           _p(self.gt), _p(self.noise), None, None, self.n, self._st()))
 
@@ -365,6 +399,7 @@ class StaticTrainStep:
         scale_keep, hyper_keep, sample_keep = self.scale_state.clone(), self.hyper.clone(), self.sample_step.clone()
         bg_step_keep = self.bg_step.clone()
         ext_keep = [] if self.ext is None else [t.clone() for t in self.ext.state()]
+        em_keep = [] if self.em is None else [t.clone() for t in self.em.state()]
         shadow = None if tr._shadow_full is None else tr._shadow_full.clone()
         side = torch.cuda.Stream()
         side.wait_stream(torch.cuda.current_stream())
@@ -391,27 +426,41 @@ class StaticTrainStep:
         if self.ext is not None:
             for t, k in zip(self.ext.state(), ext_keep):
                 t.copy_(k)
+        if self.em is not None:
+            for t, k in zip(self.em.state(), em_keep):
+                t.copy_(k)
         tr.flat_grad.zero_()
         if shadow is not None:
             tr._shadow_full.copy_(shadow)
         self._graphs[(sampled, mode)], self._kernels[(sampled, mode)] = graph, kernels
 
     # ---------------------------------------------------------------------------------------------
-    def step(self, rays_o, rays_d, rgb_gt, noise=None, alpha=None, depth=None, directions=None, img_idxs=None):
+    def step(self, rays_o, rays_d, rgb_gt, noise=None, alpha=None, depth=None, directions=None, img_idxs=None,
+             ray_w=None, pix_idxs=None):
         """Enqueues one full training step; returns the (device) loss tensor — nothing is synchronised.  ``alpha`` [N]
         (random_bg only): the images' alpha, whose transparent part of the target gets the ray's colour.  ``depth`` [N]
         (depth_loss_w > 0 only, where it is required): each ray's target z-depth, 0 where there is none.  With
         extrinsics refinement the step forms its rays itself: rays_o and rays_d are None and ``directions`` [N, 3]
-        (camera frame) and ``img_idxs`` [N] (or one index for the whole batch) are required."""
+        (camera frame) and ``img_idxs`` [N] (or one index for the whole batch) are required.  With an error map,
+        ``ray_w`` [N] (the loss weights of ErrorMap.draw), ``img_idxs`` and ``pix_idxs`` [N] are required."""
+        if self.em is not None:
+            if ray_w is None or img_idxs is None or pix_idxs is None:
+                raise ValueError("error-map sampling: step(..., ray_w=..., img_idxs=..., pix_idxs=...) (the rays' loss "
+                                 "weights and the tiles their errors go to)")
+            self.ray_w.copy_(ray_w, non_blocking=True)
+            self.em_img.copy_(torch.as_tensor(img_idxs, device=self.dev).reshape(-1), non_blocking=True)
+            self.em_pix.copy_(pix_idxs, non_blocking=True)
+        elif ray_w is not None or pix_idxs is not None:
+            raise ValueError("ray_w / pix_idxs are read by error-map sampling only (StaticTrainStep(error_map=...))")
         if self.ext is not None:
             if directions is None or img_idxs is None or rays_o is not None or rays_d is not None:
                 raise ValueError("extrinsics refinement: step(None, None, rgb, ..., directions=..., img_idxs=...) "
                                  "(the step forms the rays from the corrected poses)")
             self.cam_dirs.copy_(directions, non_blocking=True)
             self.img_idx.copy_(torch.as_tensor(img_idxs, device=self.dev).reshape(-1), non_blocking=True)
-        elif directions is not None or img_idxs is not None:
-            raise ValueError("directions / img_idxs are read by extrinsics refinement only "
-                             "(StaticTrainStep(extrinsics=...))")
+        elif directions is not None or (img_idxs is not None and self.em is None):
+            raise ValueError("directions / img_idxs are read by extrinsics refinement and error-map sampling only "
+                             "(StaticTrainStep(extrinsics=... | error_map=...))")
         if depth is None and self.depth_w > 0:
             raise ValueError("depth_loss_w > 0 needs each ray's target depth: step(..., depth=...)")
         if depth is not None and self.depth_w == 0:
@@ -481,6 +530,11 @@ class StaticTrainStep:
         bank, poses, directions = f(image_bank), f(poses), f(directions)
         if bank.ndim != 3 or bank.shape[0] != poses.shape[0] or bank.shape[1] != directions.shape[0] or bank.shape[2] < 3:
             raise ValueError(f"image bank {tuple(bank.shape)} vs {poses.shape[0]} poses x {directions.shape[0]} pixels")
+        if self.em is not None and (self.em.n_img != bank.shape[0] or self.em.W * self.em.H != bank.shape[1]
+                                    or int(fixed_img) >= 0):
+            raise ValueError(f"the error map covers {self.em.n_img} images of {self.em.W}x{self.em.H} pixels, all "
+                             f"drawn; the image bank is {tuple(bank.shape)}" + (f", fixed_img {fixed_img}"
+                                                                                if int(fixed_img) >= 0 else ""))
         self.src = dict(bank=bank, poses=poses.reshape(-1, 3, 4), dirs=directions, seed=int(seed),
                         fixed_img=int(fixed_img))
         if self.use_graph:

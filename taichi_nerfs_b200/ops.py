@@ -553,6 +553,74 @@ def pose_adam(corr, grad, exp_avg, exp_avg_sq, hyper, lr_ratio, found_inf=None, 
           "pose_adam")
 
 
+# ---- error-map ray sampling (DESIGN.md §6j) ---------------------------------------------------------------------
+def _map_buffers(n_tiles, **ts):
+    want = {"E": torch.int64, "acc": torch.int64, "cnt": torch.int32, "cdf": torch.int64}
+    for k, t in ts.items():
+        if t.dtype != want[k] or not t.is_contiguous() or t.numel() != n_tiles:
+            raise TypeError(f"error map: {k} must be a contiguous {want[k]} tensor of {n_tiles} tiles")
+
+
+def error_map_sample(cdf, geom, n_rays, seed, step=0, step_dev=None, out=None):
+    """(img [n] int64, pix [n] int64, w [n] fp32) drawn from the map's CDF; geom = (n_img, W, H, R).  ``out`` = optional
+    (img, pix, w) buffers to write (graph capture); ``step_dev`` an int32 device scalar read instead of ``step``."""
+    _need_cuda(cdf, step_dev)
+    n_img, W, H, R = (int(v) for v in geom)
+    _map_buffers(n_img * R * R, cdf=cdf)
+    if step_dev is not None and step_dev.dtype != torch.int32:
+        raise TypeError("error_map_sample: step_dev must be int32")
+    n = int(n_rays)
+    if out is None:
+        out = (torch.empty(n, device=cdf.device, dtype=torch.int64), torch.empty(n, device=cdf.device, dtype=torch.int64),
+               torch.empty(n, device=cdf.device, dtype=torch.float32))
+    img, pix, w = out
+    check(load().ngp_error_map_sample(_ptr(cdf), n_img, W, H, R, int(seed) & 0xFFFFFFFFFFFFFFFF, _ptr(step_dev),
+                                      int(step), _ptr(img), _ptr(pix), _ptr(w), n, _stream()), "error_map_sample")
+    return img, pix, w
+
+
+def error_map_accumulate(pred, target, img_idxs, pix_idxs, geom, acc, cnt, bg_rgb=None, alpha=None, b_load=1.0):
+    """acc[t] += floor(min(sum_c (pred - target')^2, 3) 2^30), cnt[t] += 1 per ray; target' = target + (bg_rgb -
+    b_load)(1 - alpha) when bg_rgb and alpha are given (the random-background head's target)."""
+    _need_cuda(pred, target, img_idxs, pix_idxs, acc, cnt, bg_rgb, alpha)
+    n_img, W, H, R = (int(v) for v in geom)
+    _map_buffers(n_img * R * R, acc=acc, cnt=cnt)
+    p, t = _f32c(pred), _f32c(target)
+    n = p.shape[0]
+    bg = None if bg_rgb is None else _f32c(bg_rgb)
+    a = None if alpha is None else _f32c(alpha)
+    ii, pi = img_idxs.to(torch.int64).contiguous(), pix_idxs.to(torch.int64).contiguous()
+    if t.shape[0] != n or ii.numel() != n or pi.numel() != n or (bg is not None and bg.shape[0] != n) \
+            or (a is not None and a.numel() != n):
+        raise ValueError("error_map_accumulate: every per-ray input needs one row per ray")
+    check(load().ngp_error_map_accumulate(_ptr(p), _ptr(t), _ptr(bg), _ptr(a), float(b_load), _ptr(ii), _ptr(pi),
+                                          n_img, W, H, R, _ptr(acc), _ptr(cnt), n, _stream()), "error_map_accumulate")
+
+
+def error_map_rebuild(E, acc, cnt, cdf, geom, ema_shift, floor_num, floor_den, workspace):
+    """EMA of the interval's errors into E (acc, cnt cleared), masses and their inclusive scan into cdf."""
+    _need_cuda(E, acc, cnt, cdf, workspace)
+    n_img, W, H, R = (int(v) for v in geom)
+    _map_buffers(n_img * R * R, E=E, acc=acc, cnt=cnt, cdf=cdf)
+    check(load().ngp_error_map_rebuild(_ptr(E), _ptr(acc), _ptr(cnt), _ptr(cdf), n_img, W, H, R, int(ema_shift),
+                                       int(floor_num), int(floor_den), _ptr(workspace),
+                                       workspace.numel() * workspace.element_size(), _stream()), "error_map_rebuild")
+
+
+def ray_grad_weight(rays_a, w, dsigmas, drgbs, found_inf=None, n_rows=None):
+    """In place: every per-sample gradient of ray r (rows of rays_a [n, 3] = (ray, start, count)) times w[r]; dsigmas
+    [S] fp32, drgbs [S, 3] fp32 or fp16.  found_inf (int32 [1], optional) is raised on a non-finite result."""
+    _need_cuda(rays_a, w, dsigmas, drgbs, found_inf)
+    if rays_a.dtype != torch.int32 or w.dtype != torch.float32 or dsigmas.dtype != torch.float32:
+        raise TypeError("ray_grad_weight: rays_a int32, w and dsigmas fp32")
+    for t in (rays_a, w, dsigmas, drgbs):
+        if not t.is_contiguous():
+            raise ValueError("ray_grad_weight: contiguous tensors only (the gradients are updated in place)")
+    rows = dsigmas.shape[0] if n_rows is None else int(n_rows)
+    check(load().ngp_ray_grad_weight(_ptr(rays_a), _ptr(w), _ptr(dsigmas), _ptr(drgbs), _tag(drgbs), _ptr(found_inf),
+                                     rays_a.shape[0], rows, _stream()), "ray_grad_weight")
+
+
 def morton3d(coords):
     _need_cuda(coords)
     c = coords.contiguous()

@@ -20,10 +20,12 @@ DENSITY_THRESHOLD = 0.01 * 1024 / 3 ** 0.5   # train.py:180
 
 def train_vs_teacher(device, steps: int = 3000, batch: int = 8192, train_views: int = 48, test_views: int = 4,
                      downsample: float = 0.5, seed: int = 23, half_opt: bool = True, graph: bool = True,
-                     teacher=None, log=None, pos_encoder_type: str = 'hash'):
+                     teacher=None, log=None, pos_encoder_type: str = 'hash', ray_sampling: str = 'all_images'):
     """pos_encoder_type='triplane' trains the reference's tri-plane model instead (fp32 planes: half_opt does not
     apply and the loss scale is 2**19, as train.py without --half_opt).  graph=True trains through the graph-captured
     step (StaticTrainStep, either encoder), graph=False through NGPTrainer.step; "path" in the result says which.
+    ray_sampling='error_map' draws the training pixels from an ErrorMap (DESIGN.md §6j) rebuilt beside every density-grid
+    update, with the rays' loss weights; the result then also holds the map ("error_map").
     Returns {"psnr": mean dB over the held-out views, "psnr_views": [...], "ssim": mean SSIM over the same views (of
     the same clamped prediction), "ssim_views": [...], "steps": ..., "steps_per_s": ...,
     "rays_per_s": ..., "model": the trained NGP} or None when the teacher fixture is not staged."""
@@ -50,9 +52,15 @@ def train_vs_teacher(device, steps: int = 3000, batch: int = 8192, train_views: 
     model = NGP(scale=0.5, max_res=1024, half_opt=half_opt, pos_encoder_type=pos_encoder_type).to(device)
     model.mark_invisible_cells(train_ds.K, train_ds.poses, train_ds.img_wh)
     trainer = NGPTrainer(model, lr=1e-2, max_steps=steps)
+    if ray_sampling not in ('all_images', 'error_map'):
+        raise ValueError(f"ray_sampling must be 'all_images' or 'error_map', got {ray_sampling!r}")
+    em = None
+    if ray_sampling == 'error_map':
+        from .error_map import ErrorMap
+        em = ErrorMap(train_views, *train_ds.img_wh, seed=seed, device=device)
     fast = None
     if graph:
-        fast = StaticTrainStep(trainer, batch, samples_per_ray_capacity=384)
+        fast = StaticTrainStep(trainer, batch, samples_per_ray_capacity=384, error_map=em)
         fast.attach_ray_source(train_ds.rays, train_ds.poses, train_ds.directions, seed=seed)
     torch.cuda.synchronize(device)
     t0 = time.perf_counter()
@@ -62,8 +70,16 @@ def train_vs_teacher(device, steps: int = 3000, batch: int = 8192, train_views: 
                 fast.flush()
             with torch.autocast('cuda', dtype=torch.float16):
                 model.update_density_grid(DENSITY_THRESHOLD, warmup=step < 256)
+            if em is not None and step > 0:
+                em.rebuild()
         if fast is not None:
             loss = fast.step_sampled()
+        elif em is not None:
+            img, pix, w = em.draw(batch, step)
+            b = train_ds.gather(img, pix)
+            rays_o, rays_d = get_rays(b['direction'], b['pose'])
+            loss, res = trainer.step(rays_o, rays_d, b['rgb'], ray_w=w)
+            em.accumulate(res['rgb'].float(), b['rgb'], img, pix)
         else:
             b = train_ds[step]
             rays_o, rays_d = get_rays(b['direction'], b['pose'])
@@ -93,4 +109,5 @@ def train_vs_teacher(device, steps: int = 3000, batch: int = 8192, train_views: 
             "ssim_views": ssims, "steps": steps, "batch": batch,
             "train_views": train_views, "test_views": test_views, "image_wh": [w, h],
             "steps_per_s": steps / dt, "rays_per_s": steps * batch / dt, "train_seconds": dt,
-            "path": "graph" if graph else "modules", "model": model, "test_dataset": test_ds}
+            "path": "graph" if graph else "modules", "model": model, "test_dataset": test_ds,
+            "ray_sampling": ray_sampling, "error_map": em}

@@ -182,11 +182,13 @@ class NGPTrainer:
         self._views = []
 
     def forward_backward(self, rays_o, rays_d, rgb_gt, exp_step_factor=0.0, extra_loss=None, bg_rgb=None, alpha=None,
-                         b_load=1.0, img_idxs=None):
+                         b_load=1.0, img_idxs=None, ray_w=None):
         """bg_rgb [N, 3] (--random_bg, ops.random_bg): each ray's background colour replaces the fixed one; with
         ``alpha`` [N] (the image's alpha), the target's loader background ``b_load`` is replaced by it too:
         rgb_gt + (bg_rgb - b_load)(1 - alpha).  With extrinsics refinement, ``img_idxs`` [N] (or one index) names each
-        ray's image and rays_o / rays_d are the PoseRefinement's rays; the pose gradient is formed by optimizer_step."""
+        ray's image and rays_o / rays_d are the PoseRefinement's rays; the pose gradient is formed by optimizer_step.
+        ``ray_w`` [N] fp32 (error-map sampling, DESIGN.md §6j): the MSE becomes mean_r w_r mean_c (rgb - gt)^2, and the
+        returned loss is that weighted value; ``extra_loss`` weights its own per-ray terms."""
         from modules.rendering import render
         refine = self.extrinsics is not None
         if refine and img_idxs is None:
@@ -198,7 +200,10 @@ class NGPTrainer:
         with torch.autocast(device_type='cuda', dtype=torch.float16):
             results = render(self.model, rays_o, rays_d, exp_step_factor=exp_step_factor, bg_rgb=bg_rgb,
                              position_grad=refine)
-            loss = F.mse_loss(results['rgb'], rgb_gt)
+            if ray_w is None:
+                loss = F.mse_loss(results['rgb'], rgb_gt)
+            else:
+                loss = ((results['rgb'].float() - rgb_gt) ** 2).mean(-1).mul(ray_w).mean()
             if extra_loss is not None:  # e.g. distortion loss (train.py:194-195)
                 loss = loss + extra_loss(results)
         # GradScaler.scale(loss): the current scale is a device scalar, no host read
@@ -335,8 +340,8 @@ class NGPTrainer:
             self.encoder.adopt_shadow(self._shadow)
 
     def step(self, rays_o, rays_d, rgb_gt, exp_step_factor=0.0, extra_loss=None, bg_rgb=None, alpha=None, b_load=1.0,
-             img_idxs=None):
+             img_idxs=None, ray_w=None):
         loss, results = self.forward_backward(rays_o, rays_d, rgb_gt, exp_step_factor, extra_loss, bg_rgb, alpha,
-                                              b_load, img_idxs)
+                                              b_load, img_idxs, ray_w)
         self.optimizer_step()
         return loss, results

@@ -6,6 +6,9 @@ test-split PSNR and SSIM (:237-304); with --extract_mesh, results/mesh.ply after
 With --depth_loss_w the loss gains the depth term (DESIGN.md §6h) and a test split with depth reports depth_mae.
 With --extrinsics_lr every training image's pose is refined with the model (DESIGN.md §6i): the training rays come from
 the corrected poses, results/poses_refined.npy holds them at the end; the test split keeps its poses as loaded.
+With --ray_sampling_strategy error_map the training pixels are drawn from a per-tile error map (DESIGN.md §6j) that is
+rebuilt beside every density-grid update; every per-ray loss term is weighted by the ray's weight, and
+results/error_map.npy holds the map at the end.
 The step body runs on the sm_90a kernels through NGPTrainer (fused Adam,
 no host sync for the inf check); under torchrun every rank trains on its own rays and the gradients are summed
 once per step: by the peer-memory optimizer kernel when all ranks share one NVLink box, else by an fp16 NCCL
@@ -68,6 +71,8 @@ def main(prefix_args=None):
         raise RuntimeError("train.py needs a CUDA device: the hot path has no CPU fallback")
     device = torch.device("cuda", local)
     torch.cuda.set_device(device)
+    if world > 1 and hparams.ray_sampling_strategy == 'error_map':
+        raise ValueError("--ray_sampling_strategy error_map trains on one GPU: the error map is not shared between ranks")
     if world > 1 and hparams.extrinsics_lr > 0:
         raise ValueError("--extrinsics_lr trains on one GPU: the pose gradient is not exchanged between ranks")
     if world > 1:
@@ -97,7 +102,13 @@ def main(prefix_args=None):
         test_dataset = dataset(root_dir=hparams.root_dir, split='test', downsample=hparams.downsample,
                                n_images=4, **extra).to(device)
     train_dataset.batch_size = hparams.batch_size
-    train_dataset.ray_sampling_strategy = hparams.ray_sampling_strategy
+    error_map = None
+    if hparams.ray_sampling_strategy == 'error_map':   # the map draws the pixels; the dataset gathers them
+        from taichi_nerfs_b200.error_map import ErrorMap
+        error_map = ErrorMap(len(train_dataset.poses), *train_dataset.img_wh, res=hparams.error_map_res,
+                             seed=seed + rank, device=device)
+    else:
+        train_dataset.ray_sampling_strategy = hparams.ray_sampling_strategy
     model_config = build_model_config(hparams)
     model = MODEL_DICT[hparams.model_name](**model_config).to(device)
     if hparams.ckpt_path:
@@ -128,15 +139,22 @@ def main(prefix_args=None):
         fast = StaticTrainStep(trainer, hparams.batch_size, exp_step_factor=exp_step_factor,
                                distortion_loss_w=hparams.distortion_loss_w, random_bg=hparams.random_bg,
                                bg_seed=seed + rank, bg_load=bg_load, depth_loss_w=hparams.depth_loss_w,
-                               extrinsics=extrinsics)
+                               extrinsics=extrinsics, error_map=error_map)
 
     tic = time.time()
     for step in range(hparams.max_steps + 1):
         model.train()
-        data = train_dataset[step % len(train_dataset)]
+        if error_map is None:
+            data = train_dataset[step % len(train_dataset)]
         with torch.autocast(device_type='cuda', dtype=torch.float16):
             if step % update_interval == 0:
                 model.update_density_grid(0.01 * MAX_SAMPLES / 3 ** 0.5, warmup=step < warmup_steps)
+        ray_w = None
+        if error_map is not None:
+            if step % update_interval == 0 and step > 0:
+                error_map.rebuild()
+            em_img, em_pix, ray_w = error_map.draw(hparams.batch_size, step)
+            data = train_dataset.gather(em_img, em_pix)
         img_idxs = rays_o = rays_d = None
         if extrinsics is not None:   # same_image gives one index: the kernels broadcast it
             img_idxs = torch.as_tensor(data['img_idxs'], device=device)
@@ -151,18 +169,20 @@ def main(prefix_args=None):
                 raise ValueError(f"--depth_loss_w: the {hparams.dataset_name} dataset at {hparams.root_dir!r} has no "
                                  f"depth (an ngp scene needs depth_path frames)")
         terms = []
+        per_ray = (lambda v: v.mean()) if ray_w is None else (lambda v: (v * ray_w).mean())  # noqa: E731
         if hparams.distortion_loss_w > 0:
-            terms.append(lambda res: hparams.distortion_loss_w * distortion_loss(res).mean())
+            terms.append(lambda res: hparams.distortion_loss_w * per_ray(distortion_loss(res)))
         if depth is not None:
-            terms.append(lambda res: hparams.depth_loss_w * depth_loss(res, depth).mean())
+            terms.append(lambda res: hparams.depth_loss_w * per_ray(depth_loss(res, depth)))
         extra_loss = (lambda res: sum(f(res) for f in terms)) if terms else None  # noqa: E731
         if fast is not None:   # one graph replay, nothing synchronises the host
+            em_args = {} if error_map is None else {'ray_w': ray_w, 'img_idxs': em_img, 'pix_idxs': em_pix}
             if extrinsics is not None:   # the step forms the rays from the corrected poses itself
                 loss = fast.step(None, None, data['rgb'], alpha=data.get('alpha') if hparams.random_bg else None,
-                                 depth=depth, directions=data['direction'], img_idxs=img_idxs)
+                                 depth=depth, directions=data['direction'], **{'img_idxs': img_idxs, **em_args})
             else:
                 loss = fast.step(rays_o, rays_d, data['rgb'],
-                                 alpha=data.get('alpha') if hparams.random_bg else None, depth=depth)
+                                 alpha=data.get('alpha') if hparams.random_bg else None, depth=depth, **em_args)
             results = {'rgb': fast.rgb, 'rm_samples': fast.counter[0].clamp(max=fast.cap), 'vr_samples':
                        fast.counter[0].clamp(max=fast.cap), 'dropped_rays': fast.counter[1]}
         else:
@@ -170,7 +190,11 @@ def main(prefix_args=None):
             if hparams.random_bg:   # the colours of step trainer.step_count + 1, as the graph step draws them
                 bg_rgb = ops.random_bg(seed + rank, trainer.step_count + 1, len(rays_o), device)
             loss, results = trainer.step(rays_o, rays_d, data['rgb'], exp_step_factor, extra_loss=extra_loss,
-                                         bg_rgb=bg_rgb, alpha=data.get('alpha'), b_load=bg_load, img_idxs=img_idxs)
+                                         bg_rgb=bg_rgb, alpha=data.get('alpha'), b_load=bg_load, img_idxs=img_idxs,
+                                         ray_w=ray_w)
+            if error_map is not None:   # the graph step accumulates inside its graph
+                error_map.accumulate(results['rgb'].float(), data['rgb'], em_img, em_pix, bg_rgb=bg_rgb,
+                                     alpha=data.get('alpha') if bg_rgb is not None else None, b_load=bg_load)
 
         if step % 1000 == 0 and rank == 0:
             with torch.no_grad():
@@ -188,6 +212,8 @@ def main(prefix_args=None):
         save_deployment_model(model=model, dataset=train_dataset, save_dir=hparams.deployment_model_path)
     os.makedirs(val_dir, exist_ok=True)
     torch.save(model.state_dict(), os.path.join(val_dir, 'model.pth'))
+    if error_map is not None:
+        np.save(os.path.join(val_dir, 'error_map.npy'), error_map.as_image().cpu().numpy())
     if extrinsics is not None:
         np.save(os.path.join(val_dir, 'poses_refined.npy'), extrinsics.refined_poses())
         rot_deg, trans = extrinsics.mean_correction()
