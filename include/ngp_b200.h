@@ -696,6 +696,31 @@ int ngp_error_map_rebuild(uint64_t* E, uint64_t* acc, uint32_t* cnt, uint64_t* c
 int ngp_ray_grad_weight(const int32_t* rays_a, const float* w, float* dL_dsigmas, void* dL_drgbs, int rgbs_dtype,
                         int32_t* found_inf_or_null, int64_t n_rays, int64_t n_rows, void* stream);
 
+/* ---- per-image exposure compensation (DESIGN.md §6k) -------------------------------------------------------------
+ * Exposures expo [n_img, 4] fp32 = (e_r, e_g, e_b, 0) in stops (log2 gain), 16-byte aligned; the gradient and the
+ * Adam moments have the same layout.  The gain of image i is g_i = 2^{e_i}, formed in fp64.  Rows are visited through
+ * rays_a [n_rays, 3] = (ray, start, count) with count clipped to min(n_rows, *n_rows_dev) (n_rows_dev optional:
+ * the march's device row counter).  img_idxs [ray] int64 is clamped to [0, n_img) as ngp_pose_apply clamps it.  rgb
+ * rows are [S, 3] fp32 or fp16 (rgbs_dtype).
+ * ngp_exposure_apply: out[s, c] = g_img(ray)[c] * rgbs[s, c], rounded once (so e = 0 copies rgbs bit for bit).  out
+ * must not alias rgbs.
+ * ngp_exposure_bwd: for each ray, G = ln2 * sum_s dL_drgbs[s] * out[s] (per channel, fp32, a fixed order within the
+ * ray), then dL_drgbs[s] becomes g * dL_drgbs[s], rounded once; grad[img] += G.  The per-image sums use atomics, so
+ * their last bits vary between runs.  found_inf (optional) is set to 1 when a stored gradient or a ray's G is not
+ * finite (fp16 overflow included).
+ * ngp_exposure_adam: one CTA; the Adam of ngp_adam_step_dyn with lr/bc1 = lr_ratio * hyper_dev[0], sqrt(bc2) =
+ * hyper_dev[1], inv_scale = hyper_dev[2], then e -= the mean of e over the images, per channel (fp64, fixed order).
+ * Nothing but the gradient changes when *found_inf != 0; the gradient is zeroed on every call. */
+int ngp_exposure_apply(const void* rgbs, int rgbs_dtype, const int32_t* rays_a, const int64_t* img_idxs,
+                       const float* expo, int64_t n_img, void* out, int64_t n_rays, int64_t n_rows,
+                       const int32_t* n_rows_dev, void* stream);
+int ngp_exposure_bwd(const void* out, void* dL_drgbs, int rgbs_dtype, const int32_t* rays_a, const int64_t* img_idxs,
+                     const float* expo, int64_t n_img, float* grad, int32_t* found_inf_or_null, int64_t n_rays,
+                     int64_t n_rows, const int32_t* n_rows_dev, void* stream);
+int ngp_exposure_adam(float* expo, float* grad, float* exp_avg, float* exp_avg_sq, const int32_t* found_inf_or_null,
+                      const float* hyper_dev, float lr_ratio, float beta1, float beta2, float eps, int64_t n_img,
+                      void* stream);
+
 #ifdef __cplusplus
 }
 #endif

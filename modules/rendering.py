@@ -13,13 +13,14 @@ NEAR_DISTANCE = 0.01
 
 
 def render(model, rays_o, rays_d, test_time=False, exp_step_factor=0, T_threshold=1e-4,
-           max_samples=MAX_SAMPLES, bg_rgb=None, position_grad=False):
+           max_samples=MAX_SAMPLES, bg_rgb=None, position_grad=False, exposure=None):
     """AABB test, then the train or test rendering path.  Returns the result dict of the
     reference (train: rgb, depth, opacity, ws, deltas, ts, rays_a, rm_samples, vr_samples;
     test: rgb, depth, opacity, total_samples).  ``bg_rgb`` [N, 3] (training path only, --random_bg): each ray's own
     background colour in place of the fixed white / black one.  ``position_grad`` (training path only, camera
     extrinsics refinement, DESIGN.md §6i): the sample positions require grad and are returned as results['xyzs'], whose
-    .grad the backward fills."""
+    .grad the backward fills.  ``exposure`` (training path only, per-image exposure compensation, DESIGN.md §6k): a
+    function (rgbs, rays_a) -> rgbs' that the network's sample colours pass through before compositing."""
     rays_o = rays_o.contiguous()
     rays_d = rays_d.contiguous()
     hits_t = ray_aabb_intersection(rays_o, rays_d, model.scale)
@@ -32,7 +33,8 @@ def render(model, rays_o, rays_d, test_time=False, exp_step_factor=0, T_threshol
                 return render_frame_compact(model, rays_o, rays_d, exp_step_factor, T_threshold, max_samples)
             return render_frame(model, rays_o, rays_d, exp_step_factor, T_threshold, max_samples)
         return _render_rays_test(model, rays_o, rays_d, hits_t, exp_step_factor, T_threshold, max_samples)
-    return _render_rays_train(model, rays_o, rays_d, hits_t, exp_step_factor, T_threshold, bg_rgb, position_grad)
+    return _render_rays_train(model, rays_o, rays_d, hits_t, exp_step_factor, T_threshold, bg_rgb, position_grad,
+                              exposure)
 
 
 def _background(exp_step_factor, device):
@@ -79,7 +81,7 @@ def _render_rays_test(model, rays_o, rays_d, hits_t, exp_step_factor=0, T_thresh
 
 
 def _render_rays_train(model, rays_o, rays_d, hits_t, exp_step_factor=0, T_threshold=1e-4, bg_rgb=None,
-                       position_grad=False):
+                       position_grad=False, exposure=None):
     results = {}
     (rays_a, xyzs, dirs, results['deltas'], results['ts'], results['rm_samples']) = raymarching_train(
         rays_o, rays_d, hits_t, model.density_bitfield, model.cascades, model.scale, exp_step_factor,
@@ -88,6 +90,8 @@ def _render_rays_train(model, rays_o, rays_d, hits_t, exp_step_factor=0, T_thres
         results['xyzs'] = xyzs.requires_grad_(True)
 
     sigmas, rgbs = model(xyzs, dirs)
+    if exposure is not None:
+        rgbs = exposure(rgbs, rays_a)
 
     (results['vr_samples'], results['opacity'], results['depth'], results['rgb'], results['ws']) = \
         model.render_func(sigmas, rgbs, results['deltas'], results['ts'], rays_a, T_threshold)

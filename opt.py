@@ -65,6 +65,9 @@ _FLAGS = [
     ('--extrinsics_lr', dict(type=float, default=0.,
                              help='learning rate of the per-image camera pose corrections (rotation and translation, '
                                   'DESIGN.md §6i), 0 to disable (default); hash encoder only, one GPU')),
+    ('--exposure_lr', dict(type=float, default=0.,
+                           help='learning rate of the per-image exposures (a log2 gain per colour channel, DESIGN.md '
+                                '§6k), 0 to disable (default); every model kind, one GPU')),
     # misc
     ('--exp_name', dict(type=str, default='exp', help='experiment name')),
     ('--gpu', dict(type=int, default=0, help='set cuda device (ignored under torchrun: LOCAL_RANK wins)')),
@@ -129,6 +132,14 @@ def get_opts(prefix_args=None):
         if hparams.encoder_type == 'triplane':
             parser.error("--extrinsics_lr does not combine with --encoder_type triplane: the tri-plane encoder gives no "
                          "gradient wrt the sample positions")
+    if not (math.isfinite(hparams.exposure_lr) and hparams.exposure_lr >= 0):
+        parser.error(f"--exposure_lr must be finite and >= 0, got {hparams.exposure_lr}")
+    if hparams.exposure_lr > 0:
+        if not (math.isfinite(hparams.lr) and hparams.lr > 0):
+            parser.error(f"--exposure_lr is set relative to the model's learning rate: it needs a finite --lr > 0, got "
+                         f"{hparams.lr}")
+        if int(os.environ.get("WORLD_SIZE", "1")) > 1:
+            parser.error("--exposure_lr trains on one GPU: the exposure gradient is not exchanged between ranks")
     if hparams.model_name == 'svox':
         for flag, bad, why in (
                 ('encoder_type', hparams.encoder_type == 'triplane',

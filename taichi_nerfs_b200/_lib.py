@@ -130,6 +130,9 @@ def _declare(lib):
         "ngp_error_map_accumulate": (ci, [vp, vp, vp, vp, f32, vp, vp, i64, i64, i64, i64, vp, vp, i64, vp]),
         "ngp_error_map_rebuild": (ci, [vp, vp, vp, vp, i64, i64, i64, i64, ci, ci, ci, vp, i64, vp]),
         "ngp_ray_grad_weight": (ci, [vp, vp, vp, vp, ci, vp, i64, i64, vp]),
+        "ngp_exposure_apply": (ci, [vp, ci, vp, vp, vp, i64, vp, i64, i64, vp, vp]),
+        "ngp_exposure_bwd": (ci, [vp, vp, ci, vp, vp, vp, i64, vp, vp, i64, i64, vp, vp]),
+        "ngp_exposure_adam": (ci, [vp, vp, vp, vp, vp, vp, f32, f32, f32, f32, i64, vp]),
     }
     for name, (res, args) in sigs.items():
         fn = getattr(lib, name)  # AttributeError if the symbol is missing: fail loudly

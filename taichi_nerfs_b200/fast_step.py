@@ -17,6 +17,10 @@ With error-map sampling (DESIGN.md §6j) each ray carries a weight w_r: the head
 backward sees the gradient of the weighted loss; loss_sum, the logged value, stays the unweighted one.  The sampled step
 draws its pixels with the error-map sampler, whose indices the batch sampler then reads.
 
+With exposure compensation (DESIGN.md §6k) the exposure apply runs between the network (or voxel) forward and the head,
+which reads its scaled copy of the sample colours; the exposure backward runs after the head (and the error-map nodes),
+rewriting the per-sample colour gradient before the network backward, and the exposures' Adam runs next to the model's.
+
 A voxel-grid model (--model_name svox) has no network: the march feeds the voxel forward (fp32 sigma / rgb) -> head ->
 voxel backward -> [regularisers] -> finite check and Adam over the fields' node block B only (DESIGN.md §6b).
 
@@ -65,6 +69,8 @@ class StaticTrainStep:
         self.ext = extrinsics
         # error_map: a taichi_nerfs_b200.error_map.ErrorMap over the training images, or None (nothing is enqueued)
         self.em = error_map
+        # exposure compensation: the trainer's ExposureCorrection (NGPTrainer(exposure=...)), shared with the module path
+        self.expo = trainer.exposure
         if self.ext is not None and overlap_optimizer:
             raise _lib.NgpError("StaticTrainStep: extrinsics refinement does not combine with overlap_optimizer (the "
                                 "next step's march would read poses one update stale)")
@@ -123,6 +129,13 @@ class StaticTrainStep:
             self.em_img = torch.zeros(self.n, device=dev, dtype=torch.int64)
             self.em_pix = torch.zeros(self.n, device=dev, dtype=torch.int64)
             self.ray_w = torch.ones(self.n, device=dev)
+        if self.expo is not None:
+            # the head's copy of the sample colours under their images' gains; each ray's image is the index buffer
+            # extrinsics refinement or the error map fill, else one of its own (step(img_idxs=...) or the sampler)
+            self.rgbs_expo = torch.zeros_like(self.rgbs)
+            self.expo_img = (self.img_idx if self.ext is not None else self.em_img if self.em is not None
+                             else torch.zeros(self.n, device=dev, dtype=torch.int64))
+        self._head_rgbs = self.rgbs_expo if self.expo is not None else self.rgbs
         # GradScaler state on the device: [scale, growth_tracker (int bits)]; growth 2x / 2000 clean steps, backoff 0.5
         trainer.dynamic_loss_scale = self.dynamic_loss_scale = bool(dynamic_loss_scale)
         self.aabb6 = (C.c_float * 6)(*[float(v) for v in m.xyz_min.flatten().tolist()],
@@ -243,28 +256,28 @@ class StaticTrainStep:
             check(L.ngp_random_bg(self.bg_seed & 0xFFFFFFFFFFFFFFFF, _p(self.bg_step), 0, _p(self.bg_rgb), self.n, st))
         if self.depth_w > 0:
             check(load().ngp_ray_head_fused_depth(
-                _p(self.sig), _p(self.rgbs), ctag, _p(self.deltas), _p(self.ts), _p(self.rays_a), _p(self.gt), bg,
-                _p(self.bg_rgb), _p(self.alpha), self.bg_load, float(self.tr.loss_scale),
+                _p(self.sig), _p(self._head_rgbs), ctag, _p(self.deltas), _p(self.ts), _p(self.rays_a), _p(self.gt),
+                bg, _p(self.bg_rgb), _p(self.alpha), self.bg_load, float(self.tr.loss_scale),
                 _p(self.scale_state) if self.dynamic_loss_scale else None, self.T_thr, self.distortion_w,
                 _p(self.depth_gt), self.depth_w, _p(self.loss_sum), _p(self.opacity), _p(self.rgb), _p(self.dsig),
                 _p(self.drgbs), self.n, self._st()))
             return
         if self.random_bg:
             check(L.ngp_ray_head_fused_random_bg(
-                _p(self.sig), _p(self.rgbs), ctag, _p(self.deltas), _p(self.ts), _p(self.rays_a), _p(self.gt),
+                _p(self.sig), _p(self._head_rgbs), ctag, _p(self.deltas), _p(self.ts), _p(self.rays_a), _p(self.gt),
                 _p(self.bg_rgb), _p(self.alpha), self.bg_load, float(self.tr.loss_scale),
                 _p(self.scale_state) if self.dynamic_loss_scale else None, self.T_thr, self.distortion_w,
                 _p(self.loss_sum), _p(self.opacity), _p(self.rgb), _p(self.dsig), _p(self.drgbs), self.n, st))
             return
         if self.distortion_w > 0:
             check(load().ngp_ray_head_fused_distortion(
-                _p(self.sig), _p(self.rgbs), ctag, _p(self.deltas), _p(self.ts), _p(self.rays_a), _p(self.gt), bg,
-                float(self.tr.loss_scale), _p(self.scale_state) if self.dynamic_loss_scale else None, self.T_thr,
+                _p(self.sig), _p(self._head_rgbs), ctag, _p(self.deltas), _p(self.ts), _p(self.rays_a), _p(self.gt),
+                bg, float(self.tr.loss_scale), _p(self.scale_state) if self.dynamic_loss_scale else None, self.T_thr,
                 self.distortion_w, _p(self.loss_sum), _p(self.opacity), _p(self.rgb), _p(self.dsig), _p(self.drgbs),
                 self.n, self._st()))
             return
-        check(load().ngp_ray_head_fused(_p(self.sig), _p(self.rgbs), ctag, _p(self.deltas), _p(self.rays_a), _p(self.gt),
-                                        bg, float(self.tr.loss_scale),
+        check(load().ngp_ray_head_fused(_p(self.sig), _p(self._head_rgbs), ctag, _p(self.deltas), _p(self.rays_a),
+                                        _p(self.gt), bg, float(self.tr.loss_scale),
                                         _p(self.scale_state) if self.dynamic_loss_scale else None, self.T_thr,
                                         _p(self.loss_sum), _p(self.opacity), _p(self.rgb), _p(self.dsig),
                                         _p(self.drgbs), self.n, self._st()))
@@ -322,24 +335,44 @@ class StaticTrainStep:
         check(load().ngp_ray_grad_weight(_p(self.rays_a), _p(self.ray_w), _p(self.dsig), _p(self.drgbs),
                                          F32 if self.vox else F16, _p(self.tr.found_inf), self.n, self.cap, self._st()))
 
+    # exposure compensation (DESIGN.md §6k): the colours the head reads; the colour gradient and the exposure gradient
+    def _k_expo_apply(self):
+        x = self.expo
+        check(load().ngp_exposure_apply(_p(self.rgbs), F32 if self.vox else F16, _p(self.rays_a), _p(self.expo_img),
+                                        _p(x.exposure), x.n_img, _p(self.rgbs_expo), self.n, self.cap,
+                                        _p(self.counter), self._st()))
+
+    def _k_expo_bwd(self):
+        x = self.expo
+        check(load().ngp_exposure_bwd(_p(self.rgbs_expo), _p(self.drgbs), F32 if self.vox else F16, _p(self.rays_a),
+                                      _p(self.expo_img), _p(x.exposure), x.n_img, _p(x.grad), _p(self.tr.found_inf),
+                                      self.n, self.cap, _p(self.counter), self._st()))
+
     def _k_head_weighted(self):
         self._k_head()
         if self.em is not None:
             self._k_em_accumulate()
             self._k_grad_weight()
 
+    def _k_head_exposed(self):
+        if self.expo is not None:
+            self._k_expo_apply()
+        self._k_head_weighted()
+        if self.expo is not None:
+            self._k_expo_bwd()
+
     def _enqueue_network(self):
         # counter[0] = number of valid sample rows, read on the device by every kernel
         if self.vox:
             self._k_voxel_fwd()
-            self._k_head_weighted()
+            self._k_head_exposed()
             self._k_voxel_bwd()
             if self.tr.voxel_reg is not None:   # TV / sparsity over B, scaled by the device loss scale
                 self.tr.add_voxel_reg()
             return
         self._k_hash_fwd()
         self._k_mlp_fwd()
-        self._k_head_weighted()
+        self._k_head_exposed()
         self._k_mlp_bwd()
         self._k_hash_bwd()
         if self.ext is not None:
@@ -357,7 +390,9 @@ class StaticTrainStep:
         check(load().ngp_sample_ray_batch(_p(src["bank"]), src["bank"].shape[2], _p(src["poses"]), _p(src["dirs"]),
                                           src["poses"].shape[0], src["dirs"].shape[0], img, pix, src["fixed_img"],
                                           src["seed"], _p(self.sample_step), 0, _p(self.rays_o), _p(self.rays_d),
-                                          _p(self.gt), _p(self.noise), None, None, self.n, self._st()))
+                                          _p(self.gt), _p(self.noise),
+                                          _p(self.expo_img) if self.expo is not None and em is None else None, None,
+                                          self.n, self._st()))
 
     def _enqueue_update(self):
         # [gradient exchange] -> check_finite -> LR/bias scalars -> fused Adam -> GradScaler.update
@@ -400,6 +435,7 @@ class StaticTrainStep:
         bg_step_keep = self.bg_step.clone()
         ext_keep = [] if self.ext is None else [t.clone() for t in self.ext.state()]
         em_keep = [] if self.em is None else [t.clone() for t in self.em.state()]
+        expo_keep = [] if self.expo is None else [t.clone() for t in self.expo.state()]
         shadow = None if tr._shadow_full is None else tr._shadow_full.clone()
         side = torch.cuda.Stream()
         side.wait_stream(torch.cuda.current_stream())
@@ -429,6 +465,9 @@ class StaticTrainStep:
         if self.em is not None:
             for t, k in zip(self.em.state(), em_keep):
                 t.copy_(k)
+        if self.expo is not None:
+            for t, k in zip(self.expo.state(), expo_keep):
+                t.copy_(k)
         tr.flat_grad.zero_()
         if shadow is not None:
             tr._shadow_full.copy_(shadow)
@@ -442,7 +481,11 @@ class StaticTrainStep:
         (depth_loss_w > 0 only, where it is required): each ray's target z-depth, 0 where there is none.  With
         extrinsics refinement the step forms its rays itself: rays_o and rays_d are None and ``directions`` [N, 3]
         (camera frame) and ``img_idxs`` [N] (or one index for the whole batch) are required.  With an error map,
-        ``ray_w`` [N] (the loss weights of ErrorMap.draw), ``img_idxs`` and ``pix_idxs`` [N] are required."""
+        ``ray_w`` [N] (the loss weights of ErrorMap.draw), ``img_idxs`` and ``pix_idxs`` [N] are required.  With exposure
+        compensation ``img_idxs`` [N] (or one index) is required."""
+        if self.expo is not None and img_idxs is None:
+            raise ValueError("exposure compensation: step(..., img_idxs=...) (each ray's image, whose gain its samples "
+                             "take)")
         if self.em is not None:
             if ray_w is None or img_idxs is None or pix_idxs is None:
                 raise ValueError("error-map sampling: step(..., ray_w=..., img_idxs=..., pix_idxs=...) (the rays' loss "
@@ -458,9 +501,12 @@ class StaticTrainStep:
                                  "(the step forms the rays from the corrected poses)")
             self.cam_dirs.copy_(directions, non_blocking=True)
             self.img_idx.copy_(torch.as_tensor(img_idxs, device=self.dev).reshape(-1), non_blocking=True)
-        elif directions is not None or (img_idxs is not None and self.em is None):
-            raise ValueError("directions / img_idxs are read by extrinsics refinement and error-map sampling only "
-                             "(StaticTrainStep(extrinsics=... | error_map=...))")
+        elif directions is not None or (img_idxs is not None and self.em is None and self.expo is None):
+            raise ValueError("directions / img_idxs are read by extrinsics refinement, error-map sampling and exposure "
+                             "compensation only (StaticTrainStep(extrinsics=... | error_map=...), "
+                             "NGPTrainer(exposure=...))")
+        elif self.expo is not None and self.em is None:   # the step's own index buffer
+            self.expo_img.copy_(torch.as_tensor(img_idxs, device=self.dev).reshape(-1), non_blocking=True)
         if depth is None and self.depth_w > 0:
             raise ValueError("depth_loss_w > 0 needs each ray's target depth: step(..., depth=...)")
         if depth is not None and self.depth_w == 0:

@@ -621,6 +621,64 @@ def ray_grad_weight(rays_a, w, dsigmas, drgbs, found_inf=None, n_rows=None):
                                      rays_a.shape[0], rows, _stream()), "ray_grad_weight")
 
 
+# ---- per-image exposure compensation (DESIGN.md §6k) ------------------------------------------------------------
+def _exposure_buffers(*ts):
+    for t in ts:
+        if t.dtype != torch.float32 or not t.is_contiguous() or t.dim() != 2 or t.shape[1] != 4:
+            raise TypeError("exposures, their gradient and moments are contiguous fp32 [n_img, 4]")
+
+
+def _exposure_rows(rows, rays_a, what):
+    if rays_a.dtype != torch.int32 or not rays_a.is_contiguous():
+        raise TypeError(f"{what}: rays_a must be contiguous int32 [n, 3]")
+    if rows.dim() != 2 or rows.shape[1] != 3 or not rows.is_contiguous():
+        raise ValueError(f"{what}: rgb rows must be contiguous [S, 3]")
+
+
+def exposure_apply(rgbs, rays_a, img_idxs, expo, out=None, n_rows_dev=None):
+    """c' = 2^e[img(ray)] * c over every ray's rows of rgbs [S, 3] (fp16 or fp32) into a new buffer of the same dtype
+    (or ``out``); rays_a [n, 3] int32 = (ray, start, count), img_idxs [n] (or one index) by ray id, expo [n_img, 4]."""
+    _need_cuda(rgbs, rays_a, img_idxs, expo, out, n_rows_dev)
+    _exposure_buffers(expo)
+    _exposure_rows(rgbs, rays_a, "exposure_apply")
+    n = rays_a.shape[0]
+    idx = _img_index(img_idxs, n)
+    out = torch.empty_like(rgbs) if out is None else out
+    if out.dtype != rgbs.dtype or out.shape != rgbs.shape or out.data_ptr() == rgbs.data_ptr():
+        raise ValueError("exposure_apply: out must be a separate buffer of rgbs' shape and dtype")
+    check(load().ngp_exposure_apply(_ptr(rgbs), _tag(rgbs), _ptr(rays_a), _ptr(idx), _ptr(expo), expo.shape[0],
+                                    _ptr(out), n, rgbs.shape[0], _ptr(n_rows_dev), _stream()), "exposure_apply")
+    return out
+
+
+def exposure_bwd(out, drgbs, rays_a, img_idxs, expo, grad, found_inf=None, n_rows_dev=None):
+    """In place: drgbs [S, 3] = dL/dc' becomes dL/dc = g * dL/dc'; grad [n_img, 4] += ln2 * sum dL/dc' * c' per image,
+    with out the rows exposure_apply wrote.  found_inf (int32 [1], optional) is raised on a non-finite result."""
+    _need_cuda(out, drgbs, rays_a, img_idxs, expo, grad, found_inf, n_rows_dev)
+    _exposure_buffers(expo, grad)
+    _exposure_rows(drgbs, rays_a, "exposure_bwd")
+    if out.dtype != drgbs.dtype or out.shape != drgbs.shape or not out.is_contiguous():
+        raise ValueError("exposure_bwd: out and drgbs are contiguous rows of one shape and dtype")
+    if grad.shape != expo.shape:
+        raise ValueError("exposure_bwd: grad must have the exposures' shape")
+    n = rays_a.shape[0]
+    idx = _img_index(img_idxs, n)
+    check(load().ngp_exposure_bwd(_ptr(out), _ptr(drgbs), _tag(drgbs), _ptr(rays_a), _ptr(idx), _ptr(expo),
+                                  expo.shape[0], _ptr(grad), _ptr(found_inf), n, drgbs.shape[0], _ptr(n_rows_dev),
+                                  _stream()), "exposure_bwd")
+
+
+def exposure_adam(expo, grad, exp_avg, exp_avg_sq, hyper, lr_ratio, found_inf=None, beta1=0.9, beta2=0.999,
+                  eps=1e-15):
+    """One Adam step of the exposures with the model's device scalars ``hyper`` (ngp_adam_hyper_update) at lr_ratio
+    times the model's learning rate, then the per-channel mean over the images subtracted; the gradient is zeroed."""
+    _need_cuda(expo, grad, exp_avg, exp_avg_sq, hyper, found_inf)
+    _exposure_buffers(expo, grad, exp_avg, exp_avg_sq)
+    check(load().ngp_exposure_adam(_ptr(expo), _ptr(grad), _ptr(exp_avg), _ptr(exp_avg_sq), _ptr(found_inf),
+                                   _ptr(hyper), float(lr_ratio), float(beta1), float(beta2), float(eps), expo.shape[0],
+                                   _stream()), "exposure_adam")
+
+
 def morton3d(coords):
     _need_cuda(coords)
     c = coords.contiguous()

@@ -31,9 +31,10 @@ def _p(t):
 class NGPTrainer:
     def __init__(self, model, lr: float = 1e-2, max_steps: int = 20000, loss_scale: float | None = None,
                  betas=(0.9, 0.999), eps: float = 1e-15, process_group=None, dynamic_loss_scale: bool = True,
-                 p2p_optimizer: bool | None = None, voxel_reg=None, extrinsics=None):
+                 p2p_optimizer: bool | None = None, voxel_reg=None, extrinsics=None, exposure=None):
         from modules.hash_encoder import HashEncoder
         from modules.voxel_grid import VoxelGrid
+        from .exposure import ExposureCorrection
         from .extrinsics import PoseRefinement
         # The model kind, decided here once (StaticTrainStep reads it too): the position encoder, whose one parameter
         # (its table) must be the first slice of the flat buffers, or None for a VoxelGrid, which has no encoder and
@@ -75,6 +76,14 @@ class NGPTrainer:
                 raise ValueError("NGPTrainer: extrinsics refinement runs on one rank (the pose gradient is not "
                                  "exchanged between ranks)")
         self.extrinsics = extrinsics
+        # per-image exposure compensation (DESIGN.md §6k): an ExposureCorrection whose Adam step runs with the model's
+        if exposure is not None:
+            if not isinstance(exposure, ExposureCorrection):
+                raise TypeError("NGPTrainer: exposure must be a taichi_nerfs_b200.exposure.ExposureCorrection")
+            if self.world_size > 1:
+                raise ValueError("NGPTrainer: exposure compensation runs on one rank (the exposure gradient is not "
+                                 "exchanged between ranks)")
+        self.exposure = exposure
         self._pose_batch = None   # (xyzs, ts, rays_a, img_idxs, rays_d) of the last forward_backward
 
         self.params = [p for p in model.parameters() if p.requires_grad]
@@ -187,19 +196,26 @@ class NGPTrainer:
         ``alpha`` [N] (the image's alpha), the target's loader background ``b_load`` is replaced by it too:
         rgb_gt + (bg_rgb - b_load)(1 - alpha).  With extrinsics refinement, ``img_idxs`` [N] (or one index) names each
         ray's image and rays_o / rays_d are the PoseRefinement's rays; the pose gradient is formed by optimizer_step.
+        With exposure compensation, ``img_idxs`` names each ray's image too, and the sample colours pass through its
+        gain (DESIGN.md §6k).
         ``ray_w`` [N] fp32 (error-map sampling, DESIGN.md §6j): the MSE becomes mean_r w_r mean_c (rgb - gt)^2, and the
         returned loss is that weighted value; ``extra_loss`` weights its own per-ray terms."""
         from modules.rendering import render
         refine = self.extrinsics is not None
+        expo = self.exposure
         if refine and img_idxs is None:
             raise ValueError("NGPTrainer: extrinsics refinement needs each ray's image index (img_idxs=...)")
-        if not refine and img_idxs is not None:
-            raise ValueError("NGPTrainer: img_idxs is read by extrinsics refinement only (NGPTrainer(extrinsics=...))")
+        if expo is not None and img_idxs is None:
+            raise ValueError("NGPTrainer: exposure compensation needs each ray's image index (img_idxs=...)")
+        if not refine and expo is None and img_idxs is not None:
+            raise ValueError("NGPTrainer: img_idxs is read by extrinsics refinement and exposure compensation only "
+                             "(NGPTrainer(extrinsics=... | exposure=...))")
+        exposure = None if expo is None else (lambda rgbs, rays_a: expo.apply(rgbs, rays_a, img_idxs))  # noqa: E731
         if bg_rgb is not None and alpha is not None:
             rgb_gt = rgb_gt + (bg_rgb - b_load) * (1 - alpha)[:, None]
         with torch.autocast(device_type='cuda', dtype=torch.float16):
             results = render(self.model, rays_o, rays_d, exp_step_factor=exp_step_factor, bg_rgb=bg_rgb,
-                             position_grad=refine)
+                             position_grad=refine, exposure=exposure)
             if ray_w is None:
                 loss = F.mse_loss(results['rgb'], rgb_gt)
             else:
@@ -278,6 +294,9 @@ class NGPTrainer:
             check(L.ngp_check_finite_f16(_p(g16), g16.numel(), _p(self.found_inf), st))
         elif check_finite:
             check(L.ngp_check_finite(_p(fg), fg.numel(), _p(self.found_inf), st))
+        if check_finite and self.exposure is not None:   # the exposure gradient is outside the flat buffer
+            eg = self.exposure.grad
+            check(L.ngp_check_finite(_p(eg), eg.numel(), _p(self.found_inf), st))
         if R is not None:
             R.barrier(self.found_inf)
         # inv_scale: static (host constant) or the device value maintained by GradScaler.update() below (-1 sentinel)
@@ -308,6 +327,8 @@ class NGPTrainer:
                                       self.betas[1], self.eps, 1, fg.numel(), st))
         if self.extrinsics is not None:   # the pose corrections' Adam, on the same device scalars (one rank)
             self.extrinsics.enqueue_adam(self)
+        if self.exposure is not None:     # the exposures' Adam and zero-mean projection, on the same scalars
+            self.exposure.enqueue_adam(self)
         if self.dynamic_loss_scale:  # GradScaler.update(): adjusts the scale used by the NEXT step
             # a flag raised at the source is not reset by the next step, so this launch clears it
             raised_at_source = not check_finite and g16 is None

@@ -9,6 +9,8 @@ the corrected poses, results/poses_refined.npy holds them at the end; the test s
 With --ray_sampling_strategy error_map the training pixels are drawn from a per-tile error map (DESIGN.md §6j) that is
 rebuilt beside every density-grid update; every per-ray loss term is weighted by the ray's weight, and
 results/error_map.npy holds the map at the end.
+With --exposure_lr every training image gets a learned per-channel exposure (DESIGN.md §6k) that scales its rays' sample
+colours; results/exposures.npy holds them (stops) at the end, and test views render at the mean exposure, e = 0.
 The step body runs on the sm_90a kernels through NGPTrainer (fused Adam,
 no host sync for the inf check); under torchrun every rank trains on its own rays and the gradients are summed
 once per step: by the peer-memory optimizer kernel when all ranks share one NVLink box, else by an fp16 NCCL
@@ -75,6 +77,8 @@ def main(prefix_args=None):
         raise ValueError("--ray_sampling_strategy error_map trains on one GPU: the error map is not shared between ranks")
     if world > 1 and hparams.extrinsics_lr > 0:
         raise ValueError("--extrinsics_lr trains on one GPU: the pose gradient is not exchanged between ranks")
+    if world > 1 and hparams.exposure_lr > 0:
+        raise ValueError("--exposure_lr trains on one GPU: the exposure gradient is not exchanged between ranks")
     if world > 1:
         torch.distributed.init_process_group("nccl", device_id=device)
 
@@ -124,8 +128,12 @@ def main(prefix_args=None):
     if hparams.extrinsics_lr > 0:   # per-image pose corrections (DESIGN.md §6i)
         from taichi_nerfs_b200.extrinsics import PoseRefinement
         extrinsics = PoseRefinement(train_dataset.poses, hparams.extrinsics_lr / hparams.lr)
+    exposure = None
+    if hparams.exposure_lr > 0:   # per-image exposures (DESIGN.md §6k)
+        from taichi_nerfs_b200.exposure import ExposureCorrection
+        exposure = ExposureCorrection(len(train_dataset.poses), hparams.exposure_lr / hparams.lr, device)
     trainer = NGPTrainer(model, lr=hparams.lr, max_steps=hparams.max_steps, voxel_reg=voxel_reg,
-                         extrinsics=extrinsics)
+                         extrinsics=extrinsics, exposure=exposure)
 
     # --random_bg (DESIGN.md §6f): every training ray gets its own background colour, drawn on the device
     bg_load = getattr(train_dataset, 'bg_load', 1.0)
@@ -156,8 +164,9 @@ def main(prefix_args=None):
             em_img, em_pix, ray_w = error_map.draw(hparams.batch_size, step)
             data = train_dataset.gather(em_img, em_pix)
         img_idxs = rays_o = rays_d = None
-        if extrinsics is not None:   # same_image gives one index: the kernels broadcast it
+        if extrinsics is not None or exposure is not None:   # same_image gives one index: the kernels broadcast it
             img_idxs = torch.as_tensor(data['img_idxs'], device=device)
+        if extrinsics is not None:
             if fast is None:         # the graph step forms the rays from the corrected poses itself
                 rays_o, rays_d = extrinsics.rays(data['direction'], img_idxs)
         else:
@@ -177,6 +186,8 @@ def main(prefix_args=None):
         extra_loss = (lambda res: sum(f(res) for f in terms)) if terms else None  # noqa: E731
         if fast is not None:   # one graph replay, nothing synchronises the host
             em_args = {} if error_map is None else {'ray_w': ray_w, 'img_idxs': em_img, 'pix_idxs': em_pix}
+            if exposure is not None and error_map is None:
+                em_args['img_idxs'] = img_idxs
             if extrinsics is not None:   # the step forms the rays from the corrected poses itself
                 loss = fast.step(None, None, data['rgb'], alpha=data.get('alpha') if hparams.random_bg else None,
                                  depth=depth, directions=data['direction'], **{'img_idxs': img_idxs, **em_args})
@@ -214,6 +225,11 @@ def main(prefix_args=None):
     torch.save(model.state_dict(), os.path.join(val_dir, 'model.pth'))
     if error_map is not None:
         np.save(os.path.join(val_dir, 'error_map.npy'), error_map.as_image().cpu().numpy())
+    if exposure is not None:
+        e = exposure.exposures()
+        np.save(os.path.join(val_dir, 'exposures.npy'), e)
+        print(f"exposure: mean |e| = {float(np.abs(e).mean()):.4f} stops | max |e| = {float(np.abs(e).max()):.4f} "
+              f"stops -> {os.path.join(val_dir, 'exposures.npy')}")
     if extrinsics is not None:
         np.save(os.path.join(val_dir, 'poses_refined.npy'), extrinsics.refined_poses())
         rot_deg, trans = extrinsics.mean_correction()
