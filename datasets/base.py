@@ -11,6 +11,10 @@ colour the loader blended transparent pixels onto (1 white, 0 black), which ``--
 A loader that reads depth (the ngp loader's ``depth_path``, DESIGN.md §6h) sets ``depths`` [N, H*W] fp32 z-depth, 0
 where there is none; samples then also carry ``depth``, indexed as ``rgb`` is.  Loaders without depth set nothing and
 their samples are unchanged.
+
+A loader built with ``lens_distortion=True`` (DESIGN.md §6l) sets ``camera`` (taichi_nerfs_b200.intrinsics.Camera);
+``to(device)`` then replaces ``directions`` by the unprojection of every pixel through it, on the GPU, and raises if
+a pixel is not invertible.  Loaders without it have ``camera = None`` and keep the pinhole ``directions``.
 """
 from __future__ import annotations
 
@@ -35,6 +39,7 @@ def stack_poses(poses):
 
 class BaseDataset(Dataset):
     bg_load = 1.0
+    camera = None
 
     def __init__(self, root_dir, split='train', downsample=1.0):
         self.root_dir = root_dir
@@ -54,6 +59,9 @@ class BaseDataset(Dataset):
         self.poses = self.poses.to(device)
         self.K = self.K.to(device)
         self.directions = self.directions.to(device)
+        if self.camera is not None:
+            from taichi_nerfs_b200.intrinsics import unproject_table
+            self.directions = unproject_table(self.camera, *self.img_wh, self.directions.device)
         if getattr(self, 'depths', None) is not None:
             self.depths = self.depths.to(device)
         return self

@@ -3,6 +3,9 @@ datasets/colmap.py without its HDR-NeRF branches, whose exposure channel the ref
 
 - Intrinsics (:25-47) come from camera 1: ``SIMPLE_RADIAL`` (f, cx, cy, k: distortion ignored), ``PINHOLE`` and
   ``OPENCV`` (fx, fy, cx, cy, ...: distortion ignored), scaled by ``downsample``.  Other models are refused by name.
+  With ``lens_distortion=True`` (DESIGN.md §6l) the distortion is kept: ``camera`` holds the model (``PINHOLE``,
+  ``SIMPLE_PINHOLE``, ``SIMPLE_RADIAL``, ``RADIAL`` or ``OPENCV``; others are refused by name) with its focal lengths and
+  principal point scaled and its distortion terms as written, and ``to(device)`` unprojects every pixel through it.
 - Poses (:49-87): images sorted by name; camera-to-world = inverse of the world-to-camera matrix in float64;
   recentred on the average pose about the sparse points' mean (``center_poses``) and scaled so that the nearest
   camera is at distance 1.
@@ -27,10 +30,11 @@ from .ray_utils import center_poses, create_spheric_poses, get_ray_directions
 class ColmapDataset(BaseDataset):
     bg_load = 0.0
 
-    def __init__(self, root_dir, split='train', downsample=1.0, read_meta=True, **_):
+    def __init__(self, root_dir, split='train', downsample=1.0, read_meta=True, lens_distortion=False, **_):
         if 'HDR-NeRF' in root_dir:
             raise ValueError(f"{root_dir}: HDR-NeRF data (multi-exposure images) is not supported by the COLMAP loader")
         super().__init__(root_dir, split, downsample)
+        self.lens_distortion = bool(lens_distortion)
         self.read_intrinsics()
         if read_meta:
             self.read_meta(split)
@@ -43,6 +47,9 @@ class ColmapDataset(BaseDataset):
         h, w = int(cam.height * self.downsample), int(cam.width * self.downsample)
         self.img_wh = (w, h)
         p = cam.params
+        if self.lens_distortion:
+            self._read_camera(cam.model, p, w, h)
+            return
         if cam.model == 'SIMPLE_RADIAL':
             fx = fy = p[0] * self.downsample
             cx, cy = p[1] * self.downsample, p[2] * self.downsample
@@ -53,6 +60,21 @@ class ColmapDataset(BaseDataset):
             raise ValueError(f"camera model {cam.model} is not supported (SIMPLE_RADIAL, PINHOLE, OPENCV are)")
         self.K = torch.tensor([[fx, 0, cx], [0, fy, cy], [0, 0, 1]], dtype=torch.float32)
         self.directions = get_ray_directions(h, w, self.K)
+
+    def _read_camera(self, model, p, w, h):
+        from taichi_nerfs_b200.intrinsics import Camera
+        d = self.downsample
+        if model in ('SIMPLE_PINHOLE', 'SIMPLE_RADIAL', 'RADIAL'):   # f, cx, cy[, k1[, k2]]
+            f, cx, cy, dist = p[0] * d, p[1] * d, p[2] * d, list(p[3:])
+            self.camera = Camera(model, f, f, cx, cy, tuple(dist + [0.0] * (4 - len(dist))))
+        elif model in ('PINHOLE', 'OPENCV'):                          # fx, fy, cx, cy[, k1, k2, p1, p2]
+            dist = list(p[4:])
+            self.camera = Camera(model, p[0] * d, p[1] * d, p[2] * d, p[3] * d, tuple(dist + [0.0] * (4 - len(dist))))
+        else:
+            raise ValueError(f"camera model {model} is not supported with lens distortion (PINHOLE, SIMPLE_PINHOLE, "
+                             f"SIMPLE_RADIAL, RADIAL, OPENCV are)")
+        self.K = self.camera.K()
+        self.directions = get_ray_directions(h, w, self.K)   # the pinhole table until to(device) unprojects
 
     def read_meta(self, split):
         imdata = read_images_binary(os.path.join(self.root_dir, 'sparse/0/images.bin'))

@@ -2,6 +2,9 @@
 reference datasets/ngp.py).  Every split reads all frames (:43-72), as the reference does.
 
 - Intrinsics (:22-41): ``w``, ``h``, ``fl_x``, ``fl_y`` scaled by ``downsample``, principal point at the centre.
+  With ``lens_distortion=True`` (DESIGN.md §6l) ``cx``, ``cy`` are read when present (scaled) and ``k1 k2 p1 p2`` as
+  an OPENCV ``camera`` (unscaled), and ``to(device)`` unprojects every pixel through it; ``is_fisheye`` and non-zero
+  ``k3`` / ``k4`` are refused.
 - Poses (:64-66): ``transform_matrix[:3, :4]`` with the y and z axes negated; no rescaling.
 - A frame whose image file (``file_path`` as written, extension included) is missing is skipped, pose and all.
 - Images are blended onto white.
@@ -28,8 +31,9 @@ from .ray_utils import get_ray_directions
 class NGPDataset(BaseDataset):
     bg_load = 1.0
 
-    def __init__(self, root_dir, split='train', downsample=1.0, read_meta=True, **_):
+    def __init__(self, root_dir, split='train', downsample=1.0, read_meta=True, lens_distortion=False, **_):
         super().__init__(root_dir, split, downsample)
+        self.lens_distortion = bool(lens_distortion)
         self.read_intrinsics()
         if read_meta:
             self.read_meta(split)
@@ -42,8 +46,27 @@ class NGPDataset(BaseDataset):
         meta = self._meta()
         w, h = int(meta['w'] * self.downsample), int(meta['h'] * self.downsample)
         fx, fy = meta['fl_x'] * self.downsample, meta['fl_y'] * self.downsample
+        if self.lens_distortion:
+            self._read_camera(meta, fx, fy, w, h)
+            return
         self.K = torch.from_numpy(np.float32([[fx, 0, w / 2], [0, fy, h / 2], [0, 0, 1]]))
         self.directions = get_ray_directions(h, w, self.K)
+        self.img_wh = (w, h)
+
+    def _read_camera(self, meta, fx, fy, w, h):
+        from taichi_nerfs_b200.intrinsics import Camera
+        where = f"{self.root_dir}/transforms.json"
+        if meta.get('is_fisheye', False):
+            raise ValueError(f"{where}: is_fisheye cameras are not supported")
+        for k in ('k3', 'k4'):
+            if float(meta.get(k, 0.0)) != 0.0:
+                raise ValueError(f"{where}: a non-zero {k} is not supported (k1 k2 p1 p2 are)")
+        cx = meta['cx'] * self.downsample if 'cx' in meta else w / 2
+        cy = meta['cy'] * self.downsample if 'cy' in meta else h / 2
+        dist = tuple(float(meta.get(k, 0.0)) for k in ('k1', 'k2', 'p1', 'p2'))
+        self.camera = Camera('OPENCV', fx, fy, cx, cy, dist)
+        self.K = self.camera.K()
+        self.directions = get_ray_directions(h, w, self.K)   # the pinhole table until to(device) unprojects
         self.img_wh = (w, h)
 
     def read_meta(self, split):

@@ -660,6 +660,39 @@ int ngp_pose_adam(float* corr, float* grad, float* exp_avg, float* exp_avg_sq, c
                   const float* hyper_dev, float lr_ratio, float beta1, float beta2, float eps, int64_t n_img,
                   void* stream);
 
+/* ---- camera intrinsics: lens distortion and intrinsics refinement (DESIGN.md §6l) ------------------------------
+ * A camera is a model id and params[8] fp64 (host memory) = (fx, fy, cx, cy, k1, k2, p1, p2) in pixels (distortion
+ * terms unscaled, on normalised coordinates): model 0 PINHOLE, 1 SIMPLE_RADIAL (k1), 2 RADIAL (k1, k2), 3 OPENCV
+ * (k1, k2, p1, p2); the terms a model does not have must be 0.  W, H in [1, 2^24].  The distortion map D sends
+ * undistorted (x, y), r^2 = x^2 + y^2, to x (1 + k1 r^2 + k2 r^4) + 2 p1 x y + p2 (r^2 + 2 x^2) and
+ * y (1 + k1 r^2 + k2 r^4) + p1 (r^2 + 2 y^2) + 2 p2 x y.  Intrinsics corrections corr [4] fp32 = (a, b_x, b_y, 0),
+ * 16-byte aligned: fx' = fx e^a, fy' = fy e^a, cx' = cx + W b_x, cy' = cy + H b_y, each in fp64 rounded once.
+ * ngp_camera_unproject: dirs [n, 3] fp32 of pixels pix_idxs [n] int64 (clamped to [0, W H)), or of every pixel when
+ * pix_idxs is null (n = W H): x_d = ((u - cx') + 0.5) / fx', y_d likewise (strict fp32, get_ray_directions' order),
+ * (x_u, y_u) = D^-1(x_d, y_d) by fp64 Newton from (x_d, y_d), rounded once; dirs = (x_u, y_u, 1).  With no distortion
+ * and zero (or null) corrections dirs equal get_ray_directions bit for bit.  A pixel whose Newton does not converge or
+ * ends with det J_D <= 0 or a radial factor 1 + k1 r^2 + k2 r^4 <= 0 is not invertible: it gets (x_d, y_d, 1), *n_bad is incremented and *found_inf set to 1 (each
+ * optional).  grad_rows [n, 4] fp32 (optional) is zeroed: the per-ray rows ngp_intrinsics_grad then fills.
+ * ngp_intrinsics_grad: for each of the first min(n_rays, *n_rays_dev) rows (ray, start, count) of rays_a, G_d =
+ * sum_s t_s dx[s] (fixed order), g_c = R'^T G_d with R' the rotation of ngp_pose_apply for poses [n_img, 3, 4] and
+ * pose corrections [n_img, 8] (or null: R), g = J_D(cam_dirs[ray])^-T g_c[0:2], and grad_rays[ray] = (-(g . (x_d,
+ * y_d)), -(W / fx') g_x, -(H / fy') g_y, 0) for rays < max_rays.  pix_idxs and img_idxs are indexed by ray id.  A
+ * non-finite row sets *found_inf = 1.
+ * ngp_intrinsics_adam: one CTA sums grad_rays [n_rays, 4] in a fixed fp64 order (bitwise reproducible), writes the sum
+ * to grad_out (optional), and unless *found_inf != 0 runs the Adam of ngp_adam_step_dyn on corr with lr/bc1 =
+ * lr_ratio * hyper_dev[0], sqrt(bc2) = hyper_dev[1], inv_scale = hyper_dev[2]. */
+int ngp_camera_unproject(const int64_t* pix_idxs_or_null, int64_t n, int64_t W, int64_t H, int model,
+                         const double* params, const float* corr_or_null, float* dirs, float* grad_rows_or_null,
+                         int32_t* n_bad_or_null, int32_t* found_inf_or_null, void* stream);
+int ngp_intrinsics_grad(const float* dx, const float* ts, const int32_t* rays_a, int64_t n_rays,
+                        const int32_t* n_rays_dev, int64_t n_rows, const int64_t* pix_idxs, const int64_t* img_idxs,
+                        const float* poses, const float* pose_corr_or_null, int64_t n_img, const float* cam_dirs,
+                        int64_t W, int64_t H, int model, const double* params, const float* corr, float* grad_rays,
+                        int64_t max_rays, int32_t* found_inf_or_null, void* stream);
+int ngp_intrinsics_adam(float* corr, const float* grad_rays, int64_t n_rays, float* exp_avg, float* exp_avg_sq,
+                        const int32_t* found_inf_or_null, const float* hyper_dev, float lr_ratio, float beta1,
+                        float beta2, float eps, float* grad_out_or_null, void* stream);
+
 /* ---- error-map ray sampling (DESIGN.md §6j) ---------------------------------------------------------------------
  * Each of n_img images (W x H) is cut into R x R tiles (0 < R <= min(W, H), n_img W H < 2^40); pixel pix = y W + x
  * lies in tile t = img R^2 + floor(y R / H) R + floor(x R / W) of T = n_img R^2.  Map state: E [T] uint64 (per-tile

@@ -170,12 +170,33 @@ class NGP(nn.Module):
         return cells
 
     @torch.no_grad()
-    def mark_invisible_cells(self, K, poses, img_wh, chunk=32 ** 3):
-        """Cells no camera sees get density -1 (networks.py:211-253); runs once before training."""
+    def mark_invisible_cells(self, K, poses, img_wh, chunk=32 ** 3, camera=None):
+        """Cells no camera sees get density -1 (networks.py:211-253); runs once before training.  With a distorted
+        ``camera`` (taichi_nerfs_b200.intrinsics.Camera, DESIGN.md §6l) a cell centre projects to (x, y) = X / Z, then
+        through the distortion map D and K; it counts only when x^2 + y^2 is at most the largest undistorted radius^2
+        of the image's border pixels, so the fold of D cannot bring far-off cells back into the image."""
         n_cams = poses.shape[0]
         self.count_grid = torch.zeros_like(self.density_grid)
         w2c_R = poses[:, :3, :3].transpose(1, 2)
         w2c_T = -w2c_R @ poses[:, :3, 3:]
+        if camera is not None and camera.has_distortion:
+            from taichi_nerfs_b200 import intrinsics, ops
+            border = torch.from_numpy(intrinsics.border_pixels(*img_wh)).to(poses.device)
+            bd = ops.camera_unproject(camera, *img_wh, border).double()
+            r2_max = float((bd[:, 0] ** 2 + bd[:, 1] ** 2).max())
+            fx, fy, cx, cy = camera.params[:4]
+
+            def project(xyzs_c):   # [n_cams, 3, n] -> (u, v, depth) [n_cams, n] each
+                z = xyzs_c[:, 2].double()
+                x, y = xyzs_c[:, 0].double() / z, xyzs_c[:, 1].double() / z
+                xd, yd = intrinsics.distort_np(camera, x, y)
+                u = torch.where(x * x + y * y <= r2_max, fx * xd + cx, -1.0)
+                return u, fy * yd + cy, xyzs_c[:, 2]
+        else:
+            def project(xyzs_c):
+                uvd = K @ xyzs_c
+                uv = uvd[:, :2] / uvd[:, 2:]
+                return uv[:, 0], uv[:, 1], uvd[:, 2]
         cells = self.get_all_cells()
         for c in range(self.cascades):
             indices, coords = cells[c]
@@ -185,14 +206,12 @@ class NGP(nn.Module):
                 xyzs = coords[i:i + chunk] / (self.grid_size - 1) * 2 - 1
                 xyzs_w = (xyzs * (s - half_grid_size)).T
                 xyzs_c = w2c_R @ xyzs_w + w2c_T
-                uvd = K @ xyzs_c
-                uv = uvd[:, :2] / uvd[:, 2:]
-                in_image = (uvd[:, 2] >= 0) & (uv[:, 0] >= 0) & (uv[:, 0] < img_wh[0]) & \
-                           (uv[:, 1] >= 0) & (uv[:, 1] < img_wh[1])
-                covered = (uvd[:, 2] >= NEAR_DISTANCE) & in_image
+                u, v, depth = project(xyzs_c)
+                in_image = (depth >= 0) & (u >= 0) & (u < img_wh[0]) & (v >= 0) & (v < img_wh[1])
+                covered = (depth >= NEAR_DISTANCE) & in_image
                 count = covered.sum(0) / n_cams
                 self.count_grid[c, indices[i:i + chunk]] = count
-                too_near = ((uvd[:, 2] < NEAR_DISTANCE) & in_image).any(0)
+                too_near = ((depth < NEAR_DISTANCE) & in_image).any(0)
                 valid = (count > 0) & (~too_near)
                 self.density_grid[c, indices[i:i + chunk]] = torch.where(valid, 0., -1.)
 

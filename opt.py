@@ -68,6 +68,12 @@ _FLAGS = [
     ('--exposure_lr', dict(type=float, default=0.,
                            help='learning rate of the per-image exposures (a log2 gain per colour channel, DESIGN.md '
                                 '§6k), 0 to disable (default); every model kind, one GPU')),
+    ('--lens_distortion', dict(action='store_true', default=False,
+                               help='keep the lens distortion of the COLMAP camera or transforms.json (k1 k2 p1 p2) '
+                                    'and unproject every pixel through it (DESIGN.md §6l); --dataset_name colmap | ngp')),
+    ('--intrinsics_lr', dict(type=float, default=0.,
+                             help='learning rate of the camera intrinsics corrections (log focal scale and principal '
+                                  'point, DESIGN.md §6l), 0 to disable (default); hash encoder only, one GPU')),
     # misc
     ('--exp_name', dict(type=str, default='exp', help='experiment name')),
     ('--gpu', dict(type=int, default=0, help='set cuda device (ignored under torchrun: LOCAL_RANK wins)')),
@@ -132,6 +138,23 @@ def get_opts(prefix_args=None):
         if hparams.encoder_type == 'triplane':
             parser.error("--extrinsics_lr does not combine with --encoder_type triplane: the tri-plane encoder gives no "
                          "gradient wrt the sample positions")
+    if hparams.lens_distortion and hparams.dataset_name not in ('colmap', 'ngp'):
+        parser.error(f"--lens_distortion reads the distortion terms of a COLMAP camera or transforms.json: it needs "
+                     f"--dataset_name colmap | ngp, got {hparams.dataset_name}")
+    if not (math.isfinite(hparams.intrinsics_lr) and hparams.intrinsics_lr >= 0):
+        parser.error(f"--intrinsics_lr must be finite and >= 0, got {hparams.intrinsics_lr}")
+    if hparams.intrinsics_lr > 0:
+        if not (math.isfinite(hparams.lr) and hparams.lr > 0):
+            parser.error(f"--intrinsics_lr is set relative to the model's learning rate: it needs a finite --lr > 0, got "
+                         f"{hparams.lr}")
+        if hparams.model_name == 'svox':
+            parser.error("--intrinsics_lr does not combine with --model_name svox: the voxel grid gives no gradient "
+                         "wrt the sample positions")
+        if hparams.encoder_type == 'triplane':
+            parser.error("--intrinsics_lr does not combine with --encoder_type triplane: the tri-plane encoder gives no "
+                         "gradient wrt the sample positions")
+        if int(os.environ.get("WORLD_SIZE", "1")) > 1:
+            parser.error("--intrinsics_lr trains on one GPU: the intrinsics gradient is not exchanged between ranks")
     if not (math.isfinite(hparams.exposure_lr) and hparams.exposure_lr >= 0):
         parser.error(f"--exposure_lr must be finite and >= 0, got {hparams.exposure_lr}")
     if hparams.exposure_lr > 0:

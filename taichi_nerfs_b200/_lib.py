@@ -125,6 +125,10 @@ def _declare(lib):
         "ngp_pose_apply": (ci, [vp, vp, vp, vp, i64, vp, vp, i64, vp]),
         "ngp_pose_grad": (ci, [vp, vp, vp, vp, vp, i64, vp, i64, i64, vp, vp, vp]),
         "ngp_pose_adam": (ci, [vp, vp, vp, vp, vp, vp, f32, f32, f32, f32, i64, vp]),
+        "ngp_camera_unproject": (ci, [vp, i64, i64, i64, ci, vp, vp, vp, vp, vp, vp, vp]),
+        "ngp_intrinsics_grad": (ci, [vp, vp, vp, i64, vp, i64, vp, vp, vp, vp, i64, vp, i64, i64, ci, vp, vp, vp, i64,
+                                     vp, vp]),
+        "ngp_intrinsics_adam": (ci, [vp, vp, i64, vp, vp, vp, vp, f32, f32, f32, f32, vp, vp]),
         "ngp_error_map_workspace_bytes": (i64, [i64]),
         "ngp_error_map_sample": (ci, [vp, i64, i64, i64, i64, C.c_uint64, vp, i32, vp, vp, vp, i64, vp]),
         "ngp_error_map_accumulate": (ci, [vp, vp, vp, vp, f32, vp, vp, i64, i64, i64, i64, vp, vp, i64, vp]),

@@ -8,38 +8,12 @@
 //   ngp_pose_grad:  per ray G_o = sum_s g_s, G_d = sum_s t_s g_s (g_s = dL/dx_s of the ray's samples); per image
 //                   grad[i] += (d' x G_d, G_o).
 //   ngp_pose_adam:  omega gradient through J_l(omega)^T, unscale, inf-skip, Adam, gradient zeroed.
-#include "common.cuh"
+#include "refine.cuh"
 
 namespace {
 
-// theta^2 below which Exp and J_l use their Taylor series (the closed forms cancel there); fp64, so the series'
-// first omitted term (theta^6 / 5040 at most) stays far below fp32 precision
-constexpr double kSeriesTheta2 = 1e-6;
-
-// Exp(w) = I + A K + B K^2, K = [w]x, A = sin(t)/t, B = (1 - cos t)/t^2 = 2 sin^2(t/2)/t^2 (no cancellation)
-__device__ void so3_exp(const double w[3], double E[9]) {
-    const double t2 = w[0] * w[0] + w[1] * w[1] + w[2] * w[2];
-    double A, B;
-    if (t2 < kSeriesTheta2) {
-        A = 1.0 - t2 / 6.0 + t2 * t2 / 120.0;
-        B = 0.5 - t2 / 24.0 + t2 * t2 / 720.0;
-    } else {
-        const double t = sqrt(t2), s = sin(0.5 * t);
-        A = sin(t) / t;
-        B = 2.0 * s * s / t2;
-    }
-    // K^2 = w w^T - t^2 I
-    const double c = 1.0 - B * t2;
-    E[0] = c + B * w[0] * w[0];
-    E[4] = c + B * w[1] * w[1];
-    E[8] = c + B * w[2] * w[2];
-    E[1] = B * w[0] * w[1] - A * w[2];
-    E[3] = B * w[0] * w[1] + A * w[2];
-    E[2] = B * w[0] * w[2] + A * w[1];
-    E[6] = B * w[0] * w[2] - A * w[1];
-    E[5] = B * w[1] * w[2] - A * w[0];
-    E[7] = B * w[1] * w[2] + A * w[0];
-}
+using ngp::kSeriesTheta2;
+using ngp::so3_exp;
 
 __device__ __forceinline__ int64_t clamp_img(int64_t img, int64_t n_img) {
     return min(max(img, (int64_t)0), n_img - 1);
@@ -55,28 +29,9 @@ __global__ void __launch_bounds__(256) pose_apply_kernel(const float* __restrict
     if (i >= n) return;
     const int64_t img = clamp_img(img_idxs[i], n_img);
     const float* P = poses + img * 12;   // row-major [3][4] camera-to-world
-    const float4 w4 = reinterpret_cast<const float4*>(corr)[img * 2 + 0];
     const float4 t4 = reinterpret_cast<const float4*>(corr)[img * 2 + 1];
     float R[9];
-#pragma unroll
-    for (int a = 0; a < 3; ++a)
-#pragma unroll
-        for (int k = 0; k < 3; ++k) R[a * 3 + k] = P[a * 4 + k];
-    if (w4.x != 0.0f || w4.y != 0.0f || w4.z != 0.0f) {
-        // R' = Exp(omega) R in fp64, rounded once; omega = 0 keeps R itself (Exp(0) R is exactly R)
-        const double w[3] = {w4.x, w4.y, w4.z};
-        double E[9];
-        so3_exp(w, E);
-        float Rn[9];
-#pragma unroll
-        for (int a = 0; a < 3; ++a)
-#pragma unroll
-            for (int k = 0; k < 3; ++k)
-                Rn[a * 3 + k] = (float)(E[a * 3 + 0] * (double)R[k] + E[a * 3 + 1] * (double)R[3 + k] +
-                                        E[a * 3 + 2] * (double)R[6 + k]);
-#pragma unroll
-        for (int k = 0; k < 9; ++k) R[k] = Rn[k];
-    }
+    ngp::corrected_rotation(poses, corr, img, R);   // omega = 0 keeps R (Exp(0) R is exactly R)
     const float d0 = dirs[i * 3 + 0], d1 = dirs[i * 3 + 1], d2 = dirs[i * 3 + 2];
     const float tau[3] = {t4.x, t4.y, t4.z};
 #pragma unroll
@@ -181,16 +136,6 @@ __device__ void so3_jl_transpose_apply(const double w[3], const double g[3], dou
     for (int a = 0; a < 3; ++a) out[a] = g[a] - B * kg[a] + Cc * (w[a] * wg - t2 * g[a]);
 }
 
-// Adam of ngp_adam_step_dyn (optim.cu, adam1), contractions spelled out the same way
-__device__ __forceinline__ void pose_adam1(float& p, float g, float& m, float& v, float lr_over_bc1, float bc2_sqrt,
-                                           float beta1, float beta2, float eps, float inv_scale) {
-    const float gg = __fmul_rn(g, inv_scale);
-    m = __fmaf_rn(__fsub_rn(gg, m), 1.0f - beta1, m);
-    v = __fmaf_rn(v, beta2, __fmul_rn(__fmul_rn(1.0f - beta2, gg), gg));
-    const float denom = __fadd_rn(__fdiv_rn(sqrtf(v), bc2_sqrt), eps);
-    p = __fmaf_rn(-lr_over_bc1, __fdiv_rn(m, denom), p);
-}
-
 __global__ void __launch_bounds__(128) pose_adam_kernel(float* __restrict__ corr, float* __restrict__ grad,
                                                         float* __restrict__ exp_avg, float* __restrict__ exp_avg_sq,
                                                         const int32_t* __restrict__ found_inf,
@@ -211,12 +156,12 @@ __global__ void __launch_bounds__(128) pose_adam_kernel(float* __restrict__ corr
         double gj[3];
         so3_jl_transpose_apply(w, gw, gj);
         const float lr = __fmul_rn(lr_ratio, hyper[0]), bc2 = hyper[1], inv = hyper[2];
-        pose_adam1(p0.x, (float)gj[0], m0.x, v0.x, lr, bc2, beta1, beta2, eps, inv);
-        pose_adam1(p0.y, (float)gj[1], m0.y, v0.y, lr, bc2, beta1, beta2, eps, inv);
-        pose_adam1(p0.z, (float)gj[2], m0.z, v0.z, lr, bc2, beta1, beta2, eps, inv);
-        pose_adam1(p1.x, g1.x, m1.x, v1.x, lr, bc2, beta1, beta2, eps, inv);
-        pose_adam1(p1.y, g1.y, m1.y, v1.y, lr, bc2, beta1, beta2, eps, inv);
-        pose_adam1(p1.z, g1.z, m1.z, v1.z, lr, bc2, beta1, beta2, eps, inv);
+        ngp::refine_adam1(p0.x, (float)gj[0], m0.x, v0.x, lr, bc2, beta1, beta2, eps, inv);
+        ngp::refine_adam1(p0.y, (float)gj[1], m0.y, v0.y, lr, bc2, beta1, beta2, eps, inv);
+        ngp::refine_adam1(p0.z, (float)gj[2], m0.z, v0.z, lr, bc2, beta1, beta2, eps, inv);
+        ngp::refine_adam1(p1.x, g1.x, m1.x, v1.x, lr, bc2, beta1, beta2, eps, inv);
+        ngp::refine_adam1(p1.y, g1.y, m1.y, v1.y, lr, bc2, beta1, beta2, eps, inv);
+        ngp::refine_adam1(p1.z, g1.z, m1.z, v1.z, lr, bc2, beta1, beta2, eps, inv);
         P[0] = p0;
         P[1] = p1;
         M[0] = m0;

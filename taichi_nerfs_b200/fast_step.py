@@ -12,6 +12,11 @@ With camera extrinsics refinement (DESIGN.md §6i) the rays come from the pose-a
 camera directions and image indices), the hash backward is followed by the position gradient and the pose gradient,
 and the corrections' Adam runs next to the model's.
 
+With camera intrinsics refinement (DESIGN.md §6l) the step's first nodes after the reset are the camera unproject (the
+rays' camera directions from their pixels under the corrected intrinsics, which also clears the per-ray gradient rows)
+and the pose apply (with the extrinsics corrections, or a zero buffer); the hash backward is followed by the one
+position-gradient pass and the intrinsics gradient, and the intrinsics Adam runs next to the model's.
+
 With error-map sampling (DESIGN.md §6j) each ray carries a weight w_r: the head is followed by the error-map accumulate
 (the rays' errors into their tiles) and by the gradient weight (every per-sample gradient of ray r times w_r), so the
 backward sees the gradient of the weighted loss; loss_sum, the logged value, stays the unweighted one.  The sampled step
@@ -35,7 +40,7 @@ import ctypes as C
 
 import torch
 
-from . import _lib, parallel
+from . import _lib, ops, parallel
 from ._lib import F16, F32, check, load
 from .fused_mlp import mlp_weights
 
@@ -67,6 +72,14 @@ class StaticTrainStep:
             raise ValueError("StaticTrainStep: extrinsics must be the trainer's PoseRefinement "
                              "(NGPTrainer(extrinsics=...)), or None for a trainer without one")
         self.ext = extrinsics
+        # intrinsics: the trainer's IntrinsicsRefinement (NGPTrainer(intrinsics=...)), shared with the module path
+        self.intr = trainer.intrinsics
+        if self.intr is not None:
+            if overlap_optimizer:
+                raise _lib.NgpError("StaticTrainStep: intrinsics refinement does not combine with overlap_optimizer "
+                                    "(the next step's march would read intrinsics one update stale)")
+            if trainer.world_size > 1:
+                raise _lib.NgpError("StaticTrainStep: intrinsics refinement runs on one rank")
         # error_map: a taichi_nerfs_b200.error_map.ErrorMap over the training images, or None (nothing is enqueued)
         self.em = error_map
         # exposure compensation: the trainer's ExposureCorrection (NGPTrainer(exposure=...)), shared with the module path
@@ -121,19 +134,27 @@ class StaticTrainStep:
         self.bg_rgb, self.alpha = (z(self.n, 3), torch.ones(self.n, device=dev)) if self.random_bg else (None, None)
         self.depth_gt = z(self.n) if self.depth_w > 0 else None   # per-ray target z-depth, 0 = none
         # extrinsics refinement: camera directions and image indices in, dL/dx of every sample row
-        if self.ext is not None:
+        if self.ext is not None or self.intr is not None:
             self.cam_dirs, self.img_idx = z(self.n, 3), torch.zeros(self.n, device=dev, dtype=torch.int64)
             self.cam_dirs[:, 2] = -1.0   # valid placeholder rays for the capture (a zero direction never advances)
             self.dx = z(C_, 3)
+        if self.intr is not None:
+            # each ray's pixel; the pose apply's corrections when extrinsics refinement is off (zero: the rays of
+            # get_rays bit for bit, DESIGN.md §6i)
+            self.pix = torch.zeros(self.n, device=dev, dtype=torch.int64)
+            self.pose_corr = self.ext.corr if self.ext is not None else z(self.intr.n_img, 8)
+            self.intr.reserve(self.n)
+            self.intr.n_rays = self.n
         if self.em is not None:   # each ray's image, pixel and loss weight
             self.em_img = torch.zeros(self.n, device=dev, dtype=torch.int64)
-            self.em_pix = torch.zeros(self.n, device=dev, dtype=torch.int64)
+            self.em_pix = self.pix if self.intr is not None else torch.zeros(self.n, device=dev, dtype=torch.int64)
             self.ray_w = torch.ones(self.n, device=dev)
         if self.expo is not None:
             # the head's copy of the sample colours under their images' gains; each ray's image is the index buffer
             # extrinsics refinement or the error map fill, else one of its own (step(img_idxs=...) or the sampler)
             self.rgbs_expo = torch.zeros_like(self.rgbs)
-            self.expo_img = (self.img_idx if self.ext is not None else self.em_img if self.em is not None
+            self.expo_img = (self.img_idx if self.ext is not None or self.intr is not None
+                             else self.em_img if self.em is not None
                              else torch.zeros(self.n, device=dev, dtype=torch.int64))
         self._head_rgbs = self.rgbs_expo if self.expo is not None else self.rgbs
         # GradScaler state on the device: [scale, growth_tracker (int bits)]; growth 2x / 2000 clean steps, backoff 0.5
@@ -305,6 +326,27 @@ class StaticTrainStep:
                                                    self.enc._tag(), C.byref(self.enc._clayout), _p(self.dx),
                                                    self.cap, _p(self.counter), self.aabb6, self._st()))
 
+    # intrinsics refinement (DESIGN.md §6l): the rays' camera directions from their pixels; the intrinsics gradient
+    def _k_unproject(self):
+        i = self.intr
+        model, params = ops._camera_args(i.camera)
+        check(load().ngp_camera_unproject(_p(self.pix), self.n, i.W, i.H, model, params, _p(i.corr), _p(self.cam_dirs),
+                                          _p(i.grad_rays), None, _p(self.tr.found_inf), self._st()))
+
+    def _k_pose_apply_intr(self):
+        i = self.intr
+        check(load().ngp_pose_apply(_p(self.cam_dirs), _p(self.img_idx), _p(i.poses), _p(self.pose_corr), i.n_img,
+                                    _p(self.rays_o), _p(self.rays_d), self.n, self._st()))
+
+    def _k_intr_grad(self):
+        i = self.intr
+        model, params = ops._camera_args(i.camera)
+        check(load().ngp_intrinsics_grad(_p(self.dx), _p(self.ts), _p(self.rays_a), self.n, None, self.cap,
+                                         _p(self.pix), _p(self.img_idx), _p(i.poses),
+                                         _p(self.ext.corr) if self.ext is not None else None, i.n_img,
+                                         _p(self.cam_dirs), i.W, i.H, model, params, _p(i.corr), _p(i.grad_rays),
+                                         self.n, _p(self.tr.found_inf), self._st()))
+
     def _k_pose_grad(self):
         e = self.ext
         check(load().ngp_pose_grad(_p(self.dx), _p(self.ts), _p(self.rays_a), _p(self.img_idx), _p(self.rays_d),
@@ -375,9 +417,12 @@ class StaticTrainStep:
         self._k_head_exposed()
         self._k_mlp_bwd()
         self._k_hash_bwd()
-        if self.ext is not None:
+        if self.ext is not None or self.intr is not None:   # one position-gradient pass feeds both
             self._k_hash_dx()
+        if self.ext is not None:
             self._k_pose_grad()
+        if self.intr is not None:
+            self._k_intr_grad()
 
     def _enqueue_sampler(self):
         """datasets/base.py:34-61 + ray_utils.py:51-80 + the marching jitter, keyed by (seed, batch counter, ray)."""
@@ -399,7 +444,7 @@ class StaticTrainStep:
         self.tr.enqueue_update(check_finite=not self.inf_at_source, voxel_block=self.block if self.vox else None)
 
     def _enqueue(self, sampled=False, mode="sync"):
-        if self.ext is not None:
+        if self.ext is not None and self.intr is None:
             self._k_pose_apply()
         if sampled:
             self._enqueue_sampler()
@@ -410,6 +455,9 @@ class StaticTrainStep:
                                     None if self.inf_at_source else _p(self.tr.found_inf),
                                     _p(self.sample_step) if sampled else _p(self.bg_step) if self.random_bg else None,
                                     self._st()))
+        if self.intr is not None:   # after the reset: a pixel that is not invertible raises found_inf for this step
+            self._k_unproject()
+            self._k_pose_apply_intr()
         if mode == "steady":
             # optimizer of the PREVIOUS step beside this step's ray_aabb + marching.  The marching branch runs on
             # a high-priority stream (the priority is kept by the captured kernel nodes): its latency-bound warps
@@ -436,6 +484,7 @@ class StaticTrainStep:
         ext_keep = [] if self.ext is None else [t.clone() for t in self.ext.state()]
         em_keep = [] if self.em is None else [t.clone() for t in self.em.state()]
         expo_keep = [] if self.expo is None else [t.clone() for t in self.expo.state()]
+        intr_keep = [] if self.intr is None else [t.clone() for t in self.intr.state()]
         shadow = None if tr._shadow_full is None else tr._shadow_full.clone()
         side = torch.cuda.Stream()
         side.wait_stream(torch.cuda.current_stream())
@@ -468,6 +517,9 @@ class StaticTrainStep:
         if self.expo is not None:
             for t, k in zip(self.expo.state(), expo_keep):
                 t.copy_(k)
+        if self.intr is not None:
+            for t, k in zip(self.intr.state(), intr_keep):
+                t.copy_(k)
         tr.flat_grad.zero_()
         if shadow is not None:
             tr._shadow_full.copy_(shadow)
@@ -482,10 +534,18 @@ class StaticTrainStep:
         extrinsics refinement the step forms its rays itself: rays_o and rays_d are None and ``directions`` [N, 3]
         (camera frame) and ``img_idxs`` [N] (or one index for the whole batch) are required.  With an error map,
         ``ray_w`` [N] (the loss weights of ErrorMap.draw), ``img_idxs`` and ``pix_idxs`` [N] are required.  With exposure
-        compensation ``img_idxs`` [N] (or one index) is required."""
+        compensation ``img_idxs`` [N] (or one index) is required.  With intrinsics refinement the step forms its rays
+        from pixels: rays_o, rays_d and ``directions`` are None, and ``img_idxs`` and ``pix_idxs`` [N] are required."""
         if self.expo is not None and img_idxs is None:
             raise ValueError("exposure compensation: step(..., img_idxs=...) (each ray's image, whose gain its samples "
                              "take)")
+        if self.intr is not None:
+            if pix_idxs is None or img_idxs is None or rays_o is not None or rays_d is not None or \
+                    directions is not None:
+                raise ValueError("intrinsics refinement: step(None, None, rgb, ..., img_idxs=..., pix_idxs=...) (the "
+                                 "step forms the rays from the pixels under the corrected intrinsics)")
+            self.pix.copy_(torch.as_tensor(pix_idxs, device=self.dev).reshape(-1), non_blocking=True)
+            self.img_idx.copy_(torch.as_tensor(img_idxs, device=self.dev).reshape(-1), non_blocking=True)
         if self.em is not None:
             if ray_w is None or img_idxs is None or pix_idxs is None:
                 raise ValueError("error-map sampling: step(..., ray_w=..., img_idxs=..., pix_idxs=...) (the rays' loss "
@@ -493,9 +553,11 @@ class StaticTrainStep:
             self.ray_w.copy_(ray_w, non_blocking=True)
             self.em_img.copy_(torch.as_tensor(img_idxs, device=self.dev).reshape(-1), non_blocking=True)
             self.em_pix.copy_(pix_idxs, non_blocking=True)
-        elif ray_w is not None or pix_idxs is not None:
+        elif ray_w is not None or (pix_idxs is not None and self.intr is None):
             raise ValueError("ray_w / pix_idxs are read by error-map sampling only (StaticTrainStep(error_map=...))")
-        if self.ext is not None:
+        if self.intr is not None:
+            pass
+        elif self.ext is not None:
             if directions is None or img_idxs is None or rays_o is not None or rays_d is not None:
                 raise ValueError("extrinsics refinement: step(None, None, rgb, ..., directions=..., img_idxs=...) "
                                  "(the step forms the rays from the corrected poses)")
@@ -513,7 +575,7 @@ class StaticTrainStep:
             raise ValueError("depth is read by the depth loss only (StaticTrainStep(depth_loss_w=...))")
         if depth is not None:
             self.depth_gt.copy_(depth, non_blocking=True)
-        if self.ext is None:
+        if self.ext is None and self.intr is None:
             self.rays_o.copy_(rays_o, non_blocking=True)
             self.rays_d.copy_(rays_d, non_blocking=True)
         self.gt.copy_(rgb_gt, non_blocking=True)
@@ -572,6 +634,9 @@ class StaticTrainStep:
         if self.ext is not None:
             raise _lib.NgpError("the device-sampled step does not support extrinsics refinement yet; use "
                                 "step(directions=..., img_idxs=...)")
+        if self.intr is not None:
+            raise _lib.NgpError("the device-sampled step does not support intrinsics refinement; use "
+                                "step(img_idxs=..., pix_idxs=...)")
         f = lambda t: t.detach().to(self.dev, torch.float32).contiguous()  # noqa: E731
         bank, poses, directions = f(image_bank), f(poses), f(directions)
         if bank.ndim != 3 or bank.shape[0] != poses.shape[0] or bank.shape[1] != directions.shape[0] or bank.shape[2] < 3:

@@ -679,6 +679,98 @@ def exposure_adam(expo, grad, exp_avg, exp_avg_sq, hyper, lr_ratio, found_inf=No
                                    _stream()), "exposure_adam")
 
 
+# ---- camera intrinsics (DESIGN.md §6l) ---------------------------------------------------------------------------
+def _camera_args(camera):
+    """(model id, fp64 [8] host array) of a taichi_nerfs_b200.intrinsics.Camera."""
+    return int(camera.model_id), (C.c_double * 8)(*[float(v) for v in camera.params])
+
+
+def _intrinsics_buffer(t, rows, what):
+    if t.dtype != torch.float32 or not t.is_contiguous() or t.dim() != 2 or t.shape[1] != 4 or \
+            (rows is not None and t.shape[0] != rows):
+        raise TypeError(f"{what} must be contiguous fp32 [{'n' if rows is None else rows}, 4]")
+
+
+def camera_unproject(camera, W, H, pix_idxs=None, corr=None, out=None, grad_rows=None, n_bad=None, found_inf=None,
+                     device=None):
+    """Camera-frame directions [n, 3] fp32 (x_u, y_u, 1) of pixels pix_idxs [n] int64 of a W x H image, or of all W*H
+    pixels of ``device`` when pix_idxs is None, under the corrections corr [1, 4] (or none).  grad_rows [n, 4]
+    (optional) is zeroed; n_bad (int32 [1]) counts and found_inf (int32 [1]) flags the pixels that are not
+    invertible."""
+    dev = torch.device(device) if pix_idxs is None else pix_idxs.device
+    if dev.type != "cuda":
+        raise _lib.NgpError("libngp_b200 ops need CUDA tensors (there is no CPU fallback)")
+    _need_cuda(pix_idxs, corr, out, grad_rows, n_bad, found_inf)
+    if pix_idxs is not None and (pix_idxs.dtype != torch.int64 or not pix_idxs.is_contiguous()):
+        raise TypeError("camera_unproject: pix_idxs must be contiguous int64")
+    n = int(W) * int(H) if pix_idxs is None else pix_idxs.numel()
+    if corr is not None:
+        _intrinsics_buffer(corr, 1, "intrinsics corrections")
+    if grad_rows is not None:
+        _intrinsics_buffer(grad_rows, None, "camera_unproject: grad_rows")
+        if grad_rows.shape[0] < n:
+            raise ValueError(f"camera_unproject: grad_rows has {grad_rows.shape[0]} rows for {n} pixels")
+    out = torch.empty(n, 3, device=dev, dtype=torch.float32) if out is None else out
+    if out.dtype != torch.float32 or not out.is_contiguous() or out.numel() != 3 * n:
+        raise ValueError(f"camera_unproject: out must be contiguous fp32 [{n}, 3]")
+    model, params = _camera_args(camera)
+    check(load().ngp_camera_unproject(_ptr(pix_idxs), n, int(W), int(H), model, params, _ptr(corr), _ptr(out),
+                                      _ptr(grad_rows), _ptr(n_bad), _ptr(found_inf), _stream()), "camera_unproject")
+    return out
+
+
+def intrinsics_grad(dx, ts, rays_a, pix_idxs, img_idxs, poses, cam_dirs, camera, W, H, corr, grad_rays,
+                    pose_corr=None, n_rays_dev=None, found_inf=None):
+    """grad_rays[ray] [max_rays, 4] = (dL/da, dL/db_x, dL/db_y, 0) of every ray of rays_a [n, 3] (ray, start, count),
+    from the sample gradients dx [S, 3] and times ts [S]; pix_idxs [n] (or more), img_idxs [n] (or one index) and
+    cam_dirs [n, 3] (the unprojected directions the rays were formed with) by ray id; poses [n_img, 3, 4] with the
+    extrinsics corrections pose_corr [n_img, 8] (or none).  Rows of rays without a rays_a row are left as they are."""
+    _need_cuda(dx, ts, rays_a, pix_idxs, img_idxs, poses, cam_dirs, corr, grad_rays, pose_corr, n_rays_dev, found_inf)
+    if dx.dtype != torch.float32 or ts.dtype != torch.float32 or rays_a.dtype != torch.int32:
+        raise TypeError("intrinsics_grad: dx and ts are fp32, rays_a int32")
+    if pix_idxs.dtype != torch.int64 or not pix_idxs.is_contiguous():
+        raise TypeError("intrinsics_grad: pix_idxs must be contiguous int64")
+    _intrinsics_buffer(corr, 1, "intrinsics corrections")
+    _intrinsics_buffer(grad_rays, None, "intrinsics_grad: grad_rays")
+    if pose_corr is not None:
+        _pose_buffers(pose_corr)
+    n = rays_a.shape[0]
+    P = _f32c(poses)
+    if P.dim() != 3 or tuple(P.shape[1:]) != (3, 4):
+        raise ValueError(f"intrinsics_grad: poses {tuple(P.shape)} must be [n_img, 3, 4]")
+    if pose_corr is not None and pose_corr.shape[0] != P.shape[0]:
+        raise ValueError("intrinsics_grad: one pose correction per pose")
+    rays = grad_rays.shape[0]
+    idx = _img_index(img_idxs, rays)
+    dxc, tsc, d = dx.contiguous(), ts.contiguous(), _f32c(cam_dirs)
+    if d.shape[0] < rays or pix_idxs.numel() < rays or tsc.shape[0] != dxc.shape[0] or n > rays:
+        raise ValueError("intrinsics_grad: cam_dirs and pix_idxs need a row per gradient row, ts one value per row of "
+                         "dx, and grad_rays a row per ray")
+    model, params = _camera_args(camera)
+    check(load().ngp_intrinsics_grad(_ptr(dxc), _ptr(tsc), _ptr(rays_a.contiguous()), n, _ptr(n_rays_dev),
+                                     dxc.shape[0], _ptr(pix_idxs), _ptr(idx), _ptr(P), _ptr(pose_corr), P.shape[0],
+                                     _ptr(d), int(W), int(H), model, params, _ptr(corr), _ptr(grad_rays), rays,
+                                     _ptr(found_inf), _stream()), "intrinsics_grad")
+
+
+def intrinsics_adam(corr, grad_rays, n_rays, exp_avg, exp_avg_sq, hyper, lr_ratio, found_inf=None, beta1=0.9,
+                    beta2=0.999, eps=1e-15, grad_out=None):
+    """The sum of grad_rays[:n_rays] (fixed fp64 order, into grad_out [1, 4] when given), then one Adam step of corr
+    [1, 4] with the model's device scalars ``hyper`` at lr_ratio times the model's learning rate (none when found_inf
+    is raised)."""
+    _need_cuda(corr, grad_rays, exp_avg, exp_avg_sq, hyper, found_inf, grad_out)
+    for t, what in ((corr, "corrections"), (exp_avg, "exp_avg"), (exp_avg_sq, "exp_avg_sq")):
+        _intrinsics_buffer(t, 1, f"intrinsics {what}")
+    if grad_out is not None:
+        _intrinsics_buffer(grad_out, 1, "intrinsics_adam: grad_out")
+    _intrinsics_buffer(grad_rays, None, "intrinsics_adam: grad_rays")
+    if not 0 <= int(n_rays) <= grad_rays.shape[0]:
+        raise ValueError(f"intrinsics_adam: n_rays {n_rays} outside [0, {grad_rays.shape[0]}]")
+    check(load().ngp_intrinsics_adam(_ptr(corr), _ptr(grad_rays), int(n_rays), _ptr(exp_avg), _ptr(exp_avg_sq),
+                                     _ptr(found_inf), _ptr(hyper), float(lr_ratio), float(beta1), float(beta2),
+                                     float(eps), _ptr(grad_out), _stream()), "intrinsics_adam")
+
+
 def morton3d(coords):
     _need_cuda(coords)
     c = coords.contiguous()

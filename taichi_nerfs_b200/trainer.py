@@ -31,11 +31,13 @@ def _p(t):
 class NGPTrainer:
     def __init__(self, model, lr: float = 1e-2, max_steps: int = 20000, loss_scale: float | None = None,
                  betas=(0.9, 0.999), eps: float = 1e-15, process_group=None, dynamic_loss_scale: bool = True,
-                 p2p_optimizer: bool | None = None, voxel_reg=None, extrinsics=None, exposure=None):
+                 p2p_optimizer: bool | None = None, voxel_reg=None, extrinsics=None, exposure=None,
+                 intrinsics=None):
         from modules.hash_encoder import HashEncoder
         from modules.voxel_grid import VoxelGrid
         from .exposure import ExposureCorrection
         from .extrinsics import PoseRefinement
+        from .intrinsics import IntrinsicsRefinement
         # The model kind, decided here once (StaticTrainStep reads it too): the position encoder, whose one parameter
         # (its table) must be the first slice of the flat buffers, or None for a VoxelGrid, which has no encoder and
         # scatters into the .grad views of its own fields.
@@ -76,6 +78,17 @@ class NGPTrainer:
                 raise ValueError("NGPTrainer: extrinsics refinement runs on one rank (the pose gradient is not "
                                  "exchanged between ranks)")
         self.extrinsics = extrinsics
+        # camera intrinsics refinement (DESIGN.md §6l): an IntrinsicsRefinement whose Adam step runs with the model's
+        if intrinsics is not None:
+            if not isinstance(intrinsics, IntrinsicsRefinement):
+                raise TypeError("NGPTrainer: intrinsics must be a taichi_nerfs_b200.intrinsics.IntrinsicsRefinement")
+            if not isinstance(enc, HashEncoder):
+                raise ValueError("NGPTrainer: intrinsics refinement needs the gradient wrt the sample positions, which "
+                                 "only the hash encoder provides (not the tri-plane encoder or the voxel grid)")
+            if self.world_size > 1:
+                raise ValueError("NGPTrainer: intrinsics refinement runs on one rank (its gradient is not exchanged "
+                                 "between ranks)")
+        self.intrinsics = intrinsics
         # per-image exposure compensation (DESIGN.md §6k): an ExposureCorrection whose Adam step runs with the model's
         if exposure is not None:
             if not isinstance(exposure, ExposureCorrection):
@@ -191,25 +204,35 @@ class NGPTrainer:
         self._views = []
 
     def forward_backward(self, rays_o, rays_d, rgb_gt, exp_step_factor=0.0, extra_loss=None, bg_rgb=None, alpha=None,
-                         b_load=1.0, img_idxs=None, ray_w=None):
+                         b_load=1.0, img_idxs=None, ray_w=None, pix_idxs=None):
         """bg_rgb [N, 3] (--random_bg, ops.random_bg): each ray's background colour replaces the fixed one; with
         ``alpha`` [N] (the image's alpha), the target's loader background ``b_load`` is replaced by it too:
         rgb_gt + (bg_rgb - b_load)(1 - alpha).  With extrinsics refinement, ``img_idxs`` [N] (or one index) names each
         ray's image and rays_o / rays_d are the PoseRefinement's rays; the pose gradient is formed by optimizer_step.
         With exposure compensation, ``img_idxs`` names each ray's image too, and the sample colours pass through its
         gain (DESIGN.md §6k).
+        With intrinsics refinement (DESIGN.md §6l) the rays' camera directions are the IntrinsicsRefinement's
+        ``directions(pix_idxs)``; ``pix_idxs`` [N] and ``img_idxs`` are required, and the intrinsics gradient is formed
+        by optimizer_step.
         ``ray_w`` [N] fp32 (error-map sampling, DESIGN.md §6j): the MSE becomes mean_r w_r mean_c (rgb - gt)^2, and the
         returned loss is that weighted value; ``extra_loss`` weights its own per-ray terms."""
         from modules.rendering import render
-        refine = self.extrinsics is not None
+        intr = self.intrinsics
+        refine = self.extrinsics is not None or intr is not None
         expo = self.exposure
         if refine and img_idxs is None:
-            raise ValueError("NGPTrainer: extrinsics refinement needs each ray's image index (img_idxs=...)")
+            raise ValueError("NGPTrainer: camera refinement needs each ray's image index (img_idxs=...)")
+        if intr is not None:
+            if pix_idxs is None or intr.pix is None or intr.n_rays != len(rays_o):
+                raise ValueError("NGPTrainer: intrinsics refinement needs each ray's pixel (pix_idxs=...), with the "
+                                 "directions of IntrinsicsRefinement.directions(pix_idxs) of this batch")
+        elif pix_idxs is not None:
+            raise ValueError("NGPTrainer: pix_idxs is read by intrinsics refinement only (NGPTrainer(intrinsics=...))")
         if expo is not None and img_idxs is None:
             raise ValueError("NGPTrainer: exposure compensation needs each ray's image index (img_idxs=...)")
         if not refine and expo is None and img_idxs is not None:
-            raise ValueError("NGPTrainer: img_idxs is read by extrinsics refinement and exposure compensation only "
-                             "(NGPTrainer(extrinsics=... | exposure=...))")
+            raise ValueError("NGPTrainer: img_idxs is read by camera refinement and exposure compensation only "
+                             "(NGPTrainer(extrinsics=... | intrinsics=... | exposure=...))")
         exposure = None if expo is None else (lambda rgbs, rays_a: expo.apply(rgbs, rays_a, img_idxs))  # noqa: E731
         if bg_rgb is not None and alpha is not None:
             rgb_gt = rgb_gt + (bg_rgb - b_load) * (1 - alpha)[:, None]
@@ -232,14 +255,20 @@ class NGPTrainer:
         return loss, results
 
     def enqueue_pose_grad(self):
-        """Extrinsics refinement: the pose gradient of the last forward_backward (its sample positions' .grad) into the
-        PoseRefinement's buffer, raising found_inf on a non-finite contribution."""
+        """Camera refinement: the pose and intrinsics gradients of the last forward_backward (its sample positions'
+        .grad) into the PoseRefinement's and IntrinsicsRefinement's buffers, raising found_inf on a non-finite
+        contribution."""
         xyzs, ts, rays_a, img_idxs, rays_d = self._pose_batch
         self._pose_batch = None
         dx = xyzs.grad
         if dx is None:   # no sample reached the network
             return
-        self.extrinsics.accumulate(dx, ts, rays_a, img_idxs, rays_d.float(), found_inf=self.found_inf)
+        if self.extrinsics is not None:
+            self.extrinsics.accumulate(dx, ts, rays_a, img_idxs, rays_d.float(), found_inf=self.found_inf)
+        if self.intrinsics is not None:
+            self.intrinsics.accumulate(dx.float(), ts, rays_a, img_idxs,
+                                       pose_corr=None if self.extrinsics is None else self.extrinsics.corr,
+                                       found_inf=self.found_inf)
 
     def add_voxel_reg(self, loss=None):
         """Add loss_scale * the gradient of the voxel regularisers into the flat gradient (the model's grad_sink), from
@@ -329,6 +358,8 @@ class NGPTrainer:
             self.extrinsics.enqueue_adam(self)
         if self.exposure is not None:     # the exposures' Adam and zero-mean projection, on the same scalars
             self.exposure.enqueue_adam(self)
+        if self.intrinsics is not None:   # the intrinsics corrections' reduction and Adam, on the same scalars
+            self.intrinsics.enqueue_adam(self)
         if self.dynamic_loss_scale:  # GradScaler.update(): adjusts the scale used by the NEXT step
             # a flag raised at the source is not reset by the next step, so this launch clears it
             raised_at_source = not check_finite and g16 is None
@@ -354,6 +385,9 @@ class NGPTrainer:
         self.check_aliasing()
         self.step_count += 1
         self.found_inf.zero_()
+        if self.intrinsics is not None:   # pixels of the batch's directions() that were not invertible
+            self.found_inf.copy_(self.intrinsics.flag)
+            self.intrinsics.flag.zero_()
         if self._pose_batch is not None:
             self.enqueue_pose_grad()
         self.enqueue_update()
@@ -361,8 +395,8 @@ class NGPTrainer:
             self.encoder.adopt_shadow(self._shadow)
 
     def step(self, rays_o, rays_d, rgb_gt, exp_step_factor=0.0, extra_loss=None, bg_rgb=None, alpha=None, b_load=1.0,
-             img_idxs=None, ray_w=None):
+             img_idxs=None, ray_w=None, pix_idxs=None):
         loss, results = self.forward_backward(rays_o, rays_d, rgb_gt, exp_step_factor, extra_loss, bg_rgb, alpha,
-                                              b_load, img_idxs, ray_w)
+                                              b_load, img_idxs, ray_w, pix_idxs)
         self.optimizer_step()
         return loss, results

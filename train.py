@@ -11,6 +11,10 @@ rebuilt beside every density-grid update; every per-ray loss term is weighted by
 results/error_map.npy holds the map at the end.
 With --exposure_lr every training image gets a learned per-channel exposure (DESIGN.md §6k) that scales its rays' sample
 colours; results/exposures.npy holds them (stops) at the end, and test views render at the mean exposure, e = 0.
+With --lens_distortion a COLMAP or ngp scene keeps its lens distortion and every pixel's direction is unprojected
+through it; with --intrinsics_lr the training camera's focal length and principal point are refined with the model
+(DESIGN.md §6l): the training rays come from the rays' pixels under the corrected intrinsics, test views render through
+the refined camera, and results/intrinsics_refined.json holds it at the end.
 The step body runs on the sm_90a kernels through NGPTrainer (fused Adam,
 no host sync for the inf check); under torchrun every rank trains on its own rays and the gradients are summed
 once per step: by the peer-memory optimizer kernel when all ranks share one NVLink box, else by an fp16 NCCL
@@ -77,6 +81,8 @@ def main(prefix_args=None):
         raise ValueError("--ray_sampling_strategy error_map trains on one GPU: the error map is not shared between ranks")
     if world > 1 and hparams.extrinsics_lr > 0:
         raise ValueError("--extrinsics_lr trains on one GPU: the pose gradient is not exchanged between ranks")
+    if world > 1 and hparams.intrinsics_lr > 0:
+        raise ValueError("--intrinsics_lr trains on one GPU: the intrinsics gradient is not exchanged between ranks")
     if world > 1 and hparams.exposure_lr > 0:
         raise ValueError("--exposure_lr trains on one GPU: the exposure gradient is not exchanged between ranks")
     if world > 1:
@@ -93,9 +99,11 @@ def main(prefix_args=None):
 
     dataset = dataset_dict[hparams.dataset_name]
     if hparams.dataset_name in DISK_DATASETS:   # the reference's arguments only (train.py:61-73)
+        extra = {'lens_distortion': True} if hparams.lens_distortion else {}
         train_dataset = dataset(root_dir=hparams.root_dir, split=hparams.split,
-                                downsample=hparams.downsample).to(device)
-        test_dataset = dataset(root_dir=hparams.root_dir, split='test', downsample=hparams.downsample).to(device)
+                                downsample=hparams.downsample, **extra).to(device)
+        test_dataset = dataset(root_dir=hparams.root_dir, split='test', downsample=hparams.downsample,
+                               **extra).to(device)
     else:
         extra = {'scene': 'analytic'} if hparams.dataset_name == 'synthetic' else {}
         if hparams.depth_loss_w > 0:
@@ -118,7 +126,11 @@ def main(prefix_args=None):
     if hparams.ckpt_path:
         model.load_state_dict(torch.load(hparams.ckpt_path, map_location=device))
         print("Load checkpoint from %s" % hparams.ckpt_path)
-    model.mark_invisible_cells(train_dataset.K, train_dataset.poses, train_dataset.img_wh)
+    camera = getattr(train_dataset, 'camera', None)   # set by --lens_distortion (DESIGN.md §6l)
+    if camera is not None:
+        model.mark_invisible_cells(train_dataset.K, train_dataset.poses, train_dataset.img_wh, camera=camera)
+    else:
+        model.mark_invisible_cells(train_dataset.K, train_dataset.poses, train_dataset.img_wh)
 
     torch.manual_seed(seed + rank)  # data / marching noise differ per rank from here on
     voxel_reg = None
@@ -128,12 +140,20 @@ def main(prefix_args=None):
     if hparams.extrinsics_lr > 0:   # per-image pose corrections (DESIGN.md §6i)
         from taichi_nerfs_b200.extrinsics import PoseRefinement
         extrinsics = PoseRefinement(train_dataset.poses, hparams.extrinsics_lr / hparams.lr)
+    intrinsics = None
+    if hparams.intrinsics_lr > 0:   # the training camera's focal length and principal point (DESIGN.md §6l)
+        from taichi_nerfs_b200.intrinsics import Camera, IntrinsicsRefinement
+        if camera is None:
+            K = train_dataset.K.double().cpu()
+            camera = Camera('PINHOLE', float(K[0, 0]), float(K[1, 1]), float(K[0, 2]), float(K[1, 2]))
+        intrinsics = IntrinsicsRefinement(camera, *train_dataset.img_wh, hparams.intrinsics_lr / hparams.lr,
+                                          train_dataset.poses)
     exposure = None
     if hparams.exposure_lr > 0:   # per-image exposures (DESIGN.md §6k)
         from taichi_nerfs_b200.exposure import ExposureCorrection
         exposure = ExposureCorrection(len(train_dataset.poses), hparams.exposure_lr / hparams.lr, device)
     trainer = NGPTrainer(model, lr=hparams.lr, max_steps=hparams.max_steps, voxel_reg=voxel_reg,
-                         extrinsics=extrinsics, exposure=exposure)
+                         extrinsics=extrinsics, exposure=exposure, intrinsics=intrinsics)
 
     # --random_bg (DESIGN.md §6f): every training ray gets its own background colour, drawn on the device
     bg_load = getattr(train_dataset, 'bg_load', 1.0)
@@ -163,14 +183,20 @@ def main(prefix_args=None):
                 error_map.rebuild()
             em_img, em_pix, ray_w = error_map.draw(hparams.batch_size, step)
             data = train_dataset.gather(em_img, em_pix)
-        img_idxs = rays_o = rays_d = None
-        if extrinsics is not None or exposure is not None:   # same_image gives one index: the kernels broadcast it
-            img_idxs = torch.as_tensor(data['img_idxs'], device=device)
-        if extrinsics is not None:
-            if fast is None:         # the graph step forms the rays from the corrected poses itself
-                rays_o, rays_d = extrinsics.rays(data['direction'], img_idxs)
+        img_idxs = rays_o = rays_d = pix_idxs = None
+        if extrinsics is not None or exposure is not None or intrinsics is not None:
+            img_idxs = torch.as_tensor(data['img_idxs'], device=device)   # same_image: one index, broadcast
+        direction = data['direction']
+        if intrinsics is not None:
+            pix_idxs = torch.as_tensor(data['pix_idxs'], device=device)
+            if fast is None:         # the graph step unprojects the pixels itself
+                direction = intrinsics.directions(pix_idxs)
+        if fast is not None and (extrinsics is not None or intrinsics is not None):
+            pass                     # the graph step forms the rays itself
+        elif extrinsics is not None:
+            rays_o, rays_d = extrinsics.rays(direction, img_idxs)
         else:
-            rays_o, rays_d = get_rays(data['direction'], data['pose'])
+            rays_o, rays_d = get_rays(direction, data['pose'])
         depth = None
         if hparams.depth_loss_w > 0:
             depth = data.get('depth')
@@ -188,7 +214,10 @@ def main(prefix_args=None):
             em_args = {} if error_map is None else {'ray_w': ray_w, 'img_idxs': em_img, 'pix_idxs': em_pix}
             if exposure is not None and error_map is None:
                 em_args['img_idxs'] = img_idxs
-            if extrinsics is not None:   # the step forms the rays from the corrected poses itself
+            if intrinsics is not None:   # the step forms the rays from the pixels itself
+                loss = fast.step(None, None, data['rgb'], alpha=data.get('alpha') if hparams.random_bg else None,
+                                 depth=depth, **{**em_args, 'img_idxs': img_idxs, 'pix_idxs': pix_idxs})
+            elif extrinsics is not None:   # the step forms the rays from the corrected poses itself
                 loss = fast.step(None, None, data['rgb'], alpha=data.get('alpha') if hparams.random_bg else None,
                                  depth=depth, directions=data['direction'], **{'img_idxs': img_idxs, **em_args})
             else:
@@ -202,7 +231,7 @@ def main(prefix_args=None):
                 bg_rgb = ops.random_bg(seed + rank, trainer.step_count + 1, len(rays_o), device)
             loss, results = trainer.step(rays_o, rays_d, data['rgb'], exp_step_factor, extra_loss=extra_loss,
                                          bg_rgb=bg_rgb, alpha=data.get('alpha'), b_load=bg_load, img_idxs=img_idxs,
-                                         ray_w=ray_w)
+                                         ray_w=ray_w, pix_idxs=pix_idxs)
             if error_map is not None:   # the graph step accumulates inside its graph
                 error_map.accumulate(results['rgb'].float(), data['rgb'], em_img, em_pix, bg_rgb=bg_rgb,
                                      alpha=data.get('alpha') if bg_rgb is not None else None, b_load=bg_load)
@@ -230,6 +259,14 @@ def main(prefix_args=None):
         np.save(os.path.join(val_dir, 'exposures.npy'), e)
         print(f"exposure: mean |e| = {float(np.abs(e).mean()):.4f} stops | max |e| = {float(np.abs(e).max()):.4f} "
               f"stops -> {os.path.join(val_dir, 'exposures.npy')}")
+    if intrinsics is not None:
+        import json
+        fx, fy, cx, cy = intrinsics.refined()
+        c = intrinsics.camera
+        with open(os.path.join(val_dir, 'intrinsics_refined.json'), 'w') as f:
+            json.dump({**c.as_dict(), 'fx': fx, 'fy': fy, 'cx': cx, 'cy': cy}, f, indent=1)
+        print(f"intrinsics: focal x{fx / c.fx:.5f} | principal point ({cx - c.cx:+.3f}, {cy - c.cy:+.3f}) px -> "
+              f"{os.path.join(val_dir, 'intrinsics_refined.json')}")
     if extrinsics is not None:
         np.save(os.path.join(val_dir, 'poses_refined.npy'), extrinsics.refined_poses())
         rot_deg, trans = extrinsics.mean_correction()
@@ -240,11 +277,13 @@ def main(prefix_args=None):
     model.eval()
     w, h = test_dataset.img_wh
     psnrs, ssims, depth_maes = [], [], []
+    # the test views share the training camera: with intrinsics refinement they render through the refined one
+    test_dirs = test_dataset.directions if intrinsics is None else intrinsics.table()
     with torch.no_grad():
         for i in range(len(test_dataset)):
             td = test_dataset[i]
             with torch.autocast(device_type='cuda', dtype=torch.float16):
-                rays_o, rays_d = get_rays(test_dataset.directions, td['pose'])
+                rays_o, rays_d = get_rays(test_dirs, td['pose'])
                 results = render(model, rays_o, rays_d, test_time=True, exp_step_factor=exp_step_factor)
             if 'rgb' in td:
                 psnrs.append(float(psnr_of(F.mse_loss(results['rgb'].float(), td['rgb']))))
